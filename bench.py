@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the weight-only matmul hot path on B200.
+"""bench.py -- headline benchmark of the weight-only matmul hot path on H100 (sm_90a).
 
 Metric (BASELINE.json): decode tokens/s, Llama-2-7B Q4_0, batch 1, 1 GPU, with the fraction of the measured HBM roofline.
 A "step" = one decode token's worth of the hot path: every weight-only matmul of Llama-2-7B (32 x {QKV, o-proj,
@@ -7,7 +7,11 @@ gate/up+SiLU*mul, down} + lm_head = 6.607e9 Q4_0 weights = 3.716 GB of packed by
 the device exactly as ne_compute_forward_mul_mat_q_f32 does, all captured in one CUDA graph.  Synthetic data:
 W ~ N(0, 0.02^2) (torch.manual_seed(1234)), quantised to Q4_0 on the device by the library's own quantiser.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--fmt q4_0|int4g128]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--fmt q4_0|int4g128] [--dump-outputs DIR]
+
+--dump-outputs DIR: after the timed steps, the arrays the last timed step produced (QKV, o-proj, FFN intermediate, FFN output,
+logits of the last layer's nodes and lm_head) are written as DIR/<name>.npy in float32.  All inputs come from fixed seeds, so two
+builds run with the same arguments can be compared output for output.
 
 Keys beyond the base contract: roofline{} (dominant kernel = the streaming GEMV, timed live with CUDA events on the
 launching stream), cpu_baseline{} (the reference's own ggml Q4_0 x Q8_0 code, oracle/_ref, timed on this box's host cores
@@ -237,8 +241,8 @@ def run_tp(world, rank, hbm_peak, steps):
     x0 = torch.randn(1, E, device="cuda")
     logits = torch.zeros(1, V, device="cuda")
     res = {}
-    # the one-shot NVLink exchange (cudaIpc peer mappings, csrc/comm.cu) is measured where it has been validated on hardware
-    # (2 GPUs: tests/test_gpu_tp.py, profiles/r02_summary.md); NS_TP_ONESHOT=1 forces it at any world size
+    # the one-shot NVLink exchange (cudaIpc peer mappings, csrc/comm.cu) is measured at the world size tests/test_gpu_tp.py
+    # validates (2 GPUs); NS_TP_ONESHOT=1 forces it at any world size
     modes = ("nccl", "nvlink_oneshot") if (world == 2 or os.environ.get("NS_TP_ONESHOT")) else ("nccl",)
     for mode in modes:
         if mode == "nvlink_oneshot":
@@ -327,8 +331,8 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_kind = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_kind = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet 3350 GB/s (not reached)"
 
     # ---- synthetic weights, quantised + repacked on the device
     torch.manual_seed(1234 + rank)
@@ -463,6 +467,10 @@ def run_ours(args):
         sampler.start()
     ms_perop = timed(run_step, args.steps, args.warmup)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in (("qkv", qkv), ("o", o), ("ffn_tmp", tmp), ("ffn", ffn), ("logits", logits)):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.detach().float().cpu().numpy())
     # a leg of at least one second of back-to-back steps: sustained clocks / power rather than a 20 ms burst
     sus_steps = max(args.steps, int(1.05 / (ms_perop * 1e-3)))
     ms_sus = timed(run_step, sus_steps, 3)
@@ -476,7 +484,7 @@ def run_ours(args):
     gemv_gbs = alg_bytes / (ms_gemv * 1e-3) / 1e9
     step_gbs = alg_bytes / (ms_step * 1e-3) / 1e9
 
-    # ---- prefill: the same matmul nodes for a 2048-token prompt through the tcgen05 tensor-core GEMM (bf16 numerics)
+    # ---- prefill: the same matmul nodes for a 2048-token prompt through the wgmma tensor-core GEMM (bf16 numerics)
     prefill = None
     if rank == 0 and not args.skip_prefill:
         MP = args.prefill_tokens
@@ -507,11 +515,11 @@ def run_ours(args):
         ms_pf = timed(prefill_calls, psteps, 1, collective=False)  # rank 0 only: no collectives in here
         flops = 2.0 * MP * sum(w.n * w.k for lay in layers for w in lay.values())
         tf = flops / (ms_pf * 1e-3) / 1e12
-        tpeak = float(peaks.get("bf16_tflops_sustained", 1400.0))
+        tpeak = float(peaks.get("bf16_tflops_sustained", 989.0))
         prefill = {"tokens": MP, "tokens_per_s": MP / (ms_pf * 1e-3), "ms": ms_pf, "tflops": tf,
                    "roofline": {"bound": "tensor", "achieved": tf, "peak": tpeak, "unit": "TFLOP/s", "frac": tf / tpeak,
-                                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in peaks else "fallback 1400",
-                                "kernel": "gemm_w4_tc_kernel<256> (tcgen05.mma kind::f16, in-smem int4->bf16 dequant)"},
+                                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in peaks else "H100 SXM data sheet 989 (dense bf16, not reached)",
+                                "kernel": "gemm_w4_tc_kernel<128> (wgmma m64n128k16 bf16, in-smem int4->bf16 dequant)"},
                    "note": f"{7 * n_layers} GEMMs of the {n_layers} layers (lm_head excluded: only the last token needs logits), "
                            "fp32 activations converted to bf16 per GEMM, outputs fp32; includes silu*mul and conversion kernels"}
         del xp, ap_, qkvp, op_, tmpp, ffnp, wsp_t
@@ -575,7 +583,7 @@ def run_ours(args):
             t_ld = time.perf_counter() - t0
             long_ctx = {"prompt_tokens": 2048, "prompt_eval_ms": t_lp2 * 1e3, "first_prompt_eval_ms": t_lp * 1e3,
                         "prompt_tokens_per_s": 2048 / t_lp2, "decode_tokens_per_s_at_2048": 64 / t_ld, "decode_ms_per_token_at_2048": t_ld / 64 * 1e3,
-                        "note": "ns_llama_eval of a 2048-token prompt (tcgen05 GEMMs + mma.sync causal attention + everything else), then "
+                        "note": "ns_llama_eval of a 2048-token prompt (wgmma GEMMs + mma.sync causal attention + everything else), then "
                                 "64 greedy tokens at positions 2048..2111 (split-context decode attention); host wall clock"}
         engine = {"tokens_per_s": world * n_new / dt_gen, "long_context": long_ctx, "ms_per_token": dt_gen / n_new * 1e3, "new_tokens": n_new,
                   "prompt_tokens": n_prompt, "n_ctx": n_ctx, "prompt_eval_ms": t_prompt2 * 1e3, "first_prompt_eval_ms": t_prompt * 1e3,
@@ -592,7 +600,7 @@ def run_ours(args):
     # bandwidth-bound path; parity of every format is covered by the tests).  Rank 0 only.
     configs = []
     if rank == 0 and not args.skip_configs and n_layers == N_LAYER:
-        tpeak = float(peaks.get("bf16_tflops_sustained", 1400.0))
+        tpeak = float(peaks.get("bf16_tflops_sustained", 989.0))
 
         def build(shape_layer, lm_shape, **kw):
             lays = [{nm: ns.Weight.random(n, k, seed=17 + 131 * li + i, queue=queue, **kw) for i, (nm, n, k) in enumerate(shape_layer)}
@@ -787,12 +795,12 @@ def run_ours(args):
                                    f"({n_layers} layers x [QKV, o, gate/up+SiLU*mul, down] + lm_head), Q8_0 activation "
                                    f"quantisation fused into each GEMV, one CUDA graph per token (graph={use_graph})",
                        "weights": int(n_weights), "packed_bytes_per_step": int(alg_bytes),
-                       "l2_policy": "inputs (3.7 GB of weights per step) exceed the 126 MB L2; no flush needed",
+                       "l2_policy": "inputs (3.7 GB of weights per step) exceed the 50 MB L2; no flush needed",
                        "parallelism": "replicas" if world > 1 else "single"},
             "roofline": {"bound": "hbm", "achieved": step_gbs, "peak": hbm_peak, "unit": "GB/s", "frac": step_gbs / hbm_peak,
-                         # dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, parsed at run time from the
-                         # committed ncu launch list of this same command (profiles/r02_launches_bench.csv); null when that
-                         # file is absent or the workload differs (other formats / layer counts)
+                         # dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, parsed at run time from an
+                         # ncu launch list of this same command at profiles/r02_launches_bench.csv; null when that file is absent
+                         # (none is committed) or the workload differs (other formats / layer counts)
                          "traffic": traffic, "traffic_source": traffic_src,
                          "kernel": "gemv_ring_kernel<S8,M=1,sym,f16,NC=14> (one CTA per SM: 14 consumer + 2 producer warps, fused Q8_0 activation quantisation)",
                          "launches_per_step": launches_per_step, "avg_launch_us": ms_step * 1e3 / max(1, launches_per_step),
@@ -833,10 +841,9 @@ def main():
     ap.add_argument("--skip-cpu", action="store_true")
     ap.add_argument("--skip-configs", action="store_true", help="skip the BASELINE configs 2-4 legs")
     ap.add_argument("--skip-tp", action="store_true", help="N > 1: skip the Llama-2-70B tensor-parallel leg (config 5)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
-        if args.steps > 20:
-            args.steps = 20
         run_reference(args)
     else:
         run_ours(args)

@@ -1,5 +1,5 @@
 /*
- * ns_b200.h -- C ABI of libns_b200.so: the B200-native (sm_100a) replacement for neural-speed's low-bit
+ * ns_b200.h -- C ABI of libns_b200.so: the H100-native (sm_90a) replacement for neural-speed's low-bit
  * weight-only matmul path.  Plain pointers and sizes only; no torch / C++ types cross this boundary.
  *
  * Every entry point names the reference interface it replaces (paths relative to /root/reference).
@@ -197,7 +197,7 @@ NS_API int ns_weight_dequant_f32(const ns_weight* w, float* dst_dev, int ld, voi
 /* dst[m][n] (ldo) = act[m][k] (lda) . W^T ; act/dst device fp32.  flags: NS_MM_* ; bias/residual may be NULL. */
 #define NS_MM_BIAS_BCAST 1   /* bias is [n] broadcast over m (else [m][ldo]) */
 #define NS_MM_FORCE_GEMV 2   /* always use the dp4a/FMA GEMV path (exact-integer numerics) regardless of m */
-#define NS_MM_FORCE_TC 4     /* always use the tcgen05 tensor-core path (bf16 numerics) */
+#define NS_MM_FORCE_TC 4     /* always use the wgmma tensor-core path (bf16 numerics) */
 NS_API int ns_mul_mat(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* bias,
                       const float* residual, int flags, void* workspace, void* queue);
 /* three weights sharing one activation (ne_mul_qkv): dst = [3][m][ldo], weights may differ in n */
@@ -320,7 +320,7 @@ NS_API int ns_llama_eval(ns_llama* ctx, const int32_t* tokens, int n_tokens, int
 /* greedy generation of n_new tokens starting with first_token at position n_past; out_tokens[i] = pick after step i */
 NS_API int ns_llama_generate(ns_llama* ctx, int32_t first_token, int n_past, int n_new, int32_t* out_tokens);
 /* Numerics of prompt evaluation.  Matmuls of up to 32 new tokens reproduce the reference's exact integer block sums (GEMV /
- * integer tensor cores); longer prompts run the bf16 tcgen05 GEMM (measured logit deviation <= 4e-2 of max|logit| on the toy
+ * integer tensor cores); longer prompts run the bf16 wgmma GEMM (measured logit deviation <= 4e-2 of max|logit| on the toy
  * models of tests/test_gpu_llama.py, KV cache entries differ at bf16 precision).  on = 1 evaluates long prompts in pieces of 32
  * tokens instead: reference numerics for the whole prompt at about 1/6 of the prefill throughput. */
 NS_API int ns_llama_set_exact_prefill(ns_llama* ctx, int on);

@@ -1,4 +1,4 @@
-"""neural_speed_b200 -- B200-native (sm_100a) low-bit weight-only matmul behind neural-speed's kernel ABI.
+"""neural_speed_b200 -- H100-native (sm_90a) low-bit weight-only matmul behind neural-speed's kernel ABI.
 
 Python is plumbing only: this module loads ``libns_b200.so`` (hand-written CUDA + C-ABI, see include/ns_b200.h) with
 ctypes and mirrors the reference's host-side interfaces for the hot path:
@@ -7,7 +7,7 @@ ctypes and mirrors the reference's host-side interfaces for the hot path:
 * ``np_bestla_qpack`` / ``np_bestla_quantize``  (neural_speed/application/main_pybind.cpp:378-437)
 * device-resident weights + matmuls used by the decode engine.
 
-There is no CPU compute fallback: every compute call needs the CUDA extension and a B200.
+There is no CPU compute fallback: every compute call needs the CUDA extension and an H100.
 """
 from __future__ import annotations
 
@@ -72,7 +72,7 @@ def lib() -> C.CDLL:
     if _lib is not None:
         return _lib
     if not os.path.exists(_LIB_PATH):
-        raise RuntimeError(f"{_LIB_PATH} missing: run `python -m neural_speed_b200.build` (nvcc, sm_100a)")
+        raise RuntimeError(f"{_LIB_PATH} missing: run `python -m neural_speed_b200.build` (nvcc, sm_90a)")
     L = C.CDLL(_LIB_PATH)
     vp, i, sz, f32p = C.c_void_p, C.c_int, C.c_size_t, C.c_void_p
     L.ns_last_error.restype = C.c_char_p

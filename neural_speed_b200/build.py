@@ -1,6 +1,6 @@
-"""Build libns_b200.so (hand-written sm_100a CUDA + the C-ABI) in-tree with nvcc.
+"""Build libns_b200.so (hand-written sm_90a CUDA + the C-ABI) in-tree with nvcc.
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.  Cross-compiles without a GPU.
+The .so and the objects are git-ignored build products.  Cross-compiles without a GPU.
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-Xcompiler", "-fPIC,-fvisibility=hidden,-fopenmp,-Wall,-Wno-unused-function",
     "-Xptxas", "-v",
 ]

@@ -30,7 +30,7 @@ def unpack_gptq(qweight, scales, qzeros, bits: int = 4, sym: bool = False):
     """-> (int_weight [K,N], scales [K/g,N] f32, zeros [K/g,N]) exactly as unpack_gptq_weight_{4,8}bits return them:
     4 bit: weight in 0..15, zeros = nibble + 1 (int8);  8 bit: already recentred to int8 (common.py:341-393)."""
     if bits not in (4, 8):
-        raise ValueError(f"unsupported bits {bits} (int3 layouts are not on the B200 path)")
+        raise ValueError(f"unsupported bits {bits} (int3 layouts are not on the GPU path)")
     per = 32 // bits
     mask = (1 << bits) - 1
     qw, qz = _as_u32(qweight), _as_u32(qzeros)

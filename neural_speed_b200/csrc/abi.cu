@@ -39,7 +39,7 @@ bool ns_cuda_ok(cudaError_t e, const char* what) {
 void ns_count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
 
 extern "C" const char* ns_last_error(void) { return g_err; }
-extern "C" const char* ns_version(void) { return "ns_b200 0.1 (sm_100a)"; }
+extern "C" const char* ns_version(void) { return "ns_b200 0.1 (sm_90a)"; }
 extern "C" unsigned long long ns_launch_count(void) { return g_launches.load(); }
 
 struct ns_device {
@@ -73,8 +73,8 @@ int ns_ensure_device() {
   int dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess || prop.major != 10) {
-    ns_set_error("device %d is sm_%d%d; this library carries sm_100a code only", dev, prop.major, prop.minor);
+  if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess || prop.major != 9 || prop.minor != 0) {
+    ns_set_error("device %d is sm_%d%d; this library carries sm_90a code only", dev, prop.major, prop.minor);
     g_dev_state = -1;
     return NS_E_NODEVICE;
   }
@@ -94,7 +94,7 @@ int ns_num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -611,8 +611,8 @@ static void* pick_ws(void* workspace, cudaStream_t st, size_t bytes) { return wo
 static bool use_tc(const ns_weight* w, int m, int flags) {
   if (flags & NS_MM_FORCE_GEMV) return false;
   if (!ns_gemm_tc_supported(w)) return false;
-  // Measured on 4096x4096 Q4_0 (profiles/r01_summary.md): the tensor-core GEMM costs ~30 us at small M (pipeline fill, split-K
-  // epilogue) while a 4-row GEMV tile costs ~7 us and keeps the exact-integer numerics: GEMV tiles win up to 16 rows.
+  // The tensor-core GEMM has a fixed cost at small M (pipeline fill, split-K epilogue) while GEMV tiles keep the exact-integer
+  // numerics: GEMV tiles up to 16 rows.  The threshold also fixes the numerics class of a call (DESIGN.md section 4).
   return m > 16 || (flags & NS_MM_FORCE_TC);
 }
 // 5..32 rows of an int4 weight with an integer compute type: integer tensor cores, exact block sums, weights read once
@@ -661,7 +661,7 @@ static int mul_mat_impl(const ns_weight* w, const float* act, int lda, float* ds
   void* ws = pick_ws(workspace, st, ws_need(w, m, tc));
   if (!ws) return NS_E_CUDA;
   if (tc) {
-    // M > 16: tcgen05 tensor-core GEMM, bf16 numerics (the reference switches from its GEMV to the blocked GEMM at M > 4)
+    // M > 16: wgmma tensor-core GEMM, bf16 numerics (the reference switches from its GEMV to the blocked GEMM at M > 4)
     if (int rc = ns_launch_act_bf16(w, act, lda, m, ws, st)) return rc;
     return ns_launch_gemm_tc(w, ws, dst, ldo, m, bias, bcast, residual, st);
   }

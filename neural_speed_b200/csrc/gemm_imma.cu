@@ -5,13 +5,13 @@
 // per K-block (kernel_ref.h:1825 / :1886; quantize_row_q8_0 for ggml weights), exact integer dot per K-block, then
 // fp32 accumulation of  isum * a_scale * w_scale  -- the same arithmetic as the M <= 4 GEMV (gemv_ring.cu), so a batch of 8 or
 // 32 sequences gets bit-for-bit the block sums a single sequence gets, and the weights are read from HBM ONCE per step
-// (the GEMV tiles re-read them every 4 rows; the bf16 tcgen05 GEMM changes the numerics and costs ~30 us per node at tiny M).
+// (the GEMV tiles re-read them every 4 rows; the bf16 wgmma GEMM changes the numerics).
 //
-// sm_100a facts this is built on (profiles/ubench.cu, T3 what=6): mma.sync m16n8k32 u8 x s8 is native (SASS IMMA.16832.U8.S8),
-// 8.6 cycles per warp-instruction per SM sub-partition = 1.07 Pop/s per GPU -- 7x the dp4a rate; int4 operands are emulated.
+// Built on mma.sync m16n8k32 u8 x s8 (native on sm_90a: SASS IMMA.16832.U8.S8); wgmma's integer form (s8 / u8 only) would need
+// the per-32 / per-128-block rescaling out of its accumulator registers every block, which mma.sync fragments give directly.
 //
 // Tiling.  CTA = 128 weight rows (8 consumer warps x 16 rows = the MMA's M) x all MT tokens (MMA N = 8 per instruction) x a
-// K range (split-K fills the 148 SMs when N/128 is small).  One producer warp feeds a shared-memory ring, a stage = 256 k:
+// K range (split-K fills the SMs when N/128 is small).  One producer warp feeds a shared-memory ring, a stage = 256 k:
 //   * the nibbles of 128 rows x 128 bytes as ONE 2-D TMA box with the 128-byte swizzle (cp.async.bulk.tensor, SASS UTMALDG), so
 //     ldmatrix over 8 rows is bank-conflict free;
 //   * the activations of the stage -- [8 chunks][MT tokens][32 B codes] + [8][MT] {scale, sum|zero point} -- as one 1-D bulk

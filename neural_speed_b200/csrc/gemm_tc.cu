@@ -1,25 +1,26 @@
-// gemm_tc.cu -- prefill / batched weight-only matmul on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), M > 4 rows.
+// gemm_tc.cu -- prefill / batched weight-only matmul on the Hopper tensor cores (wgmma + TMA + mbarrier), M > 4 rows.
 //
 // Replaces the reference's blocked GEMM for int4 weights: LauncherBase::run_block / LauncherIntKBlock::run_block
 // (bestla/bestla/bestla_wrapper.h:501,768) with WeightKBlockNInteger::getWeight + decompress_kblock_s4_fp
 // (bestla_prologue_b.h:642-733, kernel_ref.h:1113) feeding the JIT AMX/AVX512 micro-kernels (bestla_gemm.h), and the
 // ggml Q4_0 mul_mat for prompt batches (core/ne_layers.c:7085).  Numerics: weights are dequantised to bf16
-// ((u - 8 - zp) exactly in bf16, times the bf16-rounded scale), activations rounded to bf16, fp32 accumulation in TMEM --
+// ((u - 8 - zp) exactly in bf16, times the bf16-rounded scale), activations rounded to bf16, fp32 accumulation in registers --
 // the reference's own CompBf16 numerics (BF16 tolerance 2e-2 at K=4096, bestla_ut.h:80-94); logits stay within the
 // north-star's 1e-2 relative bar of the CPU path (tests/test_gpu_gemm_tc.py).
 //
-// Orientation ("swap-AB"): the WEIGHT tile is the UMMA M operand (128 output channels = 128 TMEM lanes) and the token tile
-// is the UMMA N operand (T = 32..256 columns), so small batches do not waste the 128-row MMA and the epilogue's stores
-// are coalesced along n.  Per CTA and per 64-wide k block:
-//   warp 0   TMA producer: packed nibbles [128 rows][32 B] (cp.async.bulk.tensor 2-D over the NSB rows, row pitch = pitch)
-//            and bf16 activations [T][64] (128B-swizzled) into two mbarrier rings
+// Orientation ("swap-AB"): the WEIGHT tile is the wgmma M operand (128 output channels = two warpgroups x 64 rows) and the
+// token tile is the wgmma N operand (T = 32..128 columns), so small batches do not waste the 64-row MMA.  Per CTA and per
+// 64-wide k block:
+//   warp 12     TMA producer: packed nibbles [128 rows][32 B] (cp.async.bulk.tensor 2-D over the NSB rows, row pitch = pitch)
+//               and bf16 activations [T][64] (128B-swizzled) into two mbarrier rings
 //   warps 8-11  dequant: 1 thread = 1 weight row: 2 x LDS.128 of nibbles -> 64 bf16 via (w >> 4j) & 0x000F000F | 0x4300
-//            (bf16 128+u), HSUB2 (exact), HMUL2 by the group scale -> 8 x STS.128 into the 128B-swizzled K-major tile,
-//            fence.proxy.async, arrive
-//   warp 1   MMA issuer: 4 x tcgen05.mma.cta_group::1.kind::f16 (M=128, N=T, K=16) per k block, accumulator in TMEM,
-//            tcgen05.commit releases the smem slots
-//   warps 4-7   epilogue: tcgen05.ld 32x32b.x32 -> (+bias, +residual) -> fp32 global stores, coalesced over n
-//   warp 2   TMEM alloc / dealloc
+//               (bf16 128+u), HSUB2 (exact), HMUL2 by the group scale -> 8 x STS.128 into the 128B-swizzled K-major tile,
+//               fence.proxy.async, arrive
+//   warps 0-7   two consumer warpgroups: 4 x wgmma.mma_async m64nTk16 (bf16, fp32 accumulate) per k block on their 64 weight
+//               rows, one k block kept in flight (wgmma.wait_group 1) before the smem slots are released; then the epilogue
+//               (+bias, +residual) straight from the accumulator registers to fp32 global stores
+// T stops at 128: the m64n128 accumulator is 64 fp32 registers per thread, which with 416 threads leaves room for the rest
+// (65536 registers / 416 threads = 157); a 256-token tile would need 128 and spill.  Larger M takes more CTAs on grid.y.
 // Roofline: tensor (bf16, fp32 accumulate): flops = 2*M*N*K per launch.
 #include <cuda.h>
 
@@ -27,11 +28,11 @@
 
 namespace {
 
-constexpr int BLOCK_N = 128;  // weight rows per CTA (UMMA M)
+constexpr int BLOCK_N = 128;  // weight rows per CTA (two wgmma M = 64 halves)
 constexpr int BLOCK_K = 64;   // bf16 elements per k block (one 128-byte swizzle atom)
-constexpr int UMMA_K = 16;
-constexpr int PACKED_TILE = BLOCK_N * (BLOCK_K / 2);  // 4096: nibbles of one 128-row sub-tile and k block (x2 for int8 weights)
-constexpr int DEQ_TILE = BLOCK_N * BLOCK_K * 2;       // 16384: the same as bf16
+constexpr int WG_K = 16;      // k of one wgmma
+constexpr int DEQ_TILE = BLOCK_N * BLOCK_K * 2;  // 16384: one 128-row k block as bf16
+constexpr int kConsumerThreads = 256, kDequantThreads = 128, kThreads = kConsumerThreads + kDequantThreads + 32;
 
 struct GemmParams {
   const uint8_t* rows;
@@ -79,70 +80,89 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
       "l"(map), "r"(x), "r"(y), "r"(smem_u32(bar))
       : "memory");
 }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 inputs, fp32 accumulate (SASS: UTCHMMA)
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// K-major, 128B-swizzled tile: 8-row groups 1024 B apart (SBO), LBO unused (=1), version 1 (Blackwell), layout SWIZZLE_128B
+// K-major, 128B-swizzled tile: 8-row groups 1024 B apart (SBO), LBO unused (=1), layout SWIZZLE_128B (sm_90 encoding: 1 at bit 62)
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// c_format f32 (1<<4), a/b format bf16 (1<<7, 1<<10), both K-major, N>>3 at bit 17, M>>4 at bit 24
-__device__ __forceinline__ uint32_t make_idesc_bf16(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// D[64 x N] += A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory, bf16 inputs, fp32 accumulate (SASS: HGMMA)
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(1));
 }
 
-#define TMEM_LD_32X32B_X32(taddr, r)                                                                                        \
-  asm volatile(                                                                                                             \
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                                             \
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                              \
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"                              \
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),         \
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), \
-        "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),             \
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])                                        \
-      : "r"(taddr)                                                                                                          \
-      : "memory")
+template <int T>
+__device__ __forceinline__ void wgmma_k16(float (&d)[T / 2], uint64_t adesc, uint64_t bdesc) {
+  if constexpr (T == 32) wgmma_m64n32k16(d, adesc, bdesc);
+  else if constexpr (T == 64) wgmma_m64n64k16(d, adesc, bdesc);
+  else wgmma_m64n128k16(d, adesc, bdesc);
+}
 
-// NB = number of 128-row weight sub-tiles a CTA owns (each with its own TMEM accumulator).  The bf16 activation tile is the
-// expensive operand to re-read (2 B/element against 0.5 B for the weights): at T = 256, NB = 1 a CTA pulls 36 KB per 4.2 MFLOP
-// and the GEMM is bound by L2 -> SM bandwidth (measured 36 % of the tensor peak); NB = 2 halves the activation traffic per flop.
 // W8: int8 weights (64 packed bytes per row and k block instead of 32).
-template <int T, int NB, bool W8 = false>
+template <int T, bool W8 = false>
 struct Smem {
-  static constexpr int SP = NB == 2 ? (W8 ? 3 : 4) : 6;      // packed-weight stages
-  static constexpr int SD = NB == 2 ? 2 : 3;                 // dequantised-weight stages
-  static constexpr int SA = NB == 2 ? (T >= 256 ? 3 : 4) : ((T >= 256) ? 4 : 6);  // activation stages
+  static constexpr int SP = 6;                   // packed-weight stages
+  static constexpr int SD = 3;                   // dequantised-weight stages
+  static constexpr int SA = T >= 128 ? 4 : 6;    // activation stages
   static constexpr int ROW_BYTES = W8 ? BLOCK_K : BLOCK_K / 2;  // packed bytes per weight row and k block
-  static constexpr int PACKED_STAGE = NB * BLOCK_N * ROW_BYTES;
-  static constexpr int DEQ_STAGE = NB * DEQ_TILE;
-  static constexpr int kThreads = 256 + 128 * NB;
+  static constexpr int PACKED_STAGE = BLOCK_N * ROW_BYTES;
+  static constexpr int DEQ_STAGE = DEQ_TILE;
   static constexpr int ACT_STAGE = T * BLOCK_K * 2;
   static constexpr int off_deq = 0;
   static constexpr int off_act = off_deq + SD * DEQ_STAGE;
   static constexpr int off_packed = off_act + SA * ACT_STAGE;
   static constexpr int off_bar = off_packed + SP * PACKED_STAGE;
-  static constexpr int num_bars = 2 * SP + 2 * SA + 2 * SD + 1;
-  static constexpr int off_tmem_ptr = off_bar + num_bars * 8;
-  static constexpr int total = off_tmem_ptr + 16 + 1024;  // + slack for manual 1024-B alignment
+  static constexpr int num_bars = 2 * SP + 2 * SA + 2 * SD;
+  static constexpr int total = off_bar + num_bars * 8 + 1024;  // + slack for manual 1024-B alignment
 };
 
-template <int T, int NB, bool W8>
-__global__ void __launch_bounds__(256 + 128 * NB, 1)
+template <int T, bool W8>
+__global__ void __launch_bounds__(kThreads, 1)
     gemm_w4_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_a, const GemmParams P) {
-  using L = Smem<T, NB, W8>;
+  using L = Smem<T, W8>;
   constexpr int ROW_BYTES = L::ROW_BYTES;
   constexpr int SA = L::SA, SP = L::SP, SD = L::SD, PACKED_STAGE = L::PACKED_STAGE, DEQ_STAGE = L::DEQ_STAGE;
   extern __shared__ unsigned char smem_raw[];
@@ -157,13 +177,11 @@ __global__ void __launch_bounds__(256 + 128 * NB, 1)
   uint64_t* a_empty = a_full + SA;
   uint64_t* d_full = a_empty + SA;
   uint64_t* d_empty = d_full + SD;
-  uint64_t* tmem_full = d_empty + SD;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + L::off_tmem_ptr);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n0 = blockIdx.x * (BLOCK_N * NB);
+  const int n0 = blockIdx.x * BLOCK_N;
   const int t0 = blockIdx.y * T;
-  // split-K (small M: too few output tiles to fill 148 SMs): this CTA owns k blocks [kb0, kb0 + num_kb) and adds its partial
+  // split-K (small M: too few output tiles to fill the SMs): this CTA owns k blocks [kb0, kb0 + num_kb) and adds its partial
   // tile to dst with fp32 atomics (dst zeroed by the launcher; bias / residual applied by split 0)
   const int total_kb = (P.kpad + BLOCK_K - 1) / BLOCK_K;
   const int kb0 = blockIdx.z * P.kb_per_split;
@@ -175,34 +193,25 @@ __global__ void __launch_bounds__(256 + 128 * NB, 1)
   if (threadIdx.x == 0) {
     for (int i = 0; i < SP; ++i) {
       mbar_init(&p_full[i], 1);
-      mbar_init(&p_empty[i], 4 * NB);
+      mbar_init(&p_empty[i], kDequantThreads / 32);
     }
     for (int i = 0; i < SA; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
+      mbar_init(&a_empty[i], kConsumerThreads / 128);
     }
     for (int i = 0; i < SD; ++i) {
-      mbar_init(&d_full[i], 4 * NB);
-      mbar_init(&d_empty[i], 1);
+      mbar_init(&d_full[i], kDequantThreads / 32);
+      mbar_init(&d_empty[i], kConsumerThreads / 128);
     }
-    mbar_init(tmem_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == 12 && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"((uint32_t)(T * NB))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == 12) {
     // ============================ TMA producer ============================
     if (lane == 0) {
       // packed weights never depend on the previous kernel: prefetch the first ring before griddepcontrol.wait
@@ -226,39 +235,13 @@ __global__ void __launch_bounds__(256 + 128 * NB, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================ MMA issuer ============================
-    const uint32_t idesc = make_idesc_bf16(BLOCK_N, T);
-    for (int kb = 0; kb < num_kb; ++kb) {
-      const int sd = kb % SD, sa = kb % SA;
-      mbar_wait(&d_full[sd], (kb / SD) & 1);
-      mbar_wait(&a_full[sa], (kb / SA) & 1);
-      tcgen05_fence_after();
-      if (lane == 0) {
-        const uint32_t a_addr = smem_u32(deq + sd * DEQ_STAGE);
-        const uint32_t b_addr = smem_u32(act + sa * L::ACT_STAGE);
-        if (!(P.dbg & 2))
-#pragma unroll
-        for (int nb = 0; nb < NB; ++nb)
-#pragma unroll
-          for (int k4 = 0; k4 < BLOCK_K / UMMA_K; ++k4) {
-            umma_bf16(tmem_base + (uint32_t)(nb * T), make_desc_sw128(a_addr + nb * DEQ_TILE + k4 * UMMA_K * 2),
-                      make_desc_sw128(b_addr + k4 * UMMA_K * 2), idesc, (uint32_t)((kb | k4) != 0));
-          }
-        umma_commit(&d_empty[sd]);  // fires when the MMAs above have finished reading shared memory
-        umma_commit(&a_empty[sa]);
-        if (kb == num_kb - 1) umma_commit(tmem_full);
-      }
-      __syncwarp();
-    }
   } else if (warp >= 8) {
-    // ============================ dequant: one thread per weight row (128 * NB rows) ============================
-    const int r = threadIdx.x - 256;  // row inside the CTA's 128*NB rows; packed rows are 32 B apart, bf16 sub-tiles DEQ_TILE apart
+    // ============================ dequant: one thread per weight row (128 rows) ============================
+    const int r = threadIdx.x - kConsumerThreads;  // row inside the CTA's 128 rows; packed rows are ROW_BYTES apart
     int grow = n0 + r;
     if (grow >= P.n) grow = P.n - 1;  // rows past N are zero-filled by TMA; keep the scale loads in bounds
     const uint8_t* rowp = P.rows + (size_t)grow * P.pitch;
     const int swz = r & 7;
-    unsigned char* drow_base = nullptr;
     for (int kb = 0; kb < num_kb; ++kb) {
       const int sp = kb % SP, sd = kb % SD;
       // group scale / zero point of the two 32-element halves of this k block
@@ -288,7 +271,7 @@ __global__ void __launch_bounds__(256 + 128 * NB, 1)
       __syncwarp();
       if (lane == 0) mbar_arrive(&p_empty[sp]);  // packed bytes are in registers
       if (kb >= SD) mbar_wait(&d_empty[sd], ((kb / SD) - 1) & 1);
-      drow_base = deq + sd * DEQ_STAGE + (r >> 7) * DEQ_TILE + ((r & 127) >> 3) * 1024 + swz * 128;
+      unsigned char* drow_base = deq + sd * DEQ_STAGE + (r >> 3) * 1024 + swz * 128;
       if (!(P.dbg & 1))
 #pragma unroll
       for (int c = 0; c < 8; ++c) {  // 16-byte chunk c of the bf16 row = k 8c..8c+7
@@ -327,49 +310,61 @@ __global__ void __launch_bounds__(256 + 128 * NB, 1)
       __syncwarp();
       if (lane == 0) mbar_arrive(&d_full[sd]);
     }
-  }
-  // ============================ epilogue: TMEM -> registers -> global, ALL warps ============================
-  // A warp can read the TMEM lanes of quarter (warp % 4); the warps of a quarter split the accumulator columns.  With only
-  // four epilogue warps the 128 x 512 fp32 tile took 27 us of a 112 us GEMM (nothing else runs in the CTA by then).
-  {
-    __syncwarp();
-    const int q = warp & 3;
-    const int per_quarter = (int)(blockDim.x >> 7);  // warps per lane quarter: 3 (NB = 1) or 4 (NB = 2)
-    pdl_wait();  // dst / residual may still be in use by the preceding kernel
-    mbar_wait(tmem_full, 0);
-    tcgen05_fence_after();
-#pragma unroll 1
-    for (int cc = (warp >> 2) * 32; cc < ((P.dbg & 4) ? 0 : NB * T); cc += per_quarter * 32) {
-      const int nb = cc / T, c0 = cc % T;
-      const int nrow = n0 + nb * BLOCK_N + q * 32 + lane;
-      const bool nvalid = nrow < P.n;
-      const float bcast_bias = (P.bias && P.bias_bcast && nvalid) ? P.bias[nrow] : 0.f;
-      uint32_t v[32];
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)cc;
-      TMEM_LD_32X32B_X32(taddr, v);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  } else {
+    // ============================ consumers: warpgroup g owns weight rows [64g, 64g + 64) of the tile ============================
+    const int g = warp >> 2;
+    const bool leader = (threadIdx.x & 127) == 0;
+    float acc[T / 2];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int t = t0 + c0 + j;
-        if (nvalid && t < P.m) {
-          const size_t o = (size_t)t * P.ldo + nrow;
-          float x = __uint_as_float(v[j]);
-          if (blockIdx.z == 0) {
-            x += bcast_bias;
-            if (P.bias && !P.bias_bcast) x += P.bias[o];
-            if (P.residual) x += P.residual[o];
-          }
-          if (gridDim.z > 1) atomicAdd(P.dst + o, x);
-          else P.dst[o] = x;
-        }
+    for (int i = 0; i < T / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const int sd = kb % SD, sa = kb % SA;
+      mbar_wait(&d_full[sd], (kb / SD) & 1);
+      mbar_wait(&a_full[sa], (kb / SA) & 1);
+      const uint32_t a_addr = smem_u32(deq + sd * DEQ_STAGE) + g * (64 * BLOCK_K * 2);
+      const uint32_t b_addr = smem_u32(act + sa * L::ACT_STAGE);
+      if (!(P.dbg & 2)) {
+        wgmma_fence();
+#pragma unroll
+        for (int k4 = 0; k4 < BLOCK_K / WG_K; ++k4)
+          wgmma_k16<T>(acc, make_desc_sw128(a_addr + k4 * WG_K * 2), make_desc_sw128(b_addr + k4 * WG_K * 2));
+        wgmma_commit();
+      }
+      wgmma_wait<1>();  // the previous k block's MMAs have finished reading shared memory
+      if (kb > 0 && leader) {
+        mbar_arrive(&d_empty[(kb - 1) % SD]);
+        mbar_arrive(&a_empty[(kb - 1) % SA]);
       }
     }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(T * NB)) : "memory");
+    wgmma_wait<0>();
+    // ============================ epilogue: accumulator registers -> global ============================
+    // d[4j + 2h + e] holds weight row 64g + 16(warp & 3) + lane / 4 + 8h and token 8j + 2(lane & 3) + e
+    pdl_wait();  // dst / residual may still be in use by the preceding kernel
+    if (!(P.dbg & 4)) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int nrow = n0 + g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        if (nrow >= P.n) continue;
+        const float bcast_bias = (P.bias && P.bias_bcast) ? P.bias[nrow] : 0.f;
+#pragma unroll
+        for (int j = 0; j < T / 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int t = t0 + 8 * j + 2 * (lane & 3) + e;
+            if (t < P.m) {
+              const size_t o = (size_t)t * P.ldo + nrow;
+              float x = acc[4 * j + 2 * h + e];
+              if (blockIdx.z == 0) {
+                x += bcast_bias;
+                if (P.bias && !P.bias_bcast) x += P.bias[o];
+                if (P.residual) x += P.residual[o];
+              }
+              if (gridDim.z > 1) atomicAdd(P.dst + o, x);
+              else P.dst[o] = x;
+            }
+          }
+      }
+    }
   }
 }
 
@@ -422,23 +417,23 @@ EncodeTiledFn get_encode() {
   return fn;
 }
 
-template <int T, int NB, bool W8>
+template <int T, bool W8>
 int launch_t(const CUtensorMap& mw, const CUtensorMap& ma, const GemmParams& P, cudaStream_t st) {
-  using L = Smem<T, NB, W8>;
-  auto kern = gemm_w4_tc_kernel<T, NB, W8>;
+  using L = Smem<T, W8>;
+  auto kern = gemm_w4_tc_kernel<T, W8>;
   static bool attr_set = false;
   if (!attr_set) {
     NS_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::total));
     attr_set = true;
   }
-  dim3 grid((P.n + BLOCK_N * NB - 1) / (BLOCK_N * NB), (P.m + T - 1) / T);
+  dim3 grid((P.n + BLOCK_N - 1) / BLOCK_N, (P.m + T - 1) / T);
   GemmParams Q = P;
   const int total_kb = (P.kpad + BLOCK_K - 1) / BLOCK_K;
   int splits = 1;
   const int tiles = (int)(grid.x * grid.y);
   static const int env_splits = getenv("NS_TC_SPLITS") ? atoi(getenv("NS_TC_SPLITS")) : 0;  // tuning aid
-  if (tiles < 96 && P.residual != P.dst && P.bias != P.dst) {
-    splits = ns_num_sms() / tiles;  // floor: one CTA per SM is resident (TMEM + ~100-200 KB smem), a partial second wave doubles the time
+  if (3 * tiles < 2 * ns_num_sms() && P.residual != P.dst && P.bias != P.dst) {
+    splits = ns_num_sms() / tiles;  // floor: one CTA per SM is resident (416 threads, ~100-160 KB smem), a partial second wave doubles the time
     if (splits > total_kb / 8) splits = total_kb / 8;  // keep >= 8 k blocks (512 k) per slice
     if (splits > 16) splits = 16;
     if (splits < 1) splits = 1;
@@ -448,7 +443,7 @@ int launch_t(const CUtensorMap& mw, const CUtensorMap& ma, const GemmParams& P, 
   splits = (total_kb + Q.kb_per_split - 1) / Q.kb_per_split;
   grid.z = (unsigned)splits;
   if (splits > 1) NS_CUDA_TRY(cudaMemset2DAsync(P.dst, (size_t)P.ldo * 4, 0, (size_t)P.n * 4, (size_t)P.m, st));
-  NS_CUDA_TRY(ns_launch_pdl(kern, grid, dim3(L::kThreads), (size_t)L::total, st, mw, ma, Q));
+  NS_CUDA_TRY(ns_launch_pdl(kern, grid, dim3(kThreads), (size_t)L::total, st, mw, ma, Q));
   ns_count_launch();
   return NS_OK;
 }
@@ -580,16 +575,14 @@ int ns_launch_gemm_tc(const ns_weight* w, const void* ws, float* dst, int ldo, i
     return NS_E_CUDA;
   }
   const __nv_bfloat16* abf = (const __nv_bfloat16*)ws;
-  int T = m <= 32 ? 32 : (m <= 64 ? 64 : (m <= 128 ? 128 : 256));
-  static const int force_nb = getenv("NS_TC_NB") ? atoi(getenv("NS_TC_NB")) : 0;  // tuning aid
-  const int NBsel = force_nb ? force_nb : ((T >= 128 && w->n >= 2 * BLOCK_N) ? 2 : 1);
+  const int T = m <= 32 ? 32 : (m <= 64 ? 64 : 128);
   const bool w8 = w->wfmt == NS_W_S8;
   CUtensorMap mw, ma;
   {
     // packed nibbles: uint8 [n][q_bytes] with row pitch `pitch`; box = 32 bytes (64 k) x 128 rows, no swizzle
     cuuint64_t dims[2] = {(cuuint64_t)w->q_bytes, (cuuint64_t)w->n};
     cuuint64_t strides[1] = {(cuuint64_t)w->pitch};
-    cuuint32_t box[2] = {(cuuint32_t)(w8 ? BLOCK_K : BLOCK_K / 2), (cuuint32_t)(BLOCK_N * NBsel)};
+    cuuint32_t box[2] = {(cuuint32_t)(w8 ? BLOCK_K : BLOCK_K / 2), (cuuint32_t)BLOCK_N};
     cuuint32_t es[2] = {1, 1};
     CUresult r = enc(&mw, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, (void*)w->rows, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -633,19 +626,15 @@ int ns_launch_gemm_tc(const ns_weight* w, const void* ws, float* dst, int ldo, i
   static const int dbg = getenv("NS_TC_DEBUG") ? atoi(getenv("NS_TC_DEBUG")) : 0;
   P.dbg = dbg;
   if (w8) {
-    if (NBsel == 2) return T == 128 ? launch_t<128, 2, true>(mw, ma, P, st) : launch_t<256, 2, true>(mw, ma, P, st);
     switch (T) {
-      case 32: return launch_t<32, 1, true>(mw, ma, P, st);
-      case 64: return launch_t<64, 1, true>(mw, ma, P, st);
-      case 128: return launch_t<128, 1, true>(mw, ma, P, st);
-      default: return launch_t<256, 1, true>(mw, ma, P, st);
+      case 32: return launch_t<32, true>(mw, ma, P, st);
+      case 64: return launch_t<64, true>(mw, ma, P, st);
+      default: return launch_t<128, true>(mw, ma, P, st);
     }
   }
-  if (NBsel == 2) return T == 128 ? launch_t<128, 2, false>(mw, ma, P, st) : launch_t<256, 2, false>(mw, ma, P, st);
   switch (T) {
-    case 32: return launch_t<32, 1, false>(mw, ma, P, st);
-    case 64: return launch_t<64, 1, false>(mw, ma, P, st);
-    case 128: return launch_t<128, 1, false>(mw, ma, P, st);
-    default: return launch_t<256, 1, false>(mw, ma, P, st);
+    case 32: return launch_t<32, false>(mw, ma, P, st);
+    case 64: return launch_t<64, false>(mw, ma, P, st);
+    default: return launch_t<128, false>(mw, ma, P, st);
   }
 }

@@ -4,16 +4,14 @@
 // Replaces the same reference functions as gemv.cu (ne_vec_dot_q4_0_q8_0, core/layers/vec_dot.h:131; gemv_4bit_u8s8_fp32 /
 // gemv_4bit_s8s8_fp32, bestla/bestla/kernel_ref.h:2372/2432) for M <= 4.
 //
-// Why a ring: at 6.6 TB/s each of the 148 SMs must keep >= ~45-90 KB of loads in flight (Little's law, ~1-2 us loaded
-// HBM latency); register-staged loads cap that at occupancy x 128 B per thread.  Here one elected producer thread per CTA
+// Why a ring: at 3.35 TB/s each of the 132 SMs of an H100 must keep >= ~25-50 KB of loads in flight (Little's law, ~1-2 us
+// loaded HBM latency); register-staged loads cap that at occupancy x 128 B per thread.  Here one elected producer thread per CTA
 // issues cp.async.bulk (UBLKCP) copies of whole weight-row PAIRS -- a row of the NSB layout is one contiguous
 // [nibbles | scales | zero-points] byte range -- into a ring of slots guarded by full/empty mbarriers.  Each consumer warp
 // owns a whole stage at a time (two rows): no cross-warp reduction, rows dealt round-robin over CTAs (balanced at any N).
-// 7 consumer warps + 1 producer warp per CTA, 2 CTAs per SM (~105 KB ring each = 3 slots per consumer warp for K=4096;
-// measured r01: 8 warps x 2 slots 60.0 %, 7 x 3 66.3 %, 6 x 3 64.4 % of the HBM roofline in back-to-back launches).  The producer streams BEFORE
-// griddepcontrol.wait, so under programmatic dependent launch a CTA starts filling its ring the moment it becomes
-// resident.  (Measured alternatives: quarter-SM CTAs that let the next kernel co-reside were slower -- 8 consumer warps per SM
-// cannot keep up with HBM; one persistent cooperative kernel per token was slower too, profiles/r02_summary.md section 2.)
+// 7 consumer warps + 1 producer warp per CTA, 2 CTAs per SM (~105 KB ring each = 3 slots per consumer warp for K=4096).
+// The producer streams BEFORE griddepcontrol.wait, so under programmatic dependent launch a CTA starts filling its ring the
+// moment it becomes resident.
 // Roofline: HBM.  Algorithmic bytes per launch = sum over weights of N*K/2 + N*ceil(K/g)*(scale_bytes [+1 if asym]).
 #include "gemv_ring_impl.cuh"
 
@@ -26,8 +24,8 @@ int launch_one(const GemvParams& P, int mt, cudaStream_t st) {
   const int red_off = (int)ns_round_up(img_end, 16);  // one float per consumer warp (<= 14) of reduction scratch behind the image
   const size_t act_region = ns_round_up(P.norm_w ? (size_t)red_off + 64 : img_end, 128);
   // Single-row launches that quantise their activations themselves run on the one-CTA-per-SM kernel with 14 consumer warps
-  // (gemv_ring_wide.cu; measured: 947 -> 1000 tok/s on the matmul-only token, 776 -> 849 on the whole eval step; on PRE-quantised
-  // images the two-CTA kernel stays ahead, 66 % against 62 %).  NS_RING_WIDE=0 / 1 forces the choice.
+  // (gemv_ring_wide.cu: the activation row is read and quantised once per SM); pre-quantised images stay on the two-CTA kernel.
+  // NS_RING_WIDE=0 / 1 forces the choice.
   static const int env_wide = getenv("NS_RING_WIDE") ? atoi(getenv("NS_RING_WIDE")) : -1;
   if constexpr (M == 1) {
     if (env_wide == 1 || (env_wide < 0 && P.act_f32 != nullptr)) {

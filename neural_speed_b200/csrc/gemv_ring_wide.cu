@@ -2,8 +2,8 @@
 //
 // Same kernel template as gemv_ring.cu (gemv_ring_impl.cuh), NC = 14.  Every CTA of the ring GEMV pulls the whole fp32 activation row
 // (16-44 KB) through L2 and quantises it (fused NE_TASK_INIT: quantize_row_q8_0, vectors/cpu/quantize.h:447; quantize_fp_u8/s8_colblock,
-// bestla/bestla/kernel_ref.h:1825/1886) before its first dp4a.  148 CTAs do that in 0.8 us, 296 in 2.2 us (profiles/r02_ubench.log):
-// with one CTA per SM the row is read and quantised once per SM instead of twice.  Used for single-row launches that quantise their
+// bestla/bestla/kernel_ref.h:1825/1886) before its first dp4a; with one CTA per SM the row is read and quantised once per SM
+// instead of twice.  Used for single-row launches that quantise their
 // own activations (the decode path); pre-quantised images and 2..4-row launches stay on the two-CTA shape.
 #include "gemv_ring_impl.cuh"
 

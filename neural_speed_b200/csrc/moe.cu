@@ -4,7 +4,7 @@
 // row lists (matrix_rows[n_as][ne11]) on the host and then walk the tokens of every expert ONE AT A TIME (vec_dot per row,
 // or bestla_f32f32_forward with m = 1): each token re-reads its expert's weights.  Here the tokens are sorted by expert
 // once, the activation rows are gathered into that order, every expert runs ONE matmul over its contiguous slice (GEMV ring,
-// integer tensor cores or tcgen05 by slice height -- the expert's weights are read once per node), and the result rows are
+// integer tensor cores or wgmma by slice height -- the expert's weights are read once per node), and the result rows are
 // scattered back.  Both kernels are plain coalesced row copies: HBM-bound, 2 x m x cols x 4 bytes.
 #include "nsb.cuh"
 

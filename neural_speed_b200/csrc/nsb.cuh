@@ -1,6 +1,6 @@
-// nsb.cuh -- internal definitions shared by the CUDA sources of libns_b200.so (sm_100a only).
+// nsb.cuh -- internal definitions shared by the CUDA sources of libns_b200.so (sm_90a only).
 //
-// Device ("NSB") weight layout, chosen for B200 (see DESIGN.md "Data layout in HBM"):
+// Device ("NSB") weight layout (see DESIGN.md "Data layout in HBM"):
 //   N self-contained rows of `pitch` bytes (16-B multiple), row n at rows + n*pitch:
 //     [ q      : q_bytes = kpad/2 (4-bit) or kpad (8-bit), kpad = roundup(K, 32)           ]
 //     [ scales : ngroups x {f32|bf16|f16}, ngroups = ceil(K/group)  (at sc_off = q_bytes)  ]

@@ -35,7 +35,7 @@ def build(force: bool = False) -> None:
     """Compile liboracle.so and (when /root/reference exists) oracle/_ref/."""
     need = force or not os.path.exists(os.path.join(_HERE, "liboracle.so"))
     if os.path.isdir("/root/reference/neural_speed") and not all(
-            os.path.exists(os.path.join(_HERE, "_ref", f)) for f in ("libref_ggml.so", "libref_btla.so", "libref_ne.so", "libref_ne_ns.so")):
+            os.path.exists(os.path.join(_HERE, "_ref", f)) for f in ("libref_ggml.so", "libref_btla.so", "libref_ne.so")):
         need = True
     if need:
         subprocess.run(["make", "-C", _HERE, "-s"] + (["-B"] if force else []), check=True)
@@ -71,16 +71,10 @@ def ref_ne():
     return _ref_ne
 
 
-_ref_ne_ns = None
-
-
 def _bind_llama(L):
     L.ref_ne_mul_mat_id.restype = None
     L.ref_ne_mul_mat_id.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                     C.c_int, C.c_void_p, C.c_int]
-    L.ref_ne_ffn_id_silu.restype = None
-    L.ref_ne_ffn_id_silu.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
-                                     C.c_int, C.c_void_p, C.c_int]
     L.ref_ne_llama_create.restype = C.c_void_p
     L.ref_ne_llama_create.argtypes = [C.c_int] * 7 + [C.c_float] * 3
     L.ref_ne_llama_create_ex.restype = C.c_void_p
@@ -91,24 +85,6 @@ def _bind_llama(L):
     L.ref_ne_llama_free.restype = None
     L.ref_ne_llama_free.argtypes = [C.c_void_p]
 
-
-def ref_ne_ns():
-    """The reference's graph engine LINKED AGAINST libns_b200.so (oracle/_ref/libref_ne_ns.so: every bestla_* entry point of
-    ne_layers.c resolves to the CUDA drop-ins) or None.  Needs a CUDA device to compute anything."""
-    global _ref_ne_ns
-    if _ref_ne_ns is None:
-        p = os.path.join(_HERE, "_ref", "libref_ne_ns.so")
-        if not os.path.exists(p) and os.path.isdir("/root/reference/neural_speed"):
-            try:
-                subprocess.run(["make", "-C", _HERE, "-s", "_ref/libref_ne_ns.so"], check=True)
-            except Exception:
-                pass
-        if not os.path.exists(p):
-            return None
-        L = C.CDLL(p, mode=C.RTLD_GLOBAL)
-        _bind_llama(L)
-        _ref_ne_ns = L
-    return _ref_ne_ns
 
 
 def lib():
@@ -346,23 +322,13 @@ def _blob_table(blobs):
 
 
 def ref_mul_mat_id(L, experts, wtype, n, k, ids, id, b, n_threads=1):
-    """ne_mul_mat_id through the REFERENCE's engine L (ref_ne() on the CPU, ref_ne_ns() on the CUDA drop-ins).
+    """ne_mul_mat_id through the REFERENCE's engine L (ref_ne()): NE_TYPE_Q4_0 experts.
     experts: list of Q4_0 row arrays / BesTLA blobs; ids int32 [n_tok][n_used]; b fp32 [n_tok][k] -> [n_tok][n]."""
     keep, ptrs, sizes = _blob_table(experts)
     ids = np.ascontiguousarray(ids, np.int32)
     b = np.ascontiguousarray(b, np.float32)
     out = np.zeros((b.shape[0], n), np.float32)
     L.ref_ne_mul_mat_id(ptrs, sizes, wtype, len(keep), n, k, _p(ids), ids.shape[1], id, _p(b), b.shape[0], _p(out), n_threads)
-    return out
-
-
-def ref_ffn_id_silu(L, gate, down, up, k, fmid, n_out, ids, id, src, n_threads=1):
-    """ne_mul_id_ffn_silu (BesTLA blobs) through the reference's engine L."""
-    keep, ptrs, sizes = _blob_table(list(gate) + list(down) + list(up))
-    ids = np.ascontiguousarray(ids, np.int32)
-    src = np.ascontiguousarray(src, np.float32)
-    out = np.zeros((src.shape[0], n_out), np.float32)
-    L.ref_ne_ffn_id_silu(ptrs, sizes, len(gate), k, fmid, n_out, _p(ids), ids.shape[1], id, _p(src), src.shape[0], _p(out), n_threads)
     return out
 
 
@@ -523,23 +489,17 @@ class RefNeLlama:
     through ne_mul_mat's head broadcast).  Only available where oracle/_ref was built (needs /root/reference)."""
 
     NAMES = ["attn_norm", "wq", "wk", "wv", "wo", "ffn_norm", "w1", "w2", "w3"]
-    NE_TYPE_Q4_0, NE_TYPE_BTLA = 2, 19  # core/data_types.h:32-55
+    NE_TYPE_Q4_0 = 2  # core/data_types.h:32-55
 
-    def __init__(self, hp, tok_embd, out_norm, output_rows, layers, btla=False, fused=True, n_threads=1, on_ns=False):
-        """btla=True: the matmul weights are serialized BesTLA blobs (NE_TYPE_BTLA tensors), which only the engine linked against
-        libns_b200.so (on_ns=True) can execute; fused: ne_mul_qkv / ne_ffn_silu nodes where the *_support probes agree."""
-        L = ref_ne_ns() if on_ns else ref_ne()
+    def __init__(self, hp, tok_embd, out_norm, output_rows, layers, fused=True, n_threads=1):
+        """fused: ne_mul_qkv / ne_ffn_silu nodes where the *_support probes agree."""
+        L = ref_ne()
         if L is None:
-            raise RuntimeError("oracle/_ref/libref_ne%s.so not built" % ("_ns" if on_ns else ""))
+            raise RuntimeError("oracle/_ref/libref_ne.so not built")
         self.L, self.n_vocab = L, hp["n_vocab"]
-        sizes = None
-        if btla:
-            mats = [output_rows] + [lay[n] for lay in layers for n in ("wq", "wk", "wv", "wo", "w1", "w2", "w3")]
-            sizes = np.asarray([np.asarray(m).nbytes for m in mats], np.uint64)
         self.h = C.c_void_p(L.ref_ne_llama_create_ex(hp["n_vocab"], hp["n_embd"], hp["n_head"], hp["n_head_kv"], hp["n_layer"], hp["n_ff"],
                                                      hp["n_ctx"], hp.get("norm_eps", 1e-6), hp.get("rope_theta", 10000.0),
-                                                     hp.get("rope_scale", 1.0), self.NE_TYPE_BTLA if btla else self.NE_TYPE_Q4_0,
-                                                     _p(sizes) if btla else None, 1 if fused else 0, n_threads))
+                                                     hp.get("rope_scale", 1.0), self.NE_TYPE_Q4_0, None, 1 if fused else 0, n_threads))
 
         def put(layer, which, arr, dt):
             a = _c(arr, dt)

@@ -2,7 +2,6 @@
  * oracle/ref_ne_harness.h -- TEST INFRASTRUCTURE ONLY.  Graphs driven through the reference engine's PUBLIC API (ne_init /
  * ne_new_tensor_* / ne_mul_mat / ne_mul_qkv / ne_ffn_silu / ne_graph_compute ...).  Included after "core/ne_layers.c" by
  *   ref_ne.c     the engine with the BesTLA entry points stubbed (every node takes ne_layers.c's own ggml path): the oracle pin
- *   ref_ne_ns.c  the same engine linked against libns_b200.so: the reference's ne_graph_compute running on the CUDA drop-ins
  */
 /* ---- single ops through the public graph API ------------------------------------------------------------------------ */
 static struct ne_context* ref_ne_ctx(size_t bytes) {
@@ -248,35 +247,5 @@ REF_API void ref_ne_mul_mat_id(const void* const* experts, const size_t* expert_
   gf.n_threads = n_threads > 0 ? n_threads : 1;
   ne_graph_compute(ctx, &gf);
   memcpy(out, r->data, (size_t)n * n_tok * 4);
-  ne_free(ctx);
-}
-
-/* ne_mul_id_ffn_silu (ne_layers.c:2419; BesTLA blobs only -- the model code emits it when bestla_fusion_FFN_SiLu_f32f32_support
- * agrees, models/mixtral): gate/up [k x fmid], down [fmid x n_out]; src [k x n_tok]; out [n_out x n_tok].  blobs in the order
- * gate[0..n_as), down[0..n_as), up[0..n_as). */
-REF_API void ref_ne_ffn_id_silu(const void* const* blobs, const size_t* blob_bytes, int n_as, int k, int fmid, int n_out,
-                                const int32_t* ids, int n_used, int id, const float* src, int n_tok, float* out, int n_threads) {
-  size_t bytes = (size_t)n_tok * ((size_t)k + n_out + 2 * (size_t)fmid) * 8 + (size_t)n_tok * n_used * 4 + (64u << 20);
-  for (int e = 0; e < 3 * n_as; ++e) bytes += blob_bytes[e] + 4096;
-  struct ne_context* ctx = ref_ne_ctx(bytes);
-  struct ne_tensor *gate[8], *down[8], *up[8];
-  if (n_as > 8) { fprintf(stderr, "ref_ne_ffn_id_silu: n_as > 8\n"); abort(); }
-  for (int e = 0; e < n_as; ++e) {
-    gate[e] = ne_new_tensor_2d(ctx, NE_TYPE_BTLA, k, fmid, blob_bytes[e], NE_BACKEND_CPU);
-    down[e] = ne_new_tensor_2d(ctx, NE_TYPE_BTLA, fmid, n_out, blob_bytes[n_as + e], NE_BACKEND_CPU);
-    up[e] = ne_new_tensor_2d(ctx, NE_TYPE_BTLA, k, fmid, blob_bytes[2 * n_as + e], NE_BACKEND_CPU);
-    memcpy(gate[e]->data, blobs[e], blob_bytes[e]);
-    memcpy(down[e]->data, blobs[n_as + e], blob_bytes[n_as + e]);
-    memcpy(up[e]->data, blobs[2 * n_as + e], blob_bytes[2 * n_as + e]);
-  }
-  struct ne_tensor* I = ne_new_tensor_2d(ctx, NE_TYPE_I32, n_used, n_tok, NE_SIZE_CALC, NE_BACKEND_CPU);
-  memcpy(I->data, ids, (size_t)n_used * n_tok * 4);
-  struct ne_tensor* S = ne_new_tensor_2d(ctx, NE_TYPE_F32, k, n_tok, NE_SIZE_CALC, NE_BACKEND_CPU);
-  memcpy(S->data, src, (size_t)k * n_tok * 4);
-  struct ne_tensor* r = ne_mul_id_ffn_silu(ctx, down, gate, up, n_as, I, id, S);
-  struct ne_cgraph gf = ne_build_forward(r);
-  gf.n_threads = n_threads > 0 ? n_threads : 1;
-  ne_graph_compute(ctx, &gf);
-  memcpy(out, r->data, (size_t)n_out * n_tok * 4);
   ne_free(ctx);
 }

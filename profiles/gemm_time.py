@@ -1,4 +1,4 @@
-"""Time single tcgen05 GEMMs (CUDA events) -- tuning aid.  usage: python profiles/gemm_time.py [M]"""
+"""Time single wgmma GEMMs (CUDA events) -- tuning aid.  usage: python profiles/gemm_time.py [M]"""
 import ctypes as C
 import sys
 

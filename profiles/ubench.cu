@@ -1,5 +1,5 @@
 // ubench.cu -- micro-measurements that size the persistent decode kernel (round 2): grid-barrier latency, broadcast L2 reads,
-// issue rates of the dp4a/lop3 mix.  Standalone: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o profiles/ubench.bin profiles/ubench.cu
+// issue rates of the dp4a/lop3 mix.  Standalone: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o profiles/ubench.bin profiles/ubench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -146,7 +146,7 @@ __global__ void pipe_kernel(int iters, unsigned* sink, unsigned long long* out) 
         asm volatile("fma.rn.f32 %0, %1, %2, %0;" : "+f"(f2) : "f"(f0), "f"(f3));
         asm volatile("fma.rn.f32 %0, %1, %2, %0;" : "+f"(f3) : "f"(f1), "f"(f0));
       } else if (WHAT == 6) {
-        // integer tensor-core MMA as sm_100a still offers it to mma.sync: m16n8k32 u8 x s8 -> s32, four independent accumulators
+        // integer tensor-core MMA through mma.sync: m16n8k32 u8 x s8 -> s32, four independent accumulators
         asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                      : "+r"(c0), "+r"(c1), "+r"(c2), "+r"(c3) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
         asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 tensor-core GEMM (M > 4) against the oracle.
+"""GPU parity of the wgmma tensor-core GEMM (M > 4) against the oracle.
 
 The kernel's arithmetic is bf16 x bf16 -> fp32: w_eff = bf16((q - zp) * bf16(scale)), a_eff = bf16(a).  Checks:
  (1) against an fp64-accumulated GEMM on exactly those operands: rtol 2e-3 (fp32 accumulation order only);

@@ -94,7 +94,7 @@ def test_small_prompt_eval_then_decode():
 
 @pytest.mark.parametrize("n_head", [4, 2])
 def test_long_prompt_goes_through_the_tensor_core_gemm(n_head):
-    """M > 16 rows take the bf16 tcgen05 GEMM: same graph, bf16 matmul numerics (looser bar), KV cache usable afterwards"""
+    """M > 16 rows take the bf16 wgmma GEMM: same graph, bf16 matmul numerics (looser bar), KV cache usable afterwards"""
     hp, orc, eng = _build(n_head, seed=6, n_head=n_head)
     prompt = list(np.random.default_rng(1).integers(3, hp["n_vocab"], 24))
     _check_logits(eng.eval(prompt, 0)[0], orc.eval(prompt, 0), tol=4e-2)

@@ -1,5 +1,5 @@
 """Two-GPU tensor-parallel layer: shards from ns_split_weight, matmuls in libns_b200, NCCL sum all-reduce after o-proj and
-down-proj (llama.cpp:592,693).  Needs 2 GPUs (run with `gpurun --gpus 2`); skipped on a single-GPU box."""
+down-proj (llama.cpp:592,693).  Needs 2 GPUs; skipped on a single-GPU machine."""
 import os
 import socket
 

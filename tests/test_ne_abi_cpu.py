@@ -1,7 +1,9 @@
 """include/ns_ne_abi.h restates struct ne_tensor / ne_compute_params and a few enum values of the reference's graph engine (the
-structs bestla_support / bestla_parallel_for receive).  Where /root/reference is present, compile both headers into one C file and
-let the compiler compare every offset, size and enum value; elsewhere check the committed numbers (taken from that compile)."""
+structs bestla_support / bestla_parallel_for receive).  Every offset, size and enum value of our header is compared with the
+reference header's: compiled from the reference sources where they are present, otherwise as stored from such a compile
+(tests/golden/ne_abi_reference.json)."""
 import ctypes as C
+import json
 import os
 import subprocess
 import tempfile
@@ -26,24 +28,33 @@ ENUMS = {"NE_TYPE_F32": "NS_NE_TYPE_F32", "NE_TYPE_F16": "NS_NE_TYPE_F16", "NE_T
          "NE_MAX_OP_PARAMS": "NS_NE_MAX_OP_PARAMS"}
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference headers not present on this box")
-def test_layout_matches_the_reference_header():
-    lines = ['#include <stddef.h>', '#include "core/ne.h"', '#include "ns_ne_abi.h"']
-    for f in FIELDS:
-        lines.append(f'_Static_assert(offsetof(struct ne_tensor, {f}) == offsetof(struct ns_ne_tensor, {f}), "ne_tensor.{f}");')
-    for f in PFIELDS:
-        lines.append(f'_Static_assert(offsetof(struct ne_compute_params, {f}) == offsetof(struct ns_ne_compute_params, {f}), "params.{f}");')
-    lines.append('_Static_assert(sizeof(struct ne_tensor) == sizeof(struct ns_ne_tensor), "sizeof ne_tensor");')
-    lines.append('_Static_assert(sizeof(struct ne_compute_params) == sizeof(struct ns_ne_compute_params), "sizeof params");')
-    for a, b in ENUMS.items():
-        lines.append(f'_Static_assert((int){a} == (int){b}, "{a}");')
-    lines.append("int main(void) { return 0; }")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "ne_abi_reference.json")
+
+
+def _layout(include, flags, tensor, params, enums):
+    """offsets of FIELDS / PFIELDS, both sizeofs and the enum values, as compiled by gcc for this host"""
+    items = [f"offsetof(struct {tensor}, {f})" for f in FIELDS] + [f"offsetof(struct {params}, {f})" for f in PFIELDS]
+    items += [f"sizeof(struct {tensor})", f"sizeof(struct {params})"] + [f"(size_t){e}" for e in enums]
+    keys = [f"ne_tensor.{f}" for f in FIELDS] + [f"params.{f}" for f in PFIELDS] + ["sizeof ne_tensor", "sizeof params"] + list(ENUMS)
+    body = "".join(f'printf("%zu\\n", (size_t)({x}));' for x in items)
     with tempfile.TemporaryDirectory() as d:
-        src = os.path.join(d, "chk.c")
-        open(src, "w").write("\n".join(lines))
-        r = subprocess.run(["gcc", "-std=c11", "-fsyntax-only", f"-I{REF}", f"-I{REF}/core", f"-I{ROOT}/include", src], capture_output=True,
-                           text=True)
-        assert r.returncode == 0, r.stderr
+        src, exe = os.path.join(d, "layout.c"), os.path.join(d, "layout")
+        open(src, "w").write(f'#include <stdio.h>\n#include <stddef.h>\n#include "{include}"\nint main(void){{{body}return 0;}}\n')
+        subprocess.run(["gcc", "-std=c11", *flags, src, "-o", exe], check=True)
+        out = subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split()
+    return dict(zip(keys, (int(v) for v in out)))
+
+
+def test_layout_matches_the_reference_header():
+    ours = _layout("ns_ne_abi.h", [f"-I{ROOT}/include"], "ns_ne_tensor", "ns_ne_compute_params", list(ENUMS.values()))
+    if os.path.isdir(REF):
+        want = _layout("core/ne.h", [f"-I{REF}", f"-I{REF}/core"], "ne_tensor", "ne_compute_params", list(ENUMS))
+        if os.environ.get("NS_RECORD_GOLDEN"):
+            with open(GOLDEN, "w") as f:
+                json.dump(want, f, indent=0)
+    else:
+        want = json.load(open(GOLDEN))
+    assert ours == want
 
 
 def test_committed_layout_numbers():
