@@ -597,36 +597,105 @@ extern "C" int ns_weight_dequant_f32(const ns_weight* w, float* dst_dev, int ld,
 }
 
 // ---------------------------------------------------------------------------------------------------- device matmuls
+// Every matmul node runs on one of four kernel paths, and the path fixes the node's numerics class (DESIGN.md section 4):
+//   NS_PATH_GEMV  GEMV tiles of <= 4 rows: the TMA ring, or the register GEMV for the formats the ring does not take
+//   NS_PATH_IMMA  integer tensor cores, 3..32 rows of int4 weights with an integer compute type: the GEMV's exact block sums
+//   NS_PATH_TC    wgmma GEMM, bf16 numerics
+//   NS_PATH_Q6K   ggml Q6_K x Q8_K in tiles of <= 4 rows, plain nodes only
+// ns_route is the one place that picks the path; the workspace of a node and whether an RMSNorm folds into it follow from it.
+int ns_route(int kind, const ns_weight* const* w, int m, int flags) {
+  if (kind == NS_NODE_PLAIN && w[0]->wfmt == NS_W_Q6K) return NS_PATH_Q6K;  // whatever the flags
+  const int nw = kind == NS_NODE_QKV ? 3 : (kind == NS_NODE_FFN && w[1]) ? 2 : 1;  // the weights of the node's first launch
+  if (!(flags & (NS_MM_FORCE_GEMV | NS_MM_FORCE_TC)) && ns_gemm_imma_supported(w, nw, m)) {
+    if (kind == NS_NODE_PLAIN) return NS_PATH_IMMA;
+    if (kind == NS_NODE_QKV && w[0]->n % 2 == 0 && w[1]->n % 2 == 0) return NS_PATH_IMMA;  // QKV: q and k need an even n
+    if (kind == NS_NODE_FFN && ns_gemm_imma_supported(&w[2], 1, m)) return NS_PATH_IMMA;  // FFN: gate/up and down both, or neither
+  }
+  // The tensor-core GEMM has a fixed cost at small m (pipeline fill, split-K epilogue) while GEMV tiles keep the exact-integer
+  // numerics: GEMV tiles up to 16 rows (the reference switches from its GEMV to the blocked GEMM at m > 4)
+  bool tc = !(flags & NS_MM_FORCE_GEMV) && (m > 16 || (flags & NS_MM_FORCE_TC)) && ns_gemm_tc_supported(w[0]);
+  if (kind == NS_NODE_QKV)  // one bf16 activation image for all three: equal k, no act-order shuffles
+    tc = tc && ns_gemm_tc_supported(w[1]) && ns_gemm_tc_supported(w[2]) && w[1]->k == w[0]->k && w[2]->k == w[0]->k &&
+         !w[0]->shuffle && !w[1]->shuffle && !w[2]->shuffle;
+  if (kind == NS_NODE_FFN)  // shuffles are checked on gate/up only
+    tc = tc && ns_gemm_tc_supported(w[2]) && (!w[1] || ns_gemm_tc_supported(w[1])) && !w[0]->shuffle && !(w[1] && w[1]->shuffle);
+  if (tc) return NS_PATH_TC;
+  if (kind != NS_NODE_PLAIN)  // the weights of the first launch must fit one GEMV launch
+    if (int rc = ns_gemv_check(w, nw, kind == NS_NODE_QKV ? NS_GEMV_CONCAT : nw == 2 ? NS_GEMV_GATE_UP_SILU : NS_GEMV_PLAIN)) return rc;
+  return NS_PATH_GEMV;
+}
+
+// The RMSNorm in front of a launch of 1..3 weights folds into its activation quantiser when the launch is a ring GEMV that
+// quantises its own activations: decode rows (m <= 2, below the tensor-core GEMM) that the integer tensor cores do not take
+// (NS_IMMA_MIN_M may hand them 2 rows), k % 8 == 0
+static bool norm_foldable(const ns_weight* const* w, int nw, int m) {
+  static const bool off = getenv("NS_NO_FUSED_NORM") != nullptr;  // debugging aid: separate rmsnorm launches
+  if (off || m < 1 || m > 2 || nw < 1) return false;
+  for (int i = 0; i < nw; ++i)
+    if (!w[i] || !ns_gemv_fused_quant_ok(w[i]) || w[i]->k % 8) return false;
+  return !ns_gemm_imma_supported(w, nw, m);
+}
+
+// kpad: the widest padded input of the node's launches
+static size_t path_workspace_bytes(int path, int m, int kpad) {
+  switch (path) {
+    case NS_PATH_IMMA: return ns_gemm_imma_workspace_bound(m, kpad);
+    case NS_PATH_TC: return ns_gemm_tc_workspace_bytes(m, kpad);  // bf16 [m][kpad]
+    case NS_PATH_Q6K: return ns_q6k_workspace_bytes(4, kpad);
+    default: return ns_act_workspace_bytes(4, kpad);  // activation images of <= 4-row tiles
+  }
+}
+// Covers every path a node of up to m rows may take (NS_IMMA_MIN_M may hand a single row to the integer tensor cores, which
+// take 32 at most), so one workspace serves every smaller call too
 extern "C" size_t ns_device_workspace_bytes(int m, int k) {
-  const int kpad = (int)ns_round_up((size_t)k, 32);
-  const size_t gemv = ns_act_workspace_bytes(4, kpad);  // GEMV path: activations are prepared in tiles of <= 4 rows
-  const size_t tc = m > 4 ? ns_gemm_tc_workspace_bytes(m, kpad) : 0;  // tensor-core path: bf16 [m][kpad]
-  const size_t im = (m > 1 && m <= 32) ? ns_gemm_imma_workspace_bound(m, kpad) : 0;  // integer tensor-core path
-  const size_t a = gemv > tc ? gemv : tc;
-  return a > im ? a : im;
+  const int kpad = (int)ns_round_up((size_t)k, 32), rows = m < 1 ? 1 : m;
+  size_t b = 0;
+  for (int p = NS_PATH_GEMV; p <= NS_PATH_Q6K; ++p) {
+    const size_t s = path_workspace_bytes(p, p == NS_PATH_IMMA && rows > 32 ? 32 : rows, kpad);
+    b = s > b ? s : b;
+  }
+  return b;
 }
 
 static void* pick_ws(void* workspace, cudaStream_t st, size_t bytes) { return workspace ? workspace : scratch_get(st, bytes); }
 
-static bool use_tc(const ns_weight* w, int m, int flags) {
-  if (flags & NS_MM_FORCE_GEMV) return false;
-  if (!ns_gemm_tc_supported(w)) return false;
-  // The tensor-core GEMM has a fixed cost at small M (pipeline fill, split-K epilogue) while GEMV tiles keep the exact-integer
-  // numerics: GEMV tiles up to 16 rows.  The threshold also fixes the numerics class of a call (DESIGN.md section 4).
-  return m > 16 || (flags & NS_MM_FORCE_TC);
-}
-// 5..32 rows of an int4 weight with an integer compute type: integer tensor cores, exact block sums, weights read once
-static bool use_imma(const ns_weight* const* ws, int nw, int m, int flags) {
-  if (flags & (NS_MM_FORCE_GEMV | NS_MM_FORCE_TC)) return false;
-  return ns_gemm_imma_supported(ws, nw, m);
-}
-static size_t ws_need(const ns_weight* w, int m, bool tc) {
-  return tc ? ns_gemm_tc_workspace_bytes(m, w->kpad) : ns_act_workspace_bytes(4, w->kpad);
-}
-
 static int norm_unsupported(const char* who) {
   ns_set_error("%s: the RMSNorm can only be folded into the ring GEMV (int4 weights, integer compute type, <= 2 rows)", who);
   return NS_E_UNSUPPORTED;
+}
+
+// One launch of 1..3 weights sharing one activation on its path; mode, epilogue and dst layout as ns_launch_gemv.  The wgmma
+// GEMM has no element-wise epilogue (the FFN applies its activation function on its own) and writes weight i at dst + i * m * ldo.
+static int launch_set(int path, const ns_weight* const* w, int nw, int mode, const float* act, int lda, float* dst, int ldo, int m,
+                      const float* bias, int bcast, const float* residual, int eltop, const float* norm_w, float norm_eps,
+                      int one_image, void* ws, cudaStream_t st) {
+  if (path == NS_PATH_IMMA) return ns_launch_gemm_imma(w, nw, mode, act, lda, dst, ldo, m, bias, bcast, residual, eltop, ws, st);
+  if (path == NS_PATH_TC) {
+    if (int rc = ns_launch_act_bf16(w[0], act, lda, m, ws, st)) return rc;
+    for (int i = 0; i < nw; ++i)
+      if (int rc = ns_launch_gemm_tc(w[i], ws, dst + (size_t)i * m * ldo, ldo, m, bias, bcast, residual, st)) return rc;
+    return NS_OK;
+  }
+  const int tile = path == NS_PATH_Q6K ? 4 : ns_gemv_tile_rows(w[0]);
+  const bool fused = path == NS_PATH_GEMV && ns_gemv_fused_quant_ok(w[0]);  // the GEMV quantises the activations itself
+  for (int m0 = 0; m0 < m; m0 += tile) {
+    const int mt = (m - m0 < tile) ? (m - m0) : tile;
+    const float* a = act + (size_t)m0 * lda;
+    float* d = dst + (size_t)m0 * ldo;
+    const float* b = bias ? (bcast ? bias : bias + (size_t)m0 * ldo) : nullptr;
+    const float* r = residual ? residual + (size_t)m0 * ldo : nullptr;
+    int rc = NS_OK;
+    if (path == NS_PATH_Q6K) {
+      rc = ns_launch_mul_mat_q6k(w[0], a, lda, d, ldo, mt, b, bcast, r, ws, st);
+    } else {
+      if (!fused) rc = ns_launch_act_prep(a, lda, mt, w[0], ws, st);
+      if (!rc)
+        rc = ns_launch_gemv(w, nw, mode, fused ? nullptr : ws, d, ldo, mt, m, b, bcast, r, nullptr, st, fused ? a : nullptr, lda, eltop,
+                            norm_w, norm_eps, one_image);
+    }
+    if (rc) return rc;
+  }
+  return NS_OK;
 }
 
 static int mul_mat_impl(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* bias,
@@ -637,48 +706,13 @@ static int mul_mat_impl(const ns_weight* w, const float* act, int lda, float* ds
     ns_set_error("ns_mul_mat: invalid arguments (m=%d lda=%d ldo=%d)", m, lda, ldo);
     return NS_E_INVALID;
   }
+  if (norm_w && !norm_foldable(&w, 1, m)) return norm_unsupported("ns_rmsnorm_mul_mat");
+  const int path = ns_route(NS_NODE_PLAIN, &w, m, flags);
   cudaStream_t st = stream_of(queue);
-  const int bcast = (flags & NS_MM_BIAS_BCAST) ? 1 : 0;
-  if (norm_w && ((flags & NS_MM_FORCE_TC) || !ns_gemv_fused_norm_ok(&w, 1, m))) return norm_unsupported("ns_rmsnorm_mul_mat");
-  if (w->wfmt == NS_W_Q6K) {  // ggml Q6_K x Q8_K, tiles of <= 4 activation rows
-    void* ws6 = pick_ws(workspace, st, ns_q6k_workspace_bytes(4, w->k));
-    if (!ws6) return NS_E_CUDA;
-    for (int m0 = 0; m0 < m; m0 += 4) {
-      const int mt = m - m0 < 4 ? m - m0 : 4;
-      if (int rc = ns_launch_mul_mat_q6k(w, act + (size_t)m0 * lda, lda, dst + (size_t)m0 * ldo, ldo, mt,
-                                         bias ? (bcast ? bias : bias + (size_t)m0 * ldo) : nullptr, bcast,
-                                         residual ? residual + (size_t)m0 * ldo : nullptr, ws6, st))
-        return rc;
-    }
-    return NS_OK;
-  }
-  if (use_imma(&w, 1, m, flags)) {
-    void* wsi = pick_ws(workspace, st, ns_gemm_imma_workspace_bound(m, w->kpad));
-    if (!wsi) return NS_E_CUDA;
-    return ns_launch_gemm_imma(&w, 1, NS_GEMV_PLAIN, act, lda, dst, ldo, m, bias, bcast, residual, NS_ELT_DEFAULT, wsi, st);
-  }
-  const bool tc = use_tc(w, m, flags);
-  void* ws = pick_ws(workspace, st, ws_need(w, m, tc));
+  void* ws = pick_ws(workspace, st, path_workspace_bytes(path, m, w->kpad));
   if (!ws) return NS_E_CUDA;
-  if (tc) {
-    // M > 16: wgmma tensor-core GEMM, bf16 numerics (the reference switches from its GEMV to the blocked GEMM at M > 4)
-    if (int rc = ns_launch_act_bf16(w, act, lda, m, ws, st)) return rc;
-    return ns_launch_gemm_tc(w, ws, dst, ldo, m, bias, bcast, residual, st);
-  }
-  const int tile = ns_gemv_tile_rows(w);
-  const bool fused = ns_gemv_fused_quant_ok(w);  // the GEMV quantises the activations itself: one launch per tile
-  for (int m0 = 0; m0 < m; m0 += tile) {
-    const int mt = (m - m0 < tile) ? (m - m0) : tile;
-    const float* a = act + (size_t)m0 * lda;
-    if (!fused)
-      if (int rc = ns_launch_act_prep(a, lda, mt, w, ws, st)) return rc;
-    if (int rc = ns_launch_gemv(&w, 1, NS_GEMV_PLAIN, fused ? nullptr : ws, dst + (size_t)m0 * ldo, ldo, mt, m,
-                                bias ? (bcast ? bias : bias + (size_t)m0 * ldo) : nullptr, bcast,
-                                residual ? residual + (size_t)m0 * ldo : nullptr, nullptr, st, fused ? a : nullptr, lda,
-                                NS_ELT_DEFAULT, norm_w, norm_eps, one_image))
-      return rc;
-  }
-  return NS_OK;
+  return launch_set(path, &w, 1, NS_GEMV_PLAIN, act, lda, dst, ldo, m, bias, (flags & NS_MM_BIAS_BCAST) ? 1 : 0, residual,
+                    NS_ELT_DEFAULT, norm_w, norm_eps, one_image, ws, st);
 }
 extern "C" int ns_mul_mat(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* bias,
                           const float* residual, int flags, void* workspace, void* queue) {
@@ -699,36 +733,14 @@ int ns_mul_qkv_norm(const ns_weight* wq, const ns_weight* wk, const ns_weight* w
                     int m, void* workspace, void* queue, const float* norm_w, float norm_eps) {
   if (int rc = ns_ensure_device()) return rc;
   if (!wq || !wk || !wv || !act || !dst || m <= 0) return NS_E_INVALID;
-  cudaStream_t st = stream_of(queue);
   const ns_weight* wl[3] = {wq, wk, wv};
-  if (norm_w && !ns_gemv_fused_norm_ok(wl, 3, m)) return norm_unsupported("ns_rmsnorm_mul_qkv");
-  if (use_imma(wl, 3, m, 0) && !(wq->n % 2) && !(wk->n % 2)) {
-    void* wsi = pick_ws(workspace, st, ns_gemm_imma_workspace_bound(m, wq->kpad));
-    if (!wsi) return NS_E_CUDA;
-    return ns_launch_gemm_imma(wl, 3, NS_GEMV_CONCAT, act, lda, dst, ldo, m, nullptr, 0, nullptr, NS_ELT_DEFAULT, wsi, st);
-  }
-  const bool tc = use_tc(wq, m, 0) && ns_gemm_tc_supported(wk) && ns_gemm_tc_supported(wv) && wk->k == wq->k &&
-                  wv->k == wq->k && !wq->shuffle && !wk->shuffle && !wv->shuffle;
-  void* ws = pick_ws(workspace, st, ws_need(wq, m, tc));
+  if (norm_w && !norm_foldable(wl, 3, m)) return norm_unsupported("ns_rmsnorm_mul_qkv");
+  const int path = ns_route(NS_NODE_QKV, wl, m, 0);
+  if (path < 0) return path;
+  cudaStream_t st = stream_of(queue);
+  void* ws = pick_ws(workspace, st, path_workspace_bytes(path, m, wq->kpad));
   if (!ws) return NS_E_CUDA;
-  if (tc) {
-    if (int rc = ns_launch_act_bf16(wq, act, lda, m, ws, st)) return rc;
-    for (int i = 0; i < 3; ++i)
-      if (int rc = ns_launch_gemm_tc(wl[i], ws, dst + (size_t)i * m * ldo, ldo, m, nullptr, 0, nullptr, st)) return rc;
-    return NS_OK;
-  }
-  const int tile = ns_gemv_tile_rows(wq);
-  const bool fused = ns_gemv_fused_quant_ok(wq);
-  for (int m0 = 0; m0 < m; m0 += tile) {
-    const int mt = (m - m0 < tile) ? (m - m0) : tile;
-    const float* a = act + (size_t)m0 * lda;
-    if (!fused)
-      if (int rc = ns_launch_act_prep(a, lda, mt, wq, ws, st)) return rc;
-    if (int rc = ns_launch_gemv(wl, 3, NS_GEMV_CONCAT, fused ? nullptr : ws, dst + (size_t)m0 * ldo, ldo, mt, m, nullptr, 0,
-                                nullptr, nullptr, st, fused ? a : nullptr, lda, NS_ELT_DEFAULT, norm_w, norm_eps))
-      return rc;
-  }
-  return NS_OK;
+  return launch_set(path, wl, 3, NS_GEMV_CONCAT, act, lda, dst, ldo, m, nullptr, 0, nullptr, NS_ELT_DEFAULT, norm_w, norm_eps, 0, ws, st);
 }
 extern "C" int ns_mul_qkv(const ns_weight* wq, const ns_weight* wk, const ns_weight* wv, const float* act, int lda,
                           float* dst, int ldo, int m, void* workspace, void* queue) {
@@ -752,80 +764,29 @@ static int ffn_impl(const ns_weight* w1, const ns_weight* w2, const ns_weight* w
     ns_set_error("fused FFN: invalid arguments");
     return NS_E_INVALID;
   }
+  const ns_weight* wn[3] = {w1, w3, w2};
+  const int ngu = w3 ? 2 : 1, fmid = w1->n;
+  if (norm_w && !norm_foldable(wn, ngu, m)) return norm_unsupported("fused FFN");
+  const int path = ns_route(NS_NODE_FFN, wn, m, 0);
+  if (path < 0) return path;
   cudaStream_t st = stream_of(queue);
-  const int fmid = w1->n;
-  const bool tc = use_tc(w1, m, 0) && ns_gemm_tc_supported(w2) && (!w3 || ns_gemm_tc_supported(w3)) && !w1->shuffle &&
-                  !(w3 && w3->shuffle);
-  const int kmax = w1->kpad > w2->kpad ? w1->kpad : w2->kpad;
-  {
-    const ns_weight* gu2[2] = {w1, w3};
-    if (norm_w && !ns_gemv_fused_norm_ok(gu2, w3 ? 2 : 1, m)) return norm_unsupported("fused FFN");
-    if (use_imma(gu2, w3 ? 2 : 1, m, 0) && use_imma(&w2, 1, m, 0)) {
-      void* wsi = pick_ws(workspace, st, ns_gemm_imma_workspace_bound(m, kmax));
-      if (!wsi) return NS_E_CUDA;
-      if (w3) {
-        if (int rc = ns_launch_gemm_imma(gu2, 2, NS_GEMV_GATE_UP_SILU, act, lda, tmp, fmid, m, nullptr, 0, nullptr, eltop, wsi, st)) return rc;
-      } else {
-        if (int rc = ns_launch_gemm_imma(gu2, 1, NS_GEMV_PLAIN, act, lda, tmp, fmid, m, b1, bcast, nullptr, NS_ELT_GELU, wsi, st)) return rc;
-      }
-      return ns_launch_gemm_imma(&w2, 1, NS_GEMV_PLAIN, tmp, fmid, dst, ldo, m, b2, bcast, residual, NS_ELT_DEFAULT, wsi, st);
-    }
-  }
-  void* ws = pick_ws(workspace, st, tc ? ns_gemm_tc_workspace_bytes(m, kmax) : ns_act_workspace_bytes(4, kmax));
+  void* ws = pick_ws(workspace, st, path_workspace_bytes(path, m, w1->kpad > w2->kpad ? w1->kpad : w2->kpad));
   if (!ws) return NS_E_CUDA;
-  if (tc) {
-    float* gate = tmp;
-    if (int rc = ns_launch_act_bf16(w1, act, lda, m, ws, st)) return rc;
-    if (int rc = ns_launch_gemm_tc(w1, ws, gate, fmid, m, b1, bcast, nullptr, st)) return rc;
-    if (w3) {
-      float* up = tmp + (size_t)m * fmid;
-      if (int rc = ns_launch_gemm_tc(w3, ws, up, fmid, m, nullptr, 0, nullptr, st)) return rc;
-      // one_image (the eval step: nobody reads tmp): the product goes straight into the down projection's bf16 image (the
-      // activation image of gate/up in `ws` is dead once both GEMMs have been issued -- stream order)
-      int frc = NS_OK;
-      if (one_image && ns_launch_silu_mul_bf16(w2, gate, up, m, ws, st, eltop, &frc)) {
-        if (frc) return frc;
-        return ns_launch_gemm_tc(w2, ws, dst, ldo, m, b2, bcast, residual, st);
-      }
-      if (int rc = ns_launch_silu_mul(gate, up, gate, nullptr, (size_t)m * fmid, st, eltop)) return rc;
-    } else {
-      if (int rc = ns_launch_gelu(gate, (size_t)m * fmid, st)) return rc;
-    }
-    if (int rc = ns_launch_act_bf16(w2, gate, fmid, m, ws, st)) return rc;
-    return ns_launch_gemm_tc(w2, ws, dst, ldo, m, b2, bcast, residual, st);
+  if (int rc = launch_set(path, wn, ngu, w3 ? NS_GEMV_GATE_UP_SILU : NS_GEMV_PLAIN, act, lda, tmp, fmid, m, b1, bcast, nullptr, eltop,
+                          norm_w, norm_eps, one_image, ws, st))
+    return rc;
+  if (path == NS_PATH_TC) {  // gate (and up) landed in tmp as plain GEMM outputs
+    float* up = tmp + (size_t)m * fmid;
+    int rc = NS_OK;
+    // one_image (the eval step: nobody reads tmp): the product goes straight into the down projection's bf16 image (the
+    // activation image of gate/up in `ws` is dead once both GEMMs have been issued -- stream order)
+    if (w3 && one_image && ns_launch_silu_mul_bf16(w2, tmp, up, m, ws, st, eltop, &rc))
+      return rc ? rc : ns_launch_gemm_tc(w2, ws, dst, ldo, m, b2, bcast, residual, st);
+    rc = w3 ? ns_launch_silu_mul(tmp, up, tmp, nullptr, (size_t)m * fmid, st, eltop) : ns_launch_gelu(tmp, (size_t)m * fmid, st);
+    if (rc) return rc;
   }
-  const ns_weight* gu[2] = {w1, w3};
-  int tile = ns_gemv_tile_rows(w1);
-  const bool fused1 = ns_gemv_fused_quant_ok(w1), fused2 = ns_gemv_fused_quant_ok(w2);
-  for (int m0 = 0; m0 < m; m0 += tile) {
-    const int mt = (m - m0 < tile) ? (m - m0) : tile;
-    const float* a = act + (size_t)m0 * lda;
-    if (!fused1)
-      if (int rc = ns_launch_act_prep(a, lda, mt, w1, ws, st)) return rc;
-    if (w3) {
-      if (int rc = ns_launch_gemv(gu, 2, NS_GEMV_GATE_UP_SILU, fused1 ? nullptr : ws, tmp + (size_t)m0 * fmid, fmid, mt, m, nullptr,
-                                  0, nullptr, nullptr, st, fused1 ? a : nullptr, lda, eltop, norm_w, norm_eps, one_image))
-        return rc;
-    } else {
-      if (int rc = ns_launch_gemv(gu, 1, NS_GEMV_PLAIN, fused1 ? nullptr : ws, tmp + (size_t)m0 * fmid, fmid, mt, m,
-                                  b1 ? (bcast ? b1 : b1 + (size_t)m0 * fmid) : nullptr, bcast, nullptr, nullptr, st,
-                                  fused1 ? a : nullptr, lda, NS_ELT_GELU, norm_w, norm_eps))
-        return rc;
-    }
-  }
-  tile = ns_gemv_tile_rows(w2);
-  for (int m0 = 0; m0 < m; m0 += tile) {
-    const int mt = (m - m0 < tile) ? (m - m0) : tile;
-    const float* a = tmp + (size_t)m0 * fmid;
-    if (!fused2)
-      if (int rc = ns_launch_act_prep(a, fmid, mt, w2, ws, st)) return rc;
-    if (int rc = ns_launch_gemv(&w2, 1, NS_GEMV_PLAIN, fused2 ? nullptr : ws, dst + (size_t)m0 * ldo, ldo, mt, m,
-                                b2 ? (bcast ? b2 : b2 + (size_t)m0 * ldo) : nullptr, bcast,
-                                residual ? residual + (size_t)m0 * ldo : nullptr, nullptr, st, fused2 ? a : nullptr, fmid, NS_ELT_DEFAULT,
-                                nullptr, 0.f, one_image))
-      return rc;
-  }
-  return NS_OK;
+  return launch_set(path, &w2, 1, NS_GEMV_PLAIN, tmp, fmid, dst, ldo, m, b2, bcast, residual, NS_ELT_DEFAULT, nullptr, 0.f, one_image,
+                    ws, st);
 }
 // dst = residual + FFN_SiLU(act): the decode engine's "cur = ne_add(ffn, inpFF)" (llama.cpp:698) folded into the down GEMV
 int ns_ffn_silu_residual(const ns_weight* w1, const ns_weight* w2, const ns_weight* w3, const float* act, int lda, float* tmp,
@@ -844,7 +805,7 @@ extern "C" int ns_rmsnorm_ffn_silu(const ns_weight* w1, const ns_weight* w2, con
                   norm_eps);
 }
 extern "C" int ns_rmsnorm_fusable(const ns_weight* const* weights, int nw, int m) {
-  return (weights && nw >= 1 && nw <= 3 && ns_gemv_fused_norm_ok(weights, nw, m)) ? 1 : 0;
+  return (weights && nw >= 1 && nw <= 3 && norm_foldable(weights, nw, m)) ? 1 : 0;
 }
 extern "C" int ns_ffn_silu(const ns_weight* w1, const ns_weight* w2, const ns_weight* w3, const float* act, int lda,
                            float* tmp, float* dst, int ldo, int m, void* workspace, void* queue) {
@@ -932,14 +893,6 @@ static int expert_scratch(const ExpertPlan& pl, int m, int k, int n, size_t mm_w
   return NS_OK;
 }
 
-// a slice of c <= m rows may take any of the matmul paths: the workspace must cover the largest of them
-static size_t expert_ws_bytes(int m, int k) {
-  size_t b = ns_device_workspace_bytes(m, k);
-  const size_t small = ns_device_workspace_bytes(m < 32 ? m : 32, k), q6 = ns_q6k_workspace_bytes(4, k);
-  b = b > small ? b : small;
-  return b > q6 ? b : q6;
-}
-
 extern "C" int ns_mul_mat_id(const ns_weight* const* experts, int n_as, const int32_t* ids, int ids_stride, int id, int ids_on_device,
                              const float* act, int lda, float* dst, int ldo, int m, int flags, void* queue) {
   if (int rc = ns_ensure_device()) return rc;
@@ -955,7 +908,7 @@ extern "C" int ns_mul_mat_id(const ns_weight* const* experts, int n_as, const in
   ExpertPlan pl;
   if (int rc = plan_experts(ids, ids_stride, id, ids_on_device, m, n_as, st, &pl)) return rc;
   ExpertScratch sc;
-  if (int rc = expert_scratch(pl, m, k, n, expert_ws_bytes(m, k), st, &sc)) return rc;
+  if (int rc = expert_scratch(pl, m, k, n, ns_device_workspace_bytes(m, k), st, &sc)) return rc;  // any slice of <= m rows
   const float* x = act;
   float* y = dst;
   int ldx = lda, ldy = ldo;
@@ -994,8 +947,7 @@ extern "C" int ns_ffn_id(const ns_weight* const* gate, const ns_weight* const* d
   ExpertPlan pl;
   if (int rc = plan_experts(ids, ids_stride, id, ids_on_device, m, n_as, st, &pl)) return rc;
   ExpertScratch sc;
-  const size_t w1 = expert_ws_bytes(m, k), w2 = expert_ws_bytes(m, fmid);
-  if (int rc = expert_scratch(pl, m, k, n, w1 > w2 ? w1 : w2, st, &sc)) return rc;
+  if (int rc = expert_scratch(pl, m, k, n, ns_device_workspace_bytes(m, k > fmid ? k : fmid), st, &sc)) return rc;
   const float* x = act;
   float* y = dst;
   int ldx = lda, ldy = ldo;

@@ -368,17 +368,7 @@ bool ns_gemv_fused_quant_ok(const ns_weight* w) {
   return (qg == 32 || qg == 64 || qg == 128 || qg == 256) && w->k % qg == 0;
 }
 
-bool ns_gemv_fused_norm_ok(const ns_weight* const* ws, int nw, int m) {
-  static const bool off = getenv("NS_NO_FUSED_NORM") != nullptr;  // debugging aid: separate rmsnorm launches
-  if (off || m < 1 || m > 2 || nw < 1) return false;
-  for (int i = 0; i < nw; ++i)
-    if (!ws[i] || !ns_gemv_fused_quant_ok(ws[i]) || ws[i]->k % 8) return false;
-  return !ns_gemm_imma_supported(ws, nw, m);  // (NS_IMMA_MIN_M may hand 2 rows to the integer tensor cores)
-}
-
-int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* act_ws, float* dst, int ldo, int m,
-                   int m_total, const float* bias, int bias_bcast, const float* residual, float* aux, cudaStream_t st,
-                   const float* act_f32, int lda, int eltop, const float* norm_w, float norm_eps, int one_image) {
+int ns_gemv_check(const ns_weight* const* ws_, int nw, int mode) {
   const ns_weight* w0 = ws_[0];
   for (int i = 1; i < nw; ++i) {
     const ns_weight* wi = ws_[i];
@@ -400,6 +390,23 @@ int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* ac
     ns_set_error("group size %d is not a multiple of 32", w0->group);
     return NS_E_UNSUPPORTED;
   }
+  if (w0->wfmt == NS_W_NF4 && !(w0->comp == NS_COMP_F32 || w0->comp == NS_COMP_BF16)) {
+    ns_set_error("NF4 weights need a float compute type");
+    return NS_E_UNSUPPORTED;
+  }
+  for (int i = 0; mode == NS_GEMV_CONCAT && i + 1 < nw; ++i)
+    if (ws_[i]->n & 1) {
+      ns_set_error("fused matmul: every weight but the last needs an even n");
+      return NS_E_UNSUPPORTED;
+    }
+  return NS_OK;
+}
+
+int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* act_ws, float* dst, int ldo, int m,
+                   int m_total, const float* bias, int bias_bcast, const float* residual, float* aux, cudaStream_t st,
+                   const float* act_f32, int lda, int eltop, const float* norm_w, float norm_eps, int one_image) {
+  if (int rc = ns_gemv_check(ws_, nw, mode)) return rc;
+  const ns_weight* w0 = ws_[0];
   if (m < 1 || m > ns_gemv_tile_rows(w0)) {
     ns_set_error("internal: GEMV tile of %d rows", m);
     return NS_E_INVALID;
@@ -407,10 +414,6 @@ int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* ac
   const int kpad = w0->kpad;
   const bool fmode = (w0->comp == NS_COMP_F32 || w0->comp == NS_COMP_BF16);
   const int amode = fmode ? A_F32 : (w0->comp == NS_COMP_INT8 ? A_U8 : A_S8);
-  if (w0->wfmt == NS_W_NF4 && !fmode) {
-    ns_set_error("NF4 weights need a float compute type");
-    return NS_E_UNSUPPORTED;
-  }
   const int meta_stride = ns_meta_stride(kpad);
 
   GemvParams P = {};
@@ -421,10 +424,6 @@ int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* ac
     // QKV convention of the reference: dst = [nw][M][ldo] (ip_fusion_qkv.cpp:84-86)
     P.dst_off[i] = (mode == NS_GEMV_CONCAT) ? (long long)i * m_total * ldo : 0;
     ntot += ws_[i]->n;
-    if (mode == NS_GEMV_CONCAT && i + 1 < nw && (ws_[i]->n & 1)) {
-      ns_set_error("fused matmul: every weight but the last needs an even n");
-      return NS_E_UNSUPPORTED;
-    }
   }
   P.nw = nw;
   P.mode = mode;

@@ -39,7 +39,7 @@ int launch_one(const GemvParams& P, int mt, cudaStream_t st) {
     ns_set_error("gemv_ring: row pitch %d too large for shared memory", P.pitch);
     return NS_E_UNSUPPORTED;
   }
-  if constexpr (M <= 2) {  // the norm is only ever folded into launches of <= 2 rows (ns_gemv_fused_norm_ok)
+  if constexpr (M <= 2) {  // the norm is only ever folded into launches of <= 2 rows (norm_foldable, abi.cu)
     if ((P.norm_w || P.one_image) && P.act_f32) {
       if (plan.rows == 2) return launch_rows<AMODE, M, ASYM, STYPE, 2, true>(P, plan, act_region, act_row, red_off, st);
       return launch_rows<AMODE, M, ASYM, STYPE, 1, true>(P, plan, act_region, act_row, red_off, st);

@@ -80,8 +80,7 @@ int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* ac
                    const float* act_f32 = nullptr, int lda = 0, int eltop = 0, const float* norm_w = nullptr, float norm_eps = 0.f,
                    int one_image = 0);
 bool ns_gemv_fused_quant_ok(const ns_weight* w);  // can the GEMV quantise the activations itself (one launch)?
-// can RMSNorm(x) * norm_w be folded into that quantiser for m rows (m <= 2: the rows the ring GEMV takes before IMMA does)?
-bool ns_gemv_fused_norm_ok(const ns_weight* const* ws, int nw, int m);
+int ns_gemv_check(const ns_weight* const* ws, int nw, int mode);  // can these weights share one GEMV launch? NS_OK or the error
 int ns_launch_repack_q4_0(const void* rows_dev, size_t nb01, ns_weight* w, cudaStream_t st);
 int ns_launch_repack_canonical(const int8_t* q_kn_dev, const float* sc_dev, const int8_t* zp_dev, ns_weight* w,
                                cudaStream_t st);
@@ -98,6 +97,11 @@ int ns_launch_dequant_q6k(const ns_weight* w, float* dst, int ld, cudaStream_t s
 int ns_launch_mul_mat_q6k(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* bias,
                           int bias_bcast, const float* residual, void* ws, cudaStream_t st);
 
+// abi.cu: the kernel path of a matmul node (DESIGN.md section 4), or a negative NS_E_* when its weights cannot form the node.
+// w: {w} (plain), {wq, wk, wv} (QKV concat) or {w1, w3, w2} (FFN gate, up (NULL: two-weight FFN), down); flags: NS_MM_*
+enum { NS_PATH_GEMV, NS_PATH_IMMA, NS_PATH_TC, NS_PATH_Q6K };
+enum { NS_NODE_PLAIN, NS_NODE_QKV, NS_NODE_FFN };
+int ns_route(int kind, const ns_weight* const* w, int m, int flags);
 // abi.cu: fused FFN with the residual add folded into the down projection (used by the decode engine, llama.cu)
 int ns_ffn_silu_residual(const ns_weight* w1, const ns_weight* w2, const ns_weight* w3, const float* act, int lda, float* tmp,
                          float* dst, int ldo, int m, const float* residual, void* workspace, cudaStream_t st,
