@@ -301,7 +301,7 @@ typedef struct ns_llama_hparams {
   int n_vocab, n_embd, n_head, n_head_kv, n_layer, n_ff, n_ctx;
   float norm_eps;   /* hparams.norm_eps   (<= 0: 1e-6)  */
   float rope_theta; /* hparams.freq_base  (<= 0: 10000) */
-  float rope_scale; /* hparams.freq_scale (<= 0: 1)     */
+  float rope_scale; /* hparams.freq_scale (<= 0: 1): divides the RoPE angle, as ne_rope does */
 } ns_llama_hparams;
 enum ns_llama_tensor {
   NS_LT_TOK_EMBD = 0, /* others[0]  [n_vocab][n_embd] f32 */
@@ -325,6 +325,27 @@ NS_API int ns_llama_generate(ns_llama* ctx, int32_t first_token, int n_past, int
  * tokens instead: reference numerics for the whole prompt at about 1/6 of the prefill throughput. */
 NS_API int ns_llama_set_exact_prefill(ns_llama* ctx, int on);
 NS_API unsigned long long ns_llama_kv_bytes(const ns_llama* ctx);
+/* One layer's attention of the eval step on its own, for parity tests: RoPE (mode 0, angle = p * rope_theta^(-2i/hd) / rope_scale)
+ * of q [m][n_head * hd] in place and of the m new rows k [m][n_head_kv * hd] at positions n_past .. n_past + m - 1, k and v appended
+ * to the fp16 caches kc / vc [n_head_kv][n_ctx][hd], out [m][n_head * hd] = causal softmax(K q / sqrt(hd)) V (llama.cpp:286-302).
+ * All pointers are device memory.  kernel: NS_ATTN_AUTO (what ns_llama_eval runs for this shape) or one kernel forced:
+ *   NS_ATTN_SPLIT_DECODE  m = 1, hd 64 / 128: context split over 256-position ranges, per-range results merged
+ *   NS_ATTN_ROWS          hd 64 / 128: one CTA per (head, row); RoPE and the KV append fused in when m = 1
+ *   NS_ATTN_MMA           hd 64 / 128: causal prompt attention on mma.sync tensor cores
+ *   NS_ATTN_GENERIC       any even hd: one CTA per (head, row) after a separate RoPE + KV-append launch
+ * A forced kernel that cannot take the shape returns NS_E_UNSUPPORTED without launching anything.
+ * ws: device workspace of ns_llama_attention_workspace_bytes(n_head, hd, n_ctx) bytes, zeroed once by the caller:
+ *   int state[4] (the call writes n_past to state[1]) | unsigned tickets[n_head] (zero again after every call), padded to 16 bytes |
+ *   float partials[n_head][ceil(n_ctx / 256)][hd + 2] (split decode scratch, no value carried between calls) */
+#define NS_ATTN_AUTO 0
+#define NS_ATTN_SPLIT_DECODE 1
+#define NS_ATTN_ROWS 2
+#define NS_ATTN_MMA 3
+#define NS_ATTN_GENERIC 4
+NS_API size_t ns_llama_attention_workspace_bytes(int n_head, int hd, int n_ctx);
+NS_API int ns_llama_attention(int kernel, float* q, const float* k, const float* v, void* kc, void* vc, int n_head, int n_head_kv,
+                              int hd, int n_ctx, int n_past, int m, float rope_theta, float rope_scale, float* out, void* ws,
+                              void* queue);
 
 /* ---- tensor-parallel exchange step over NVLink peer memory (SURVEY 8e) --------------------------------------------
  * One-shot sum all-reduce replacing reduce_add / ne_all_reduce (core/parallel_context.cpp:47, ne_layers.c:5466) for the

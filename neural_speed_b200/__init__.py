@@ -31,6 +31,7 @@ BTLA_S8 = 8 | (1 << 8)
 BTLA_S4_CLIP = 4 | (1 << 8)
 BTLA_F4_NF4 = 4 | (2 << 16)
 MM_BIAS_BCAST, MM_FORCE_GEMV, MM_FORCE_TC = 1, 2, 4
+ATTN_AUTO, ATTN_SPLIT_DECODE, ATTN_ROWS, ATTN_MMA, ATTN_GENERIC = 0, 1, 2, 3, 4
 
 EXPORTS = [
     "ns_last_error", "ns_version", "ns_launch_count",
@@ -58,7 +59,7 @@ EXPORTS = [
     "ns_device_quantize_q4_0", "ns_device_quantize_act",
     "BTLAGemmPackBSize", "BTLAGemmQuantPackB", "BTLAGemmPackB", "BTLAGemmUnPackB", "ns_quantize_row_q4_0", "ns_split_weight_size", "ns_split_weight",
     "ns_llama_create", "ns_llama_free", "ns_llama_set_f32", "ns_llama_set_weight", "ns_llama_eval", "ns_llama_generate", "ns_llama_set_exact_prefill",
-    "ns_llama_kv_bytes",
+    "ns_llama_kv_bytes", "ns_llama_attention_workspace_bytes", "ns_llama_attention",
     "ns_comm_handle_bytes", "ns_comm_create", "ns_comm_get_handle", "ns_comm_open_peers", "ns_comm_link_local", "ns_comm_all_reduce_f32",
     "ns_comm_status", "ns_comm_free",
 ]
@@ -180,6 +181,9 @@ def lib() -> C.CDLL:
     L.ns_llama_generate.argtypes = [vp, C.c_int32, i, i, vp]
     L.ns_llama_kv_bytes.restype = C.c_ulonglong
     L.ns_llama_kv_bytes.argtypes = [vp]
+    L.ns_llama_attention_workspace_bytes.restype = sz
+    L.ns_llama_attention_workspace_bytes.argtypes = [i, i, i]
+    L.ns_llama_attention.argtypes = [i, vp, vp, vp, vp, vp, i, i, i, i, i, i, C.c_float, C.c_float, vp, vp, vp]
     L.ns_comm_handle_bytes.restype = sz
     L.ns_comm_create.restype = vp
     L.ns_comm_create.argtypes = [i, i, sz, vp]

@@ -40,7 +40,8 @@ def _f16(x):
 
 def rope_mode0(x, pos, hd, freq_base=10000.0, rope_scale=1.0):
     """ne_rope_inplace(mode 0) on x [n_head, hd] at position pos (ne_layers.c:9300, 9380-9396): theta_base = p, then
-    theta_base *= theta_scale per pair (fp32); dst0 = x0*cos - x1*sin, dst1 = x0*sin + x1*cos.  The reference's default build
+    theta_base *= theta_scale per pair (fp32), angle = freq_scale * theta_base (rope_yarn, :9207) with freq_scale =
+    1 / rope_scale (the op's parameter, hparams.freq_scale, is inverted at :9263); dst0 = x0*cos - x1*sin, dst1 = x0*sin + x1*cos.  The reference's default build
     (-O3 -mfma) contracts these to fma(x0, cos, -(x1*sin)) and fma(x0, sin, x1*cos); pinned bit-exact against the reference's
     own engine (oracle/_ref/libref_ne.so, tests/test_oracle_vs_ref.py)."""
     theta_scale = np.float32(_libm.powf(float(np.float32(freq_base)), float(np.float32(-2.0) / np.float32(hd))))
@@ -56,6 +57,43 @@ def rope_mode0(x, pos, hd, freq_base=10000.0, rope_scale=1.0):
             x0, x1 = float(x[h, i0]), float(x[h, i0 + 1])
             out[h, i0] = _libm.fmaf(x0, c, -float(np.float32(np.float32(x1) * np.float32(s))))
             out[h, i0 + 1] = _libm.fmaf(x0, s, float(np.float32(np.float32(x1) * np.float32(c))))
+    return out
+
+
+def _fmaf(a, b, c):
+    """fp32 fma, element-wise: a*b is exact in double; the double sum is rounded to odd before the fp32 rounding, so the two
+    roundings give the correctly rounded fp32 result (no double-rounding error)"""
+    p = np.asarray(a, np.float32).astype(np.float64) * np.asarray(b, np.float32).astype(np.float64)
+    c = np.asarray(c, np.float32).astype(np.float64)
+    hi = p + c
+    bb = hi - p
+    lo = (p - (hi - bb)) + (c - bb)  # two-sum: hi + lo == p + c exactly
+    even = (hi.view(np.int64) & 1) == 0
+    hi = np.where((lo != 0) & even, np.nextafter(hi, np.where(lo > 0, np.inf, -np.inf)), hi)
+    return hi.astype(np.float32)
+
+
+def rope_mode0_rows(x, pos, hd, freq_base=10000.0, rope_scale=1.0):
+    """rope_mode0 of x [T, n_head, hd] with row t at position pos[t], vectorised: the same fp32 theta recurrence, the same
+    libm cosf / sinf (one call per distinct (position, pair)), the same contractions -- bit-identical to rope_mode0."""
+    x = np.asarray(x, np.float32)
+    pos = np.asarray(pos, np.int64).reshape(-1)
+    assert x.shape[0] == pos.size and x.shape[-1] == hd
+    theta_scale = np.float32(_libm.powf(float(np.float32(freq_base)), float(np.float32(-2.0) / np.float32(hd))))
+    freq_scale = np.float32(1.0) / np.float32(rope_scale)
+    upos, inv = np.unique(pos, return_inverse=True)
+    th = np.empty((upos.size, hd // 2), np.float32)
+    theta = upos.astype(np.float32)
+    for i in range(hd // 2):
+        th[:, i] = freq_scale * theta
+        theta = (theta * theta_scale).astype(np.float32)
+    cosf, sinf = _libm.cosf, _libm.sinf
+    c = np.array([cosf(float(t)) for t in th.ravel()], np.float32).reshape(th.shape)[inv][:, None, :]
+    s = np.array([sinf(float(t)) for t in th.ravel()], np.float32).reshape(th.shape)[inv][:, None, :]
+    x0, x1 = x[..., 0::2], x[..., 1::2]
+    out = np.empty_like(x)
+    out[..., 0::2] = _fmaf(x0, c, -(x1 * s))
+    out[..., 1::2] = _fmaf(x0, s, x1 * c)
     return out
 
 
@@ -91,6 +129,89 @@ def soft_max_f16table(s):
     s = np.asarray(s, np.float32)
     e = _f16(np.exp(_f16(s - s.max()).astype(np.float64)))
     return (e * np.float32(1.0 / np.float64(e.astype(np.float64).sum()))).astype(np.float32)
+
+
+SPLIT_KEYS = 256  # positions per context range of the split decode attention (kSplitKeys in csrc/llama.cu)
+
+
+def attention_scores(q, kc, n_past, n_head_kv=None):
+    """Causally masked, scaled K.Q of the ggml attention (llama.cpp:286-302): q [m, n_head, hd] fp32 (rotated), kc [n_head_kv,
+    >= n_past + m, hd] fp16 -> s [n_head, m, n_past + m] fp32, -inf on masked keys.  q is rounded to fp16 and each dot product of
+    fp16 values is summed in double, then rounded to fp32 (the reference sums in fp32; only that order differs), then scaled
+    in fp32.  Query heads h share kv head h // (n_head / n_head_kv) (ne_mul_mat's broadcast)."""
+    q = _f16(q)
+    m, H, hd = q.shape
+    HK = kc.shape[0] if n_head_kv is None else n_head_kv
+    L = n_past + m
+    scale = np.float32(1.0) / np.float32(np.sqrt(np.float32(hd)))
+    s = np.empty((H, m, L), np.float32)
+    for h in range(H):
+        k = np.asarray(kc[h // (H // HK), :L], np.float64)
+        s[h] = (q[:, h, :].astype(np.float64) @ k.T).astype(np.float32) * scale
+    s[:, np.arange(L)[None, :] > n_past + np.arange(m)[:, None]] = -np.inf
+    return s
+
+
+def attend_reference(s, v):
+    """soft_max_f16table of every row of s [..., L] (-inf = masked), p rounded to fp16, V.P summed in double -> fp32:
+    v [L, hd] fp16 values -> [..., hd]"""
+    s = np.asarray(s, np.float32)
+    mx = s.max(axis=-1, keepdims=True)
+    e = _f16(np.exp(_f16(s - mx).astype(np.float64)))
+    inv = (1.0 / e.astype(np.float64).sum(axis=-1, keepdims=True)).astype(np.float32)
+    p = _f16((e * inv).astype(np.float32))
+    return (p.astype(np.float64) @ np.asarray(v, np.float64)).astype(np.float32)
+
+
+def attend_stated(s, v, kind, ranges=SPLIT_KEYS):
+    """The arithmetic the deviating kernels state (DESIGN.md section 4), for scores s [..., L] and v [L, hd]:
+      "mma"    e = fp16(exp(fp16(s - max))), out = (sum e V) / (sum e): the division after the V product, p never rounded
+      "split"  per context range [r * ranges, r * ranges + ranges): its own max m_r, e_r as above, l_r = sum e_r,
+               o_r = sum e_r V; merged as sum_r w_r o_r / sum_r w_r l_r with w_r = exp(m_r - max_r m_r) in fp32.
+               One range: exactly the reference order."""
+    s = np.asarray(s, np.float32)
+    v = np.asarray(v, np.float64)
+    L = s.shape[-1]
+    if kind == "mma" or (kind == "split" and L <= ranges):
+        if kind == "split":
+            return attend_reference(s, v)
+        mx = s.max(axis=-1, keepdims=True)
+        e = _f16(np.exp(_f16(s - mx).astype(np.float64))).astype(np.float64)
+        return ((e @ v) / e.sum(axis=-1, keepdims=True)).astype(np.float32)
+    assert kind == "split", kind
+    parts = []
+    for r0 in range(0, L, ranges):
+        sr = s[..., r0:r0 + ranges]
+        mr = sr.max(axis=-1, keepdims=True)
+        e = _f16(np.exp(_f16(sr - mr).astype(np.float64))).astype(np.float64)
+        parts.append((mr, e.sum(axis=-1, keepdims=True), e @ v[r0:r0 + ranges]))
+    gm = np.max(np.concatenate([p[0] for p in parts], axis=-1), axis=-1, keepdims=True)
+    w = [np.exp((p[0] - gm).astype(np.float32)).astype(np.float64) for p in parts]
+    num = sum(wi * p[2] for wi, p in zip(w, parts))
+    den = sum(wi * p[1] for wi, p in zip(w, parts))
+    return (num / den).astype(np.float32)
+
+
+def _attention(q, kc, vc, n_past, fn):
+    q = np.asarray(q, np.float32)
+    m, H, hd = q.shape
+    HK = kc.shape[0]
+    s = attention_scores(q, kc, n_past)
+    out = np.empty((m, H, hd), np.float32)
+    for h in range(H):
+        out[:, h, :] = fn(s[h], vc[h // (H // HK), :n_past + m])
+    return out
+
+
+def attention_reference(q, kc, vc, n_past):
+    """The reference's causal attention (llama.cpp:286-302, ne_diag_mask_inf past n_past + t) in its own order, vectorised:
+    q [m, n_head, hd] fp32 rotated, kc / vc [n_head_kv, >= n_past + m, hd] fp16 caches holding the new rows -> [m, n_head, hd]."""
+    return _attention(q, kc, vc, n_past, attend_reference)
+
+
+def attention_stated(q, kc, vc, n_past, kind):
+    """attention_reference's inputs through attend_stated(kind): "mma" (prompt kernel) or "split" (decode kernel, m = 1)"""
+    return _attention(q, kc, vc, n_past, lambda s, v: attend_stated(s, v, kind))
 
 
 def rms_norm(x, eps):

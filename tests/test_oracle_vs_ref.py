@@ -188,6 +188,16 @@ def test_llama_rope_mode0_bit_exact(hd):
     x = r.normal(0, 1, (2, 3, hd)).astype(np.float32)
     golden.check(f"rope[{hd}-2tok]", np.stack([lm.rope_mode0(x[t], 10 + t, hd) for t in range(2)]),
                  lambda: _ref_inplace(ref_n.ref_ne_rope, x, hd, 3, 2, 10, 10000.0, 1.0), N)
+    # Llama-3's base and both directions of the scale, out to 8191: the reference's last argument is hparams.freq_scale, whose
+    # inverse multiplies the angle (ne_layers.c:9263, 9207) -- rope_scale means the same
+    for base, scale in ((500000.0, 1.0), (10000.0, 0.25), (10000.0, 4.0), (500000.0, 0.25), (500000.0, 4.0)):
+        for pos in (1, 255, 4095, 8191):
+            x = r.normal(0, 1, (3, hd)).astype(np.float32)
+            golden.check(f"rope[{hd}-{pos}-{base:g}-{scale:g}]", lm.rope_mode0(x, pos, hd, base, scale),
+                         lambda: _ref_inplace(ref_n.ref_ne_rope, x.reshape(1, 3, hd), hd, 3, 1, pos, base, scale)[0], N)
+        x = r.normal(0, 1, (4, 3, hd)).astype(np.float32)
+        golden.check(f"rope[{hd}-4tok-8188-{base:g}-{scale:g}]", lm.rope_mode0_rows(x, 8188 + np.arange(4), hd, base, scale),
+                     lambda: _ref_inplace(ref_n.ref_ne_rope, x, hd, 3, 4, 8188, base, scale), N)
 
 
 def test_llama_softmax_and_rms_norm_bit_exact():
