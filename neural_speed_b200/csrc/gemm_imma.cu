@@ -25,7 +25,7 @@
 #include <cuda.h>
 
 #include "nsb.cuh"
-#include "quant_smem.cuh"
+#include "act_quant.cuh"
 
 namespace {
 
@@ -134,9 +134,9 @@ __device__ __forceinline__ void imma0(int (&c)[4], const uint32_t (&a)[4], uint3
 __device__ __forceinline__ float i2f_small(int i) { return __int_as_float(i + 0x4B400000) - 12582912.f; }
 
 // ---- activation image ------------------------------------------------------------------------------------------------
-// One warp per (token, activation block).  Same arithmetic as act_quant_kernel<COMP> (act_prep.cu) -- bit-exact codes, scales,
-// zero points -- different destination: per K-slice of 256, [8 chunks][MT tokens][32 B] codes then [8][MT] {scale, S|za<<16}
-// where S is the sum of the codes of the WHOLE activation block (the matmul corrects per block, not per chunk).
+// One warp per (token, activation block), arithmetic of act_quant.cuh -- bit-exact codes, scales, zero points -- into the
+// image of this kernel: per K-slice of 256, [8 chunks][MT tokens][32 B] codes then [8][MT] meta words, where Sa is the sum of
+// the codes of the WHOLE activation block (the matmul corrects per block, not per chunk).
 // Tokens >= M and chunks past K are written as zeros (scale 0): they contribute nothing.  Block 0 also clears the tickets.
 template <int COMP>
 __global__ void __launch_bounds__(256) act_quant_imma_kernel(const float* __restrict__ A, int lda, int M, int K, int qg, int MT, int nslices,
@@ -157,8 +157,7 @@ __global__ void __launch_bounds__(256) act_quant_imma_kernel(const float* __rest
   const float* row = A + (size_t)(live ? m : 0) * lda;
   const int kend = min(k0 + qg, K);
 
-  float vmax = (COMP == NS_COMP_Q8_0) ? 0.f : 1.17549435e-38f, vmin = 0.f;
-  if (COMP == NS_COMP_INT8 && live && k0 + qg > K) vmax = 0.f;  // partial block: as act_quant_kernel
+  float vmax = nsq::range_start<COMP>(k0 + qg > K), vmin = 0.f;
   float v[8];
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
@@ -167,57 +166,31 @@ __global__ void __launch_bounds__(256) act_quant_imma_kernel(const float* __rest
       const int k = k0 + c * 32 + lane;
       if (live && k < kend) {
         v[c] = row[k];
-        if (COMP == NS_COMP_INT8) {
-          vmax = fmaxf(v[c], vmax);
-          vmin = fminf(v[c], vmin);
-        } else {
-          vmax = fmaxf(vmax, fabsf(v[c]));
-        }
+        nsq::range_fold<COMP>(v[c], vmax, vmin);
       }
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    vmax = fmaxf(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
-    if (COMP == NS_COMP_INT8) vmin = fminf(vmin, __shfl_xor_sync(0xffffffffu, vmin, o));
-  }
-  float scale, rscale;
-  int za = 0;
-  if (COMP == NS_COMP_Q8_0) {
-    scale = __half2float(__float2half_rn(vmax / 127.f));
-    rscale = vmax != 0.f ? 127.f / vmax : 0.f;
-  } else if (COMP == NS_COMP_INT8) {
-    scale = (vmax - vmin) / 255;
-    za = nsq::cast_u8((0 - vmin) / scale);
-    rscale = 1.f / scale;
-  } else {
-    scale = vmax / 127;
-    rscale = 1.f / scale;
-  }
+  nsq::range_reduce<COMP>(vmax, vmin, 32);
+  nsq::BlockQuant bq = nsq::block_quant<COMP>(vmax, vmin);
   int q[8], stot = 0;
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
     q[c] = 0;
     if (c < cpb) {
       const int k = k0 + c * 32 + lane;
-      if (live && k < kend) {
-        if (COMP == NS_COMP_Q8_0) q[c] = __float2int_rn(v[c] * rscale);
-        else if (COMP == NS_COMP_INT8) q[c] = nsq::cast_u8((float)za + (float)(int)roundf(v[c] * rscale));
-        else q[c] = nsq::cast_s8(v[c] * rscale);
-      } else if (live) {
-        q[c] = za;  // padding inside a live block contributes (a - za) == 0
-      }
+      if (live && k < kend) q[c] = nsq::quant_code<COMP>(v[c], bq);
+      else if (live) q[c] = bq.za;  // padding inside a live block
       stot += q[c];
     }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) stot += __shfl_xor_sync(0xffffffffu, stot, o);
   if (!live) {
-    scale = 0.f;
-    za = 0;
+    bq.scale = 0.f;
+    bq.za = 0;
     stot = 0;
   }
-  const int pos = (lane & ~7) | (((lane & 3) << 1) | ((lane & 7) >> 2));  // byte order of the dp4a / MMA operands (nsb.cuh)
+  const int pos = (lane & ~7) | nsq::dp4a_pos(lane & 7);
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
     if (c < cpb) {
@@ -225,9 +198,7 @@ __global__ void __launch_bounds__(256) act_quant_imma_kernel(const float* __rest
       uint8_t* sl = img + (size_t)(ch >> 3) * slice_bytes;
       const int j = ch & 7;
       sl[(size_t)j * MT * 32 + (size_t)m * 32 + pos] = (uint8_t)q[c];
-      if (lane == 0)
-        *reinterpret_cast<int2*>(sl + (size_t)MT * 256 + ((size_t)j * MT + m) * 8) =
-            make_int2(__float_as_int(scale), (stot & 0xffff) | (za << 16));
+      if (lane == 0) *reinterpret_cast<int2*>(sl + (size_t)MT * 256 + ((size_t)j * MT + m) * 8) = nsq::meta_word(bq.scale, stot, bq.za);
     }
   }
 }
