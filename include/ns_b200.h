@@ -324,6 +324,19 @@ NS_API int ns_llama_generate(ns_llama* ctx, int32_t first_token, int n_past, int
  * models of tests/test_gpu_llama.py, KV cache entries differ at bf16 precision).  on = 1 evaluates long prompts in pieces of 32
  * tokens instead: reference numerics for the whole prompt at about 1/6 of the prefill throughput. */
 NS_API int ns_llama_set_exact_prefill(ns_llama* ctx, int on);
+/* Generation past n_ctx: the StreamingLLM ring of the reference's shift-RoPE-K mode (model_context.shift_roped_k / n_keep,
+ * models/llama/llama.cpp:102-107, 351-354, 430-470).  0 <= n_keep < n_ctx enables it with n_keep attention-sink slots, -1
+ * disables it.  With it on, n_past is the number of tokens evaluated so far (the reference's n_total) and may reach or pass n_ctx
+ * for one-token steps (ns_llama_eval with n_tokens = 1, ns_llama_generate for any n_new).  Once the cache is full, the new token's
+ * K / V go to slot n_keep + (n_total - n_ctx) mod (n_ctx - n_keep) -- the sinks are never overwritten -- every cached key at or
+ * past n_keep is rotated one position back in the fp16 cache (the reference's fp16 arithmetic, rounding included), and attention
+ * covers all n_ctx slots without a mask.  Steps that stay inside n_ctx are bit-identical to a context without streaming.
+ *   NS_E_UNSUPPORTED  rope_scale != 1 (the reference divides positions by freq_scale but builds its shift table from freq_scale
+ *                     undivided, so the two disagree), or a head size other than 64 / 128
+ *   ns_llama_eval then returns NS_E_UNSUPPORTED for n_tokens > 1 with n_past + n_tokens > n_ctx (the reference's mask is
+ *   meaningless in ring order, llama.cpp:467), and, once a step has passed n_ctx, NS_E_INVALID for any n_past other than the next
+ *   position or a restart at n_past <= n_keep.  Enabling or disabling drops the captured decode graph. */
+NS_API int ns_llama_set_streaming(ns_llama* ctx, int n_keep);
 NS_API unsigned long long ns_llama_kv_bytes(const ns_llama* ctx);
 /* One layer's attention of the eval step on its own, for parity tests: RoPE (mode 0, angle = p * rope_theta^(-2i/hd) / rope_scale)
  * of q [m][n_head * hd] in place and of the m new rows k [m][n_head_kv * hd] at positions n_past .. n_past + m - 1, k and v appended
@@ -346,6 +359,13 @@ NS_API size_t ns_llama_attention_workspace_bytes(int n_head, int hd, int n_ctx);
 NS_API int ns_llama_attention(int kernel, float* q, const float* k, const float* v, void* kc, void* vc, int n_head, int n_head_kv,
                               int hd, int n_ctx, int n_past, int m, float rope_theta, float rope_scale, float* out, void* ws,
                               void* queue);
+/* One layer's single-token step of the streaming ring (ns_llama_set_streaming) on its own, for parity tests: n_total tokens
+ * evaluated before this one, n_keep sink slots, rope_scale 1.  While n_total < n_ctx it is the one-row step of ns_llama_attention;
+ * after that q is rotated at n_ctx - 1, the new k at n_ctx, k / v stored in the ring slot, every cached key at or past n_keep
+ * shifted one position back in place, and out covers all n_ctx slots.  Same workspace and argument rules as ns_llama_attention;
+ * NS_E_UNSUPPORTED (nothing launched) for head sizes other than 64 / 128. */
+NS_API int ns_llama_attention_ring(float* q, const float* k, const float* v, void* kc, void* vc, int n_head, int n_head_kv, int hd,
+                                   int n_ctx, int n_keep, int n_total, float rope_theta, float* out, void* ws, void* queue);
 
 /* ---- tensor-parallel exchange step over NVLink peer memory (SURVEY 8e) --------------------------------------------
  * One-shot sum all-reduce replacing reduce_add / ne_all_reduce (core/parallel_context.cpp:47, ne_layers.c:5466) for the

@@ -59,7 +59,7 @@ EXPORTS = [
     "ns_device_quantize_q4_0", "ns_device_quantize_act",
     "BTLAGemmPackBSize", "BTLAGemmQuantPackB", "BTLAGemmPackB", "BTLAGemmUnPackB", "ns_quantize_row_q4_0", "ns_split_weight_size", "ns_split_weight",
     "ns_llama_create", "ns_llama_free", "ns_llama_set_f32", "ns_llama_set_weight", "ns_llama_eval", "ns_llama_generate", "ns_llama_set_exact_prefill",
-    "ns_llama_kv_bytes", "ns_llama_attention_workspace_bytes", "ns_llama_attention",
+    "ns_llama_set_streaming", "ns_llama_kv_bytes", "ns_llama_attention_workspace_bytes", "ns_llama_attention", "ns_llama_attention_ring",
     "ns_comm_handle_bytes", "ns_comm_create", "ns_comm_get_handle", "ns_comm_open_peers", "ns_comm_link_local", "ns_comm_all_reduce_f32",
     "ns_comm_status", "ns_comm_free",
 ]
@@ -184,6 +184,8 @@ def lib() -> C.CDLL:
     L.ns_llama_attention_workspace_bytes.restype = sz
     L.ns_llama_attention_workspace_bytes.argtypes = [i, i, i]
     L.ns_llama_attention.argtypes = [i, vp, vp, vp, vp, vp, i, i, i, i, i, i, C.c_float, C.c_float, vp, vp, vp]
+    L.ns_llama_attention_ring.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, i, i, C.c_float, vp, vp, vp]
+    L.ns_llama_set_streaming.argtypes = [vp, i]
     L.ns_comm_handle_bytes.restype = sz
     L.ns_comm_create.restype = vp
     L.ns_comm_create.argtypes = [i, i, sz, vp]
@@ -490,6 +492,11 @@ class Llama:
     def set_exact_prefill(self, on: bool = True):
         """prompts longer than 32 tokens in pieces of 32: the reference's integer block sums instead of the bf16 tensor-core GEMM"""
         _check(lib().ns_llama_set_exact_prefill(self.h, 1 if on else 0), "ns_llama_set_exact_prefill")
+
+    def set_streaming(self, n_keep: int):
+        """Generate past n_ctx through the StreamingLLM ring with n_keep attention-sink slots (-1: off); n_past then counts every
+        token evaluated so far (include/ns_b200.h, ns_llama_set_streaming)"""
+        _check(lib().ns_llama_set_streaming(self.h, n_keep), "ns_llama_set_streaming")
 
     def close(self):
         if self.h:

@@ -380,6 +380,14 @@ __global__ void __launch_bounds__(kAW * 32) attn_fast_kernel(const float* __rest
 // p = fp16(e / sum), fp32 sums).  Several: every CTA leaves {max, sum e, sum e V} of its range, the last one to arrive (ticket per
 // head) merges them with exp(max_s - max) weights -- same values up to the fp16 rounding of p (measured: tests/test_gpu_attention.py).
 // Bound: latency at short contexts; HBM (2 x len x hd x 2 B per kv head) at long ones, spread over n_head x ceil(len / 256) CTAs.
+//
+// RING = true: the StreamingLLM ring of the reference's shift-RoPE-K mode (llama.cpp:102-107, 351-354, 430-470), grid
+// (n_head_kv, ranges).  One CTA per (kv head, range) serves every query head of its group from the one staged tile, so no two CTAs
+// of a launch touch the same K row.  Until the cache is full (state[1] < n_ctx) each head's arithmetic is the RING = false
+// kernel's.  Once it is full, with n_total = state[1]: q is rotated at n_ctx - 1, the new k at n_ctx (fp32, then fp16) and stored
+// with v in slot n_keep + (n_total - n_ctx) mod (n_ctx - n_keep), inside whichever range holds it; then every staged K row at or
+// past n_keep, the new one included, is rotated one position back with the fp16 shift table (ne_layers.c:9514-9526), scored
+// and written back with one bulk store; attention covers all n_ctx slots with no mask.
 constexpr int kSplitKeys = 256;
 constexpr int kDW = 16;  // warps per CTA
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -387,12 +395,16 @@ template <int HD>
 static constexpr size_t attn_decode_smem() {
   return (size_t)2 * kSplitKeys * HD * 2 + (size_t)(3 + kDW) * HD * 4 + (size_t)(kSplitKeys + 8) * 4 + 16;
 }
-template <int HD>
+// {cos, sin} of the one-position back shift per rotary pair, fp16 (model_utils.cpp:165-192); passed by value
+struct ShiftTable {
+  __half2 cs[64];
+};
+template <int HD, bool RING>
 __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __restrict__ q, const float* __restrict__ knew,
                                                             const float* __restrict__ vnew, __half* __restrict__ kc, __half* __restrict__ vc,
                                                             const int* __restrict__ state, float* __restrict__ out, float* __restrict__ part_ws,
                                                             unsigned* __restrict__ tickets, int n_head, int n_head_kv, int n_ctx, int nsplit,
-                                                            float scale, float theta_scale, float freq_scale) {
+                                                            float scale, float theta_scale, float freq_scale, int n_keep, const ShiftTable tab) {
   constexpr int EPL = HD / 32;
   extern __shared__ __align__(128) unsigned char smraw[];
   __half* Kt = reinterpret_cast<__half*>(smraw);  // [kSplitKeys][HD]
@@ -410,15 +422,21 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   // The position was written by the PREVIOUS token's argmax kernel (an earlier graph launch / an H2D copy ahead of this eval's
   // first kernel), never by a kernel of this token: it may be read before griddepcontrol.wait.  CTAs whose range the sequence
   // has not reached leave at once, without holding 141 KB of an SM until the Q/K/V launch in front of this one has drained.
-  const int h = blockIdx.x, split = blockIdx.y;
-  const int group = n_head / n_head_kv, hk = h / group;
+  const int split = blockIdx.y;
+  const int group = n_head / n_head_kv;
+  const int hk = RING ? (int)blockIdx.x : (int)blockIdx.x / group;
+  const int h0 = RING ? hk * group : (int)blockIdx.x;  // query heads h0 .. h0 + nh - 1
+  const int nh = RING ? group : 1;
   const int pos = state[1];
+  const bool wrapped = RING && pos >= n_ctx;
   const int len = min(pos + 1, n_ctx);
   const int nact = (len + kSplitKeys - 1) / kSplitKeys;
   if (split >= nact) return;
   const int i0 = split * kSplitKeys, i1 = min(len, i0 + kSplitKeys);
-  const bool has_new = (i1 == len) && pos < n_ctx;  // the token being evaluated sits in this range: its k / v come from registers
-  const int ncache = (has_new ? i1 - 1 : i1) - i0;  // rows read from the cache
+  const int slot = wrapped ? n_keep + (pos - n_ctx) % (n_ctx - n_keep) : pos;  // cache row of the token being evaluated
+  const bool has_new = wrapped ? slot >= i0 && slot < i1 : (i1 == len) && pos < n_ctx;  // ... sits in this range
+  const bool tail_new = has_new && !wrapped;  // ... after the staged rows, its k / v from registers (else staged over its slot)
+  const int ncache = (tail_new ? i1 - 1 : i1) - i0;  // rows staged from the cache
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   __half* kh = kc + (size_t)hk * n_ctx * HD;
   __half* vh = vc + (size_t)hk * n_ctx * HD;
@@ -427,7 +445,9 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar_a), "r"(1) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     // the cached rows of this range were written by earlier tokens' launches: their copies start before the wait as well and
-    // overlap the tail of the Q/K/V launch
+    // overlap the tail of the Q/K/V launch.  In the ring, the rows this token rewrites (shifted K, the new K / V slot) were
+    // likewise last written by this layer's launch of the previous token -- the launch whose appended row the plain step
+    // already reads here -- so the same ordering covers them.
     if (ncache > 0) {
       const uint32_t bytes = (uint32_t)ncache * HD * 2;
       asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(2 * bytes) : "memory");
@@ -441,39 +461,13 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   }
   __syncthreads();
   pdl_wait();  // q, k, v of the new token come from the launch in front
-  // RoPE of this head's q (every range needs it) and of the new k row; KV append by one CTA per kv head -- while the copies fly
-  if (threadIdx.x < HD / 2) {
-    const int i = threadIdx.x;
-    float theta = (float)pos;
+  auto rope_angle = [&](int p, int i, float* sn, float* cs) {
+    float theta = (float)p;
     for (int j = 0; j < i; ++j) theta *= theta_scale;  // ne_layers.c:9385: same sequence of roundings
     theta *= freq_scale;
-    float sn, cs;
-    sincosf(theta, &sn, &cs);
-    const float* qr = q + (size_t)h * HD;
-    const float q0 = qr[2 * i], q1 = qr[2 * i + 1];
-    sq[2 * i] = __half2float(__float2half_rn(q0 * cs - q1 * sn));
-    sq[2 * i + 1] = __half2float(__float2half_rn(q0 * sn + q1 * cs));
-    if (has_new) {
-      const float* kr = knew + (size_t)hk * HD;
-      const float k0 = kr[2 * i], k1 = kr[2 * i + 1];
-      const __half r0 = __float2half_rn(k0 * cs - k1 * sn), r1 = __float2half_rn(k0 * sn + k1 * cs);
-      sk[2 * i] = __half2float(r0);
-      sk[2 * i + 1] = __half2float(r1);
-      const float* vr = vnew + (size_t)hk * HD;
-      const __half w0 = __float2half_rn(vr[2 * i]), w1 = __float2half_rn(vr[2 * i + 1]);
-      sv[2 * i] = __half2float(w0);
-      sv[2 * i + 1] = __half2float(w1);
-      if (h % group == 0) {
-        *reinterpret_cast<__half2*>(kh + (size_t)pos * HD + 2 * i) = __halves2half2(r0, r1);
-        *reinterpret_cast<__half2*>(vh + (size_t)pos * HD + 2 * i) = __halves2half2(w0, w1);
-      }
-    }
-  }
-  __syncthreads();
-  float ql[EPL];
-#pragma unroll
-  for (int e = 0; e < EPL; ++e) ql[e] = sq[lane * EPL + e];
-  if (ncache > 0) {
+    sincosf(theta, sn, cs);
+  };
+  auto wait_tiles = [&]() {
     uint32_t ok;
     do {
       asm volatile(
@@ -486,7 +480,75 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
           : "r"(bar_a), "r"(0)
           : "memory");
     } while (!ok);
+  };
+  // RoPE of the new k row; KV append by one CTA per kv head -- while the copies fly
+  float qsn = 0.f, qcs = 0.f;  // the queries' angle (thread i < HD / 2: pair i)
+  __half2 knew_h = __float2half2_rn(0.f), vnew_h = knew_h;
+  if (threadIdx.x < HD / 2) {
+    const int i = threadIdx.x;
+    rope_angle(wrapped ? n_ctx - 1 : pos, i, &qsn, &qcs);  // llama.cpp:351: q at max(n_cached - N, n_past)
+    if (has_new) {
+      float sn = qsn, cs = qcs;
+      if (wrapped) rope_angle(n_ctx, i, &sn, &cs);  // llama.cpp:353-354: the new k enters at n_ctx, shifted back below
+      const float* kr = knew + (size_t)hk * HD;
+      const float k0 = kr[2 * i], k1 = kr[2 * i + 1];
+      const __half r0 = __float2half_rn(k0 * cs - k1 * sn), r1 = __float2half_rn(k0 * sn + k1 * cs);
+      sk[2 * i] = __half2float(r0);
+      sk[2 * i + 1] = __half2float(r1);
+      const float* vr = vnew + (size_t)hk * HD;
+      const __half w0 = __float2half_rn(vr[2 * i]), w1 = __float2half_rn(vr[2 * i + 1]);
+      sv[2 * i] = __half2float(w0);
+      sv[2 * i + 1] = __half2float(w1);
+      knew_h = __halves2half2(r0, r1);
+      vnew_h = __halves2half2(w0, w1);
+      if (!wrapped && (RING || h0 % group == 0)) {
+        *reinterpret_cast<__half2*>(kh + (size_t)pos * HD + 2 * i) = knew_h;
+        *reinterpret_cast<__half2*>(vh + (size_t)pos * HD + 2 * i) = vnew_h;
+      }
+    }
   }
+  const int shift0 = wrapped ? min(max(n_keep - i0, 0), ncache) : ncache;  // staged rows [shift0, ncache) are shifted
+  if (wrapped) {
+    wait_tiles();
+    if (has_new && threadIdx.x < HD / 2) {  // the new row goes over its slot (write before shift: llama.cpp:408-409, :443)
+      reinterpret_cast<__half2*>(Kt + (size_t)(slot - i0) * HD)[threadIdx.x] = knew_h;
+      reinterpret_cast<__half2*>(Vt + (size_t)(slot - i0) * HD)[threadIdx.x] = vnew_h;
+      reinterpret_cast<__half2*>(vh + (size_t)slot * HD)[threadIdx.x] = vnew_h;
+    }
+    __syncthreads();
+    // blockDim.x is a multiple of HD / 2: a thread always meets the same rotary pair
+    const float2 t = __half22float2(tab.cs[threadIdx.x % (HD / 2)]);
+    __half2* kt2 = reinterpret_cast<__half2*>(Kt);
+    for (int e = shift0 * (HD / 2) + threadIdx.x; e < ncache * (HD / 2); e += blockDim.x) {
+      const float2 x = __half22float2(kt2[e]);
+      // x0*cos - x1*sin, x1*cos + x0*sin (ne_layers.c:9524-9525): the products of two fp16 values are exact in fp32, so this
+      // form rounds once per output, as every contraction of the reference's expressions does
+      kt2[e] = __floats2half2_rn(fmaf(x.x, t.x, -(x.y * t.y)), fmaf(x.y, t.x, x.x * t.y));
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the shifted rows, visible to the bulk store
+    __syncthreads();
+    if (threadIdx.x == 0 && shift0 < ncache) {
+      asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(kh + (size_t)(i0 + shift0) * HD),
+                   "r"(smem_addr(Kt + (size_t)shift0 * HD)), "r"((uint32_t)(ncache - shift0) * HD * 2)
+                   : "memory");
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+  }
+  for (int hi = 0; hi < nh; ++hi) {
+  const int h = h0 + hi;
+  if (threadIdx.x < HD / 2) {  // RoPE of this head's q (every range needs it)
+    const int i = threadIdx.x;
+    const float sn = qsn, cs = qcs;
+    const float* qr = q + (size_t)h * HD;
+    const float q0 = qr[2 * i], q1 = qr[2 * i + 1];
+    sq[2 * i] = __half2float(__float2half_rn(q0 * cs - q1 * sn));
+    sq[2 * i + 1] = __half2float(__float2half_rn(q0 * sn + q1 * cs));
+  }
+  __syncthreads();
+  float ql[EPL];
+#pragma unroll
+  for (int e = 0; e < EPL; ++e) ql[e] = sq[lane * EPL + e];
+  if (ncache > 0) wait_tiles();
   auto row = [&](const __half* base, int r, float* dst) {
     if (EPL == 4) {
       const uint2 u = *reinterpret_cast<const uint2*>(base + (size_t)r * HD + lane * 4);
@@ -507,7 +569,7 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
     acc = warp_sum(acc);
     if (lane == 0) sc[r] = acc * scale;
   }
-  if (has_new && warp == kDW - 1) {
+  if (tail_new && warp == kDW - 1) {
     float acc = 0.f;
 #pragma unroll
     for (int e = 0; e < EPL; ++e) acc = fmaf(ql[e], sk[lane * EPL + e], acc);
@@ -515,7 +577,7 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
     if (lane == 0) sc[ncache] = acc * scale;
   }
   __syncthreads();
-  const int nloc = ncache + (has_new ? 1 : 0);
+  const int nloc = ncache + (tail_new ? 1 : 0);
   float lmax = -INFINITY;
   for (int i = threadIdx.x; i < nloc; i += blockDim.x) lmax = fmaxf(lmax, sc[i]);
 #pragma unroll
@@ -560,7 +622,7 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
 #pragma unroll
     for (int e = 0; e < EPL; ++e) acc[e] = fmaf(p, vr[e], acc[e]);
   }
-  if (has_new && warp == kDW - 1) {
+  if (tail_new && warp == kDW - 1) {
     const float p = single ? __half2float(__float2half_rn(sc[ncache] * inv)) : sc[ncache];
 #pragma unroll
     for (int e = 0; e < EPL; ++e) acc[e] = fmaf(p, sv[lane * EPL + e], acc[e]);
@@ -575,8 +637,7 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   }
   if (single) {
     if (threadIdx.x < HD) out[(size_t)h * HD + threadIdx.x] = mine;
-    return;
-  }
+  } else {
   // several ranges: leave {sum e V, max, sum e}; the last CTA of the head merges
   float* mypart = part_ws + ((size_t)h * nsplit + split) * (HD + 2);
   if (threadIdx.x < HD) mypart[threadIdx.x] = mine;
@@ -588,7 +649,7 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   __syncthreads();
   if (threadIdx.x == 0) last_flag = (atomicAdd(&tickets[h], 1u) == (unsigned)(nact - 1)) ? 1 : 0;
   __syncthreads();
-  if (!last_flag) return;
+  if (last_flag) {
   __threadfence();
   if (threadIdx.x < HD) {
     const float* base = part_ws + (size_t)h * nsplit * (HD + 2);
@@ -603,6 +664,12 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
     out[(size_t)h * HD + threadIdx.x] = num / den;
   }
   if (threadIdx.x == 0) tickets[h] = 0u;  // ready for the next launch (graph replay)
+  }
+  }
+  if (RING) __syncthreads();  // sq, sc, part and the reduction slots serve the next query head
+  }
+  // the bulk store reads the shifted rows out of shared memory: it must be complete before the CTA exits
+  if (wrapped && threadIdx.x == 0 && shift0 < ncache) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 // ---- prompt attention on the tensor cores ------------------------------------------------------------------------------------
@@ -890,11 +957,30 @@ static int attn_resolve(int kind, int hd, int m, int n_ctx) {
   return kind;
 }
 
+// The fp16 table that shifts a cached key one position back (model_utils.cpp:165-192 with freq_scale 1): theta starts at -1 and
+// is multiplied by freq_base^(-2 / hd) per pair in fp32; cos and sin come from the host libm, as in the reference.
+static ShiftTable shift_table(int hd, float freq_base) {
+  ShiftTable t{};
+  const float theta_scale = std::pow(freq_base, -2.0f / hd);
+  float theta = -1.0f;
+  for (int i = 0; i < hd / 2; ++i) {
+    t.cs[i] = __halves2half2(__float2half_rn(std::cos(theta)), __float2half_rn(std::sin(theta)));
+    theta *= theta_scale;
+  }
+  return t;
+}
+
 // part: [n_head][attn_ranges(n_ctx)][hd + 2] floats, tickets: [n_head] zero words (both read by attn_decode_kernel only; the
-// last CTA of a head leaves its ticket at zero again)
+// last CTA of a head leaves its ticket at zero again).  ring (nullable): one-token steps run the ring variant of the split decode
+// attention with ring->n_keep sink slots; prompts (m > 1, which never reach past n_ctx) run the plain kernels.
+struct Ring {
+  int n_keep;
+  ShiftTable tab;
+};
 static int launch_attention(int kind, float* q, const float* k, const float* v, __half* kc, __half* vc, const int* state, float* out,
                             float* part, unsigned* tickets, int n_head, int n_head_kv, int hd, int n_ctx, int m, float rope_theta,
-                            float rope_scale, AttnAttr& attr, cudaStream_t st) {
+                            float rope_scale, AttnAttr& attr, cudaStream_t st, const Ring* ring = nullptr) {
+  if (ring && m == 1) kind = NS_ATTN_SPLIT_DECODE;  // the only kernel that carries the shift
   kind = attn_resolve(kind, hd, m, n_ctx);
   if (kind < 0) return kind;
   const int ldq = n_head * hd, ldk = n_head_kv * hd;
@@ -912,15 +998,20 @@ static int launch_attention(int kind, float* q, const float* k, const float* v, 
   if (kind == NS_ATTN_SPLIT_DECODE) {
     // rope + KV append + attention in one launch, K / V staged by TMA, the context split over CTAs
     if (!attr.decode) {
-      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<128>()));
-      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<64>()));
+      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<128>()));
+      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<64>()));
+      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<128>()));
+      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<64>()));
       attr.decode = true;
     }
     const int nsplit = attn_ranges(n_ctx);
     const size_t dsm = hd == 128 ? attn_decode_smem<128>() : attn_decode_smem<64>();
-    auto kern = hd == 128 ? attn_decode_kernel<128> : attn_decode_kernel<64>;
-    NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)n_head, (unsigned)nsplit), dim3(kDW * 32), dsm, st, (const float*)q, k, v, kc, vc, state,
-                              out, part, tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale, theta_scale, freq_scale));
+    auto kern = ring ? (hd == 128 ? attn_decode_kernel<128, true> : attn_decode_kernel<64, true>)
+                     : (hd == 128 ? attn_decode_kernel<128, false> : attn_decode_kernel<64, false>);
+    const unsigned gx = (unsigned)(ring ? n_head_kv : n_head);  // ring: one CTA per (kv head, range)
+    NS_CUDA_TRY(ns_launch_pdl(kern, dim3(gx, (unsigned)nsplit), dim3(kDW * 32), dsm, st, (const float*)q, k, v, kc, vc, state, out, part,
+                              tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale, theta_scale, freq_scale, ring ? ring->n_keep : -1,
+                              ring ? ring->tab : ShiftTable{}));
     ns_count_launch();
     return NS_OK;
   }
@@ -988,6 +1079,28 @@ extern "C" int ns_llama_attention(int kernel, float* q, const float* k, const fl
                           rope_scale, attr, st);
 }
 
+extern "C" int ns_llama_attention_ring(float* q, const float* k, const float* v, void* kc, void* vc, int n_head, int n_head_kv, int hd,
+                                       int n_ctx, int n_keep, int n_total, float rope_theta, float* out, void* ws, void* queue) {
+  if (int rc = ns_ensure_device()) return rc;
+  if (!q || !k || !v || !kc || !vc || !out || !ws || n_head <= 0 || n_head_kv <= 0 || n_head % n_head_kv || hd <= 0 || hd % 2 ||
+      n_ctx <= 0 || n_keep < 0 || n_keep >= n_ctx || n_total < 0 || !(rope_theta > 0.f)) {
+    ns_set_error("ns_llama_attention_ring: invalid arguments (n_head=%d n_head_kv=%d hd=%d n_ctx=%d n_keep=%d n_total=%d)", n_head,
+                 n_head_kv, hd, n_ctx, n_keep, n_total);
+    return NS_E_INVALID;
+  }
+  if (int rc = attn_resolve(NS_ATTN_SPLIT_DECODE, hd, 1, n_ctx); rc < 0) return rc;
+  cudaStream_t st = ns_stream_of(queue);
+  char* w = static_cast<char*>(ws);
+  const int state[4] = {0, n_total, 0, 0};
+  NS_CUDA_TRY(cudaMemcpyAsync(w, state, sizeof(state), cudaMemcpyHostToDevice, st));  // pageable source: staged before the call returns
+  AttnAttr attr;
+  const Ring ring{n_keep, shift_table(hd, rope_theta)};
+  return launch_attention(NS_ATTN_SPLIT_DECODE, q, k, v, static_cast<__half*>(kc), static_cast<__half*>(vc), reinterpret_cast<const int*>(w),
+                          out, reinterpret_cast<float*>(w + attn_ws_part_offset(n_head)),
+                          reinterpret_cast<unsigned*>(w + attn_ws_tickets_offset()), n_head, n_head_kv, hd, n_ctx, 1, rope_theta, 1.f, attr,
+                          st, &ring);
+}
+
 struct ns_llama {
   ns_llama_hparams hp;
   cudaStream_t st;
@@ -1009,6 +1122,10 @@ struct ns_llama {
   unsigned* attn_tickets = nullptr;     // [n_head]
   int attn_nsplit = 0;
   int exact_prefill = 0;               // ns_llama_set_exact_prefill
+  bool streaming = false;              // ns_llama_set_streaming: ring.n_keep sink slots, ring.tab the shift table
+  Ring ring{};
+  int n_total = 0;                     // tokens evaluated so far (the n_past a continuation passes)
+  bool wrapped = false;                // a ring step has run since the last restart: only continuations and restarts are valid
   float *x = nullptr, *xn = nullptr, *qkv = nullptr, *attn = nullptr, *tmp = nullptr, *logits = nullptr;
   void* ws = nullptr;
   size_t ws_bytes = 0;
@@ -1228,7 +1345,7 @@ static int check_complete(const ns_llama* c) {
 
 // enqueue the whole forward pass for m new tokens (ids in c->tokens[0..m) or, when from_state, the single id in
 // state[0]); position base = state[1].  Leaves logits of the LAST token in c->logits and the greedy pick in state[3].
-static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int* record) {
+static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int* record, bool ring) {
   const ns_llama_hparams& hp = c->hp;
   cudaStream_t st = c->st;
   const int E = hp.n_embd, hd = E / hp.n_head, kvd = hd * hp.n_head_kv;
@@ -1265,7 +1382,7 @@ static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int
     static const int dbg_skip = getenv("NS_LLAMA_DEBUG_SKIP") ? atoi(getenv("NS_LLAMA_DEBUG_SKIP")) : 0;  // timing experiments only
     if (!(m == 1 && (dbg_skip & 1)))  // (else results are wrong: the attention launch is left out to measure what it costs)
       if (int rc = launch_attention(NS_ATTN_AUTO, q, k, v, kc, vc, c->state, c->attn, c->attn_part, c->attn_tickets, hp.n_head, hp.n_head_kv,
-                                    hd, hp.n_ctx, m, hp.rope_theta, hp.rope_scale, c->attn_attr, st))
+                                    hd, hp.n_ctx, m, hp.rope_theta, hp.rope_scale, c->attn_attr, st, ring ? &c->ring : nullptr))
         return rc;
     // inpFF = wo * attn + inpSA, written over x (every row is read by its own output only after the matmul finished)
     if (int rc = ns_mul_mat_engine(L.wo, c->attn, E, c->xn, E, m, c->x, c->ws, st, nullptr, 0.f)) return rc;
@@ -1298,11 +1415,12 @@ static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int
 static int ensure_decode_graph(ns_llama* c) {
   if (c->decode_exec) return NS_OK;
   // one eager pass (no state advance; it writes the same K/V the real pass will) sets kernel attributes and sizes every
-  // lazily-grown buffer outside the capture, then capture
-  if (int rc = enqueue_forward(c, 1, true, 0, nullptr)) return rc;
+  // lazily-grown buffer outside the capture, then capture.  The eager pass runs the plain attention even when streaming: a
+  // ring step rotates the cache, which must happen once; the plain kernel writes nothing once the cache is full.
+  if (int rc = enqueue_forward(c, 1, true, 0, nullptr, false)) return rc;
   NS_CUDA_TRY(cudaStreamSynchronize(c->st));
   NS_CUDA_TRY(cudaStreamBeginCapture(c->st, cudaStreamCaptureModeThreadLocal));
-  int rc = enqueue_forward(c, 1, true, 1, c->record);
+  int rc = enqueue_forward(c, 1, true, 1, c->record, c->streaming);
   cudaGraph_t g = nullptr;
   cudaError_t e = cudaStreamEndCapture(c->st, &g);
   if (rc) {
@@ -1326,12 +1444,74 @@ extern "C" int ns_llama_set_exact_prefill(ns_llama* c, int on) {
   return NS_OK;
 }
 
+static void drop_decode_graph(ns_llama* c) {
+  if (!c->decode_exec) return;
+  cudaGraphExecDestroy(c->decode_exec);
+  cudaGraphDestroy(c->decode_graph);
+  c->decode_exec = nullptr;
+  c->decode_graph = nullptr;
+}
+
+extern "C" int ns_llama_set_streaming(ns_llama* c, int n_keep) {
+  if (!c || n_keep < -1 || n_keep >= c->hp.n_ctx) {
+    ns_set_error("ns_llama_set_streaming: n_keep %d outside [-1, n_ctx)", n_keep);
+    return NS_E_INVALID;
+  }
+  const int hd = c->hp.n_embd / c->hp.n_head;
+  if (n_keep >= 0 && c->hp.rope_scale != 1.f) {
+    ns_set_error("ns_llama_set_streaming: rope_scale %g != 1 (the reference's positions and shift table disagree)", c->hp.rope_scale);
+    return NS_E_UNSUPPORTED;
+  }
+  if (n_keep >= 0 && hd != 64 && hd != 128) {
+    ns_set_error("ns_llama_set_streaming: head size %d (the shift rides in the split decode attention: 64 or 128)", hd);
+    return NS_E_UNSUPPORTED;
+  }
+  NS_CUDA_TRY(cudaStreamSynchronize(c->st));  // nothing in flight replays the graph dropped below
+  drop_decode_graph(c);
+  c->streaming = n_keep >= 0;
+  c->ring = Ring{n_keep, c->streaming ? shift_table(hd, c->hp.rope_theta) : ShiftTable{}};
+  c->wrapped = false;
+  return NS_OK;
+}
+
+// Positions of a streaming context: n_past is n_total.  Steps that reach past n_ctx take one token and continue the sequence;
+// once such a step has run, only a continuation or a restart inside the sinks (n_past <= n_keep) is meaningful.
+static int check_streaming(ns_llama* c, const char* who, int n_past, int n) {
+  const int n_ctx = c->hp.n_ctx;
+  if (!c->streaming) {
+    if (n_past + n > n_ctx) {
+      ns_set_error("%s: invalid arguments (n_tokens=%d n_past=%d n_ctx=%d)", who, n, n_past, n_ctx);
+      return NS_E_INVALID;
+    }
+    return NS_OK;
+  }
+  const bool cont = n_past == c->n_total;
+  if ((c->wrapped && !cont && n_past > c->ring.n_keep) || (n_past >= n_ctx && !cont)) {
+    ns_set_error("%s: n_past %d is neither the next position %d nor a restart at <= n_keep %d of the full ring", who, n_past,
+                 c->n_total, c->ring.n_keep);
+    return NS_E_INVALID;
+  }
+  return NS_OK;
+}
+
+// the sequence position after a successful call
+static void advance_position(ns_llama* c, int n_past, int n) {
+  c->n_total = n_past + n;
+  c->wrapped = c->streaming && ((c->wrapped && n_past > c->ring.n_keep) || n_past + n > c->hp.n_ctx);
+}
+
 extern "C" int ns_llama_eval(ns_llama* c, const int32_t* tokens, int n_tokens, int n_past, float* logits_host, int32_t* next_token) {
   if (int rc = ns_ensure_device()) return rc;
-  if (!c || !tokens || n_tokens <= 0 || n_past < 0 || n_past + n_tokens > c->hp.n_ctx) {
+  if (!c || !tokens || n_tokens <= 0 || n_past < 0) {
     ns_set_error("ns_llama_eval: invalid arguments (n_tokens=%d n_past=%d n_ctx=%d)", n_tokens, n_past, c ? c->hp.n_ctx : 0);
     return NS_E_INVALID;
   }
+  if (c->streaming && n_tokens > 1 && n_past + n_tokens > c->hp.n_ctx) {
+    // the reference masks a multi-token step in slot order, which means nothing in ring order (llama.cpp:467, a TODO there)
+    ns_set_error("ns_llama_eval: %d tokens past n_ctx %d: the ring takes one token per step", n_tokens, c->hp.n_ctx);
+    return NS_E_UNSUPPORTED;
+  }
+  if (int rc = check_streaming(c, "ns_llama_eval", n_past, n_tokens)) return rc;
   if (c->exact_prefill && n_tokens > 32) {
     // parity mode: prompts go through in pieces of <= 32 tokens, which the matmuls run on the integer tensor cores with the
     // reference's exact block sums (causal attention over the fp16 KV cache makes the split invisible to the arithmetic)
@@ -1355,13 +1535,14 @@ extern "C" int ns_llama_eval(ns_llama* c, const int32_t* tokens, int n_tokens, i
     NS_CUDA_TRY(cudaGraphLaunch(c->decode_exec, st));
   } else {
     NS_CUDA_TRY(cudaMemcpyAsync(c->tokens, tokens, (size_t)n_tokens * sizeof(int), cudaMemcpyHostToDevice, st));
-    if (int rc = enqueue_forward(c, n_tokens, false, 1, nullptr)) return rc;
+    if (int rc = enqueue_forward(c, n_tokens, false, 1, nullptr, false)) return rc;
   }
   if (logits_host) NS_CUDA_TRY(cudaMemcpyAsync(c->h_logits, c->logits, (size_t)c->hp.n_vocab * 4, cudaMemcpyDeviceToHost, st));
   NS_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->state, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
   NS_CUDA_TRY(cudaStreamSynchronize(st));
   if (logits_host) memcpy(logits_host, c->h_logits, (size_t)c->hp.n_vocab * 4);
   if (next_token) *next_token = c->h_state[3];
+  advance_position(c, n_past, n_tokens);
   return NS_OK;
 }
 
@@ -1369,10 +1550,11 @@ extern "C" int ns_llama_eval(ns_llama* c, const int32_t* tokens, int n_tokens, i
 // device (one graph launch per token, no host synchronisation in between).  out_tokens[i] = pick after step i.
 extern "C" int ns_llama_generate(ns_llama* c, int32_t first_token, int n_past, int n_new, int32_t* out_tokens) {
   if (int rc = ns_ensure_device()) return rc;
-  if (!c || !out_tokens || n_new <= 0 || n_past < 0 || n_past + n_new > c->hp.n_ctx) {
+  if (!c || !out_tokens || n_new <= 0 || n_past < 0) {
     ns_set_error("ns_llama_generate: invalid arguments (n_past=%d n_new=%d n_ctx=%d)", n_past, n_new, c ? c->hp.n_ctx : 0);
     return NS_E_INVALID;
   }
+  if (int rc = check_streaming(c, "ns_llama_generate", n_past, n_new)) return rc;
   if (int rc = check_complete(c)) return rc;
   if (int rc = ensure_buffers(c, 1)) return rc;
   if (int rc = ensure_decode_graph(c)) return rc;
@@ -1382,9 +1564,15 @@ extern "C" int ns_llama_generate(ns_llama* c, int32_t first_token, int n_past, i
   c->h_state[2] = 0;
   c->h_state[3] = 0;
   NS_CUDA_TRY(cudaMemcpyAsync(c->state, c->h_state, 4 * sizeof(int), cudaMemcpyHostToDevice, st));
-  for (int i = 0; i < n_new; ++i) NS_CUDA_TRY(cudaGraphLaunch(c->decode_exec, st));
-  NS_CUDA_TRY(cudaMemcpyAsync(out_tokens, c->record, (size_t)n_new * sizeof(int), cudaMemcpyDeviceToHost, st));
+  // the record buffer holds n_ctx picks: a streaming generation past n_ctx drains it in pieces (stream-ordered, no host wait)
+  for (int i0 = 0; i0 < n_new; i0 += c->hp.n_ctx) {
+    const int n = n_new - i0 < c->hp.n_ctx ? n_new - i0 : c->hp.n_ctx;
+    if (i0) NS_CUDA_TRY(cudaMemsetAsync(c->state + 2, 0, sizeof(int), st));
+    for (int i = 0; i < n; ++i) NS_CUDA_TRY(cudaGraphLaunch(c->decode_exec, st));
+    NS_CUDA_TRY(cudaMemcpyAsync(out_tokens + i0, c->record, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  }
   NS_CUDA_TRY(cudaStreamSynchronize(st));
+  advance_position(c, n_past, n_new);
   return NS_OK;
 }
 
