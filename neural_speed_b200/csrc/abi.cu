@@ -620,8 +620,10 @@ int ns_route(int kind, const ns_weight* const* w, int m, int flags) {
   if (kind == NS_NODE_FFN)  // shuffles are checked on gate/up only
     tc = tc && ns_gemm_tc_supported(w[2]) && (!w[1] || ns_gemm_tc_supported(w[1])) && !w[0]->shuffle && !(w[1] && w[1]->shuffle);
   if (tc) return NS_PATH_TC;
-  if (kind != NS_NODE_PLAIN)  // the weights of the first launch must fit one GEMV launch
-    if (int rc = ns_gemv_check(w, nw, kind == NS_NODE_QKV ? NS_GEMV_CONCAT : nw == 2 ? NS_GEMV_GATE_UP_SILU : NS_GEMV_PLAIN)) return rc;
+  // the weights of the first launch must fit one GEMV launch, and an FFN's down projection one of its own
+  if (int rc = ns_gemv_check(w, nw, kind == NS_NODE_QKV ? NS_GEMV_CONCAT : nw == 2 ? NS_GEMV_GATE_UP_SILU : NS_GEMV_PLAIN)) return rc;
+  if (kind == NS_NODE_FFN)
+    if (int rc = ns_gemv_check(&w[2], 1, NS_GEMV_PLAIN)) return rc;
   return NS_PATH_GEMV;
 }
 
@@ -708,6 +710,7 @@ static int mul_mat_impl(const ns_weight* w, const float* act, int lda, float* ds
   }
   if (norm_w && !norm_foldable(&w, 1, m)) return norm_unsupported("ns_rmsnorm_mul_mat");
   const int path = ns_route(NS_NODE_PLAIN, &w, m, flags);
+  if (path < 0) return path;
   cudaStream_t st = stream_of(queue);
   void* ws = pick_ws(workspace, st, path_workspace_bytes(path, m, w->kpad));
   if (!ws) return NS_E_CUDA;

@@ -17,7 +17,8 @@ namespace {
 
 constexpr int kWarps = 8;
 constexpr int kThreads = kWarps * 32;
-constexpr int U = 4;  // chunks per row per lane per batch
+constexpr int U = 4;                        // chunks per row per lane per batch
+constexpr size_t kSmemMax = 200 * 1024;     // dynamic shared memory the kernels are set up for (launch_one)
 
 template <int WFMT>
 struct WChunk {  // one 32-element chunk of one row
@@ -318,7 +319,7 @@ int launch_one(const GemvParams& P, size_t smem, cudaStream_t st) {
   auto kern = gemv_kernel<WFMT, AMODE, M, ASYM>;
   static bool attr_set = false;
   if (!attr_set) {
-    NS_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    NS_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax));
     attr_set = true;
   }
   const int need = (P.npairs + kWarps - 1) / kWarps;
@@ -343,6 +344,18 @@ int launch_m(const GemvParams& P, int mt, size_t smem, cudaStream_t st) {
 template <int WFMT, int AMODE>
 int launch_asym(const GemvParams& P, bool asym, int mt, size_t smem, cudaStream_t st) {
   return asym ? launch_m<WFMT, AMODE, true>(P, mt, smem, st) : launch_m<WFMT, AMODE, false>(P, mt, smem, st);
+}
+
+// Bytes of one activation row in the register GEMV's shared-memory image (fp32 values, or int8 codes + chunk meta)
+size_t act_row_bytes(const ns_weight* w) {
+  return (w->wfmt == NS_W_S4) ? ns_round_up((size_t)w->kpad, 1024) : (size_t)w->kpad;
+}
+bool float_mode(const ns_weight* w) { return w->comp == NS_COMP_F32 || w->comp == NS_COMP_BF16; }
+// Dynamic shared memory of a register-GEMV launch with an mt-row kernel template
+size_t gemv_smem(const ns_weight* w, int mt) {
+  const size_t s = float_mode(w) ? (size_t)mt * w->kpad * 4
+                                 : ns_round_up((size_t)mt * act_row_bytes(w), 16) + (size_t)mt * ns_meta_stride(w->kpad) * 8;
+  return ns_round_up(s, 16);
 }
 
 }  // namespace
@@ -399,6 +412,12 @@ int ns_gemv_check(const ns_weight* const* ws_, int nw, int mode) {
       ns_set_error("fused matmul: every weight but the last needs an even n");
       return NS_E_UNSUPPORTED;
     }
+  // the register GEMV stages a whole activation row in shared memory: fp32 compute takes K <= 51200
+  if (!(w0->wfmt == NS_W_S4 && !float_mode(w0)) && gemv_smem(w0, 1) > kSmemMax) {
+    ns_set_error("GEMV: one activation row of k=%d needs %zu B of shared memory, more than the %zu B the kernel has", w0->k,
+                 gemv_smem(w0, 1), kSmemMax);
+    return NS_E_UNSUPPORTED;
+  }
   return NS_OK;
 }
 
@@ -412,7 +431,7 @@ int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* ac
     return NS_E_INVALID;
   }
   const int kpad = w0->kpad;
-  const bool fmode = (w0->comp == NS_COMP_F32 || w0->comp == NS_COMP_BF16);
+  const bool fmode = float_mode(w0);
   const int amode = fmode ? A_F32 : (w0->comp == NS_COMP_INT8 ? A_U8 : A_S8);
   const int meta_stride = ns_meta_stride(kpad);
 
@@ -464,21 +483,17 @@ int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* ac
   }
 
   const int mt = m >= 3 ? 4 : m;  // kernel template rows (1, 2, 4)
-  size_t smem;
   if (fmode) {
     P.act_bytes = (int)((size_t)m * kpad * 4);
     P.meta_off = 0;
     P.meta_stride = 0;
-    smem = (size_t)mt * kpad * 4;
   } else {
     // int8 image: [m][act_row] bytes then [m][meta_stride] int2; 4-bit weights use the ring layout (act_prep.cu)
-    const size_t act_row = (w0->wfmt == NS_W_S4) ? ns_round_up((size_t)kpad, 1024) : (size_t)kpad;
-    P.meta_off = (int)ns_round_up((size_t)m * act_row, 16);
+    P.meta_off = (int)ns_round_up((size_t)m * act_row_bytes(w0), 16);
     P.meta_stride = meta_stride;
     P.act_bytes = (int)(P.meta_off + (size_t)m * meta_stride * 8);
-    smem = ns_round_up((size_t)mt * act_row, 16) + (size_t)mt * meta_stride * 8;
   }
-  smem = ns_round_up(smem, 16);
+  const size_t smem = gemv_smem(w0, mt);
   const bool asym = w0->asym != 0;
   if (w0->wfmt == NS_W_S4 && !fmode) return ns_launch_gemv_ring(P, amode, asym, mt, st);  // the hot decode path
   if (w0->wfmt == NS_W_S4) return launch_asym<NS_W_S4, A_F32>(P, asym, mt, smem, st);

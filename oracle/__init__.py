@@ -472,6 +472,27 @@ def gemm_f64acc(a, w_kn):
     return c
 
 
+# Float-compute GEMV bar: |got - model| <= GEMV_F32_C * sqrt(K) * 2^-24 * sum_k |a_eff w_eff| per output, model = the fp64 sum.
+# Measured on an H100 80GB HBM3 (700 W limit; tests/test_gpu_gemv.py, uniform(-0.5, 0.5) data, K = 1000 .. 51200): at most 0.0116
+# of the unit bar.  Dropping the bf16 rounding of the activations moves a bf16-compute output by 4 (K = 28672) to 30 (K = 4128).
+GEMV_F32_C = 0.05
+
+
+def gemv_stated(a_eff, w_eff):
+    """fp64 model of a GEMV in fp32 arithmetic on its effective operands (bf16-rounded activations for bf16 compute, dequantised
+    fp32 weights [K,N]): (sum_k a_eff w_eff, sum_k |a_eff w_eff|), each [M,N] float64."""
+    a = np.asarray(a_eff, np.float64)
+    w = np.asarray(w_eff, np.float64)
+    return a @ w, np.abs(a) @ np.abs(w)
+
+
+def gemv_bound_ratio(got, a_eff, w_eff):
+    """max over outputs of |got - model| / (sqrt(K) * 2^-24 * sum_k |a_eff w_eff|); a float-compute GEMV stays below GEMV_F32_C"""
+    want, mag = gemv_stated(a_eff, w_eff)
+    unit = np.sqrt(np.asarray(a_eff).shape[1]) * 2.0 ** -24 * np.maximum(mag, np.finfo(np.float32).tiny)
+    return float((np.abs(np.asarray(got, np.float64) - want) / unit).max())
+
+
 def f32_to_bf16_bits(x):
     """RNE fp32 -> bf16 bit pattern (bestla_utils.h:146-153), vectorised."""
     u = _c(x, np.float32).view(np.uint32).astype(np.uint64)

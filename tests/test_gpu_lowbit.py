@@ -81,3 +81,5 @@ def test_f4_codebook_blobs(name, cdt, m):
     # fp32 compute: the reference UT bar; bf16 compute: bf16 rounding of the dequantised weight too (GEMV keeps it in fp32, the tensor-core
     # GEMM for > 16 rows rounds level x scale to bf16 as the reference does)
     assert np.abs(out - want).max() <= (1e-3 if cdt == "fp32" else 2e-2 if m <= 16 else 4e-2)
+    if m <= 16:  # the GEMV's stated arithmetic: bf16 (or fp32) activations, the dequantised weight in fp32, fp32 FMAs
+        assert oracle.gemv_bound_ratio(out, a_eff, wdq) <= oracle.GEMV_F32_C

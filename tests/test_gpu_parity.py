@@ -298,6 +298,8 @@ def test_btla_bf16_scales_and_bf16_compute():
     got = run_mul_mat(ns.Weight.from_unpacked(q, sc, None, g, ns.W_S4, ns.S_F32, ns.COMP_BF16), a)
     a_b = oracle.bf16_bits_to_f32(oracle.f32_to_bf16_bits(a))
     assert np.abs(got - oracle.gemm_f64acc(a_b, oracle.btla_dequant(q, sc, None, g))).max() <= 2e-2  # BF16 tol, bestla_ut.h:80-94
+    # the GEMV's stated bf16-compute arithmetic: bf16 activations, fp32 weights, fp32 FMAs
+    assert oracle.gemv_bound_ratio(got, a_b, oracle.btla_dequant(q, sc, None, g)) <= oracle.GEMV_F32_C
 
 
 def test_gptq_act_order_shuffle():
