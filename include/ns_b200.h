@@ -337,7 +337,34 @@ NS_API int ns_llama_set_exact_prefill(ns_llama* ctx, int on);
  *   meaningless in ring order, llama.cpp:467), and, once a step has passed n_ctx, NS_E_INVALID for any n_past other than the next
  *   position or a restart at n_past <= n_keep.  Enabling or disabling drops the captured decode graph. */
 NS_API int ns_llama_set_streaming(ns_llama* ctx, int n_keep);
-NS_API unsigned long long ns_llama_kv_bytes(const ns_llama* ctx);
+/* ---- continuous batching (the reference's model_eval over an array of model_input, models/llama/llama.cpp:53-90) ----------
+ * The KV cache holds n_seq blocks, one per sequence ([n_layer][n_seq][n_head_kv][n_ctx][hd] fp16; kv_n_ctx_block =
+ * max_request_num, model_utils.cpp:1027-1036).  A batched step takes one new token of each of n distinct sequences through one
+ * forward pass of n rows: every matmul runs on all n rows at once (the weights are read once), K / V go to each row's block at
+ * its own position (llama.cpp:370-411), attention runs per row (:414-489), and every row's logits are returned (:745-758).
+ * Each row's arithmetic per matmul node is what a prompt of n rows gets (GEMV for n <= 2, the integer tensor cores for 3 .. 32
+ * rows of int4 weights with an integer compute type); the attention of each row is the one-token step's, bit for bit.
+ *
+ * 1 <= n_seq <= 32 KV blocks (default 1).  Reallocates and zeroes the cache; every sequence restarts at n_past 0; drops the
+ * captured graphs.  NS_E_UNSUPPORTED for n_seq > 1 with streaming on (llama.cpp:104 forbids the pair) or a head size other
+ * than 64 / 128.  ns_llama_set_streaming returns NS_E_UNSUPPORTED for n_keep >= 0 while n_seq > 1.  ns_llama_eval and
+ * ns_llama_generate serve sequence 0. */
+NS_API int ns_llama_set_sequences(ns_llama* ctx, int n_seq);
+/* ns_llama_eval on KV block `seq` (prompts, exact-prefill mode and all argument rules as ns_llama_eval) */
+NS_API int ns_llama_eval_seq(ns_llama* ctx, int seq, const int32_t* tokens, int n_tokens, int n_past, float* logits_host,
+                             int32_t* next_token);
+/* one new token for each of n DISTINCT sequences in one forward pass of n rows; logits_host (nullable) [n][n_vocab],
+ * next_tokens (nullable) [n] greedy picks; n_past[i] + 1 <= n_ctx.  One CUDA graph per n (captured on first use) serves any
+ * set of sequences at any positions.  NS_E_INVALID (nothing launched) for n outside [1, n_seq], a sequence id outside
+ * [0, n_seq) or given twice, n_past[i] < 0 or past the context, null pointers; NS_E_UNSUPPORTED with streaming on or a head
+ * size other than 64 / 128. */
+NS_API int ns_llama_decode_batch(ns_llama* ctx, int n, const int* seq, const int32_t* tokens, const int* n_past,
+                                 float* logits_host, int32_t* next_tokens);
+/* greedy generation for n distinct sequences, each pick fed back on the device; out_tokens [n][n_new];
+ * n_past[i] + n_new <= n_ctx; argument rules as ns_llama_decode_batch */
+NS_API int ns_llama_generate_batch(ns_llama* ctx, int n, const int* seq, const int32_t* first_tokens, const int* n_past,
+                                   int n_new, int32_t* out_tokens);
+NS_API unsigned long long ns_llama_kv_bytes(const ns_llama* ctx); /* all n_seq blocks */
 /* One layer's attention of the eval step on its own, for parity tests: RoPE (mode 0, angle = p * rope_theta^(-2i/hd) / rope_scale)
  * of q [m][n_head * hd] in place and of the m new rows k [m][n_head_kv * hd] at positions n_past .. n_past + m - 1, k and v appended
  * to the fp16 caches kc / vc [n_head_kv][n_ctx][hd], out [m][n_head * hd] = causal softmax(K q / sqrt(hd)) V (llama.cpp:286-302).
@@ -366,6 +393,17 @@ NS_API int ns_llama_attention(int kernel, float* q, const float* k, const float*
  * NS_E_UNSUPPORTED (nothing launched) for head sizes other than 64 / 128. */
 NS_API int ns_llama_attention_ring(float* q, const float* k, const float* v, void* kc, void* vc, int n_head, int n_head_kv, int hd,
                                    int n_ctx, int n_keep, int n_total, float rope_theta, float* out, void* ws, void* queue);
+/* One layer's batched decode attention on its own, for parity tests (as ns_llama_attention with NS_ATTN_SPLIT_DECODE, row by row):
+ * q [n][n_head * hd] (rotated in registers only), k / v [n][n_head_kv * hd], caches [n_seq][n_head_kv][n_ctx][hd] fp16; row i
+ * appends to block seq[i] at position n_past[i] and attends to positions 0 .. n_past[i] of that block; out [n][n_head * hd].
+ * seq / n_past are host arrays of n entries (distinct ids in [0, n_seq), 0 <= n_past[i] < n_ctx, else NS_E_INVALID); hd 64 / 128
+ * (else NS_E_UNSUPPORTED); nothing is launched on a refused call.  ws: ns_llama_attention_batch_workspace_bytes(n, n_head, hd,
+ * n_ctx) bytes, zeroed once by the caller: int rows[n][4] (n_past in slot 1) | int seq[n], padded to 16 bytes | unsigned
+ * tickets[n][n_head] (zero again after every call), padded to 16 bytes | float partials[n][n_head][ceil(n_ctx / 256)][hd + 2]. */
+NS_API size_t ns_llama_attention_batch_workspace_bytes(int n, int n_head, int hd, int n_ctx);
+NS_API int ns_llama_attention_batch(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n,
+                                    const int* seq, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
+                                    float rope_theta, float rope_scale, float* out, void* ws, void* queue);
 
 /* ---- tensor-parallel exchange step over NVLink peer memory (SURVEY 8e) --------------------------------------------
  * One-shot sum all-reduce replacing reduce_add / ne_all_reduce (core/parallel_context.cpp:47, ne_layers.c:5466) for the

@@ -60,6 +60,8 @@ EXPORTS = [
     "BTLAGemmPackBSize", "BTLAGemmQuantPackB", "BTLAGemmPackB", "BTLAGemmUnPackB", "ns_quantize_row_q4_0", "ns_split_weight_size", "ns_split_weight",
     "ns_llama_create", "ns_llama_free", "ns_llama_set_f32", "ns_llama_set_weight", "ns_llama_eval", "ns_llama_generate", "ns_llama_set_exact_prefill",
     "ns_llama_set_streaming", "ns_llama_kv_bytes", "ns_llama_attention_workspace_bytes", "ns_llama_attention", "ns_llama_attention_ring",
+    "ns_llama_set_sequences", "ns_llama_eval_seq", "ns_llama_decode_batch", "ns_llama_generate_batch",
+    "ns_llama_attention_batch_workspace_bytes", "ns_llama_attention_batch",
     "ns_comm_handle_bytes", "ns_comm_create", "ns_comm_get_handle", "ns_comm_open_peers", "ns_comm_link_local", "ns_comm_all_reduce_f32",
     "ns_comm_status", "ns_comm_free",
 ]
@@ -186,6 +188,13 @@ def lib() -> C.CDLL:
     L.ns_llama_attention.argtypes = [i, vp, vp, vp, vp, vp, i, i, i, i, i, i, C.c_float, C.c_float, vp, vp, vp]
     L.ns_llama_attention_ring.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, i, i, C.c_float, vp, vp, vp]
     L.ns_llama_set_streaming.argtypes = [vp, i]
+    L.ns_llama_set_sequences.argtypes = [vp, i]
+    L.ns_llama_eval_seq.argtypes = [vp, i, vp, i, i, vp, vp]
+    L.ns_llama_decode_batch.argtypes = [vp, i, vp, vp, vp, vp, vp]
+    L.ns_llama_generate_batch.argtypes = [vp, i, vp, vp, vp, i, vp]
+    L.ns_llama_attention_batch_workspace_bytes.restype = sz
+    L.ns_llama_attention_batch_workspace_bytes.argtypes = [i, i, i, i]
+    L.ns_llama_attention_batch.argtypes = [vp, vp, vp, vp, vp, i, i, vp, vp, i, i, i, i, C.c_float, C.c_float, vp, vp, vp]
     L.ns_comm_handle_bytes.restype = sz
     L.ns_comm_create.restype = vp
     L.ns_comm_create.argtypes = [i, i, sz, vp]
@@ -498,6 +507,37 @@ class Llama:
         token evaluated so far (include/ns_b200.h, ns_llama_set_streaming)"""
         _check(lib().ns_llama_set_streaming(self.h, n_keep), "ns_llama_set_streaming")
 
+    def set_sequences(self, n_seq: int):
+        """n_seq KV blocks for continuous batching; every sequence restarts empty (include/ns_b200.h, ns_llama_set_sequences)"""
+        _check(lib().ns_llama_set_sequences(self.h, n_seq), "ns_llama_set_sequences")
+
+    def eval_seq(self, seq: int, tokens, n_past: int, want_logits=True):
+        """eval() on KV block `seq`: a joining sequence's prompt, or any single step of one sequence"""
+        t = np.ascontiguousarray(tokens, np.int32)
+        logits = np.empty(self.hp.n_vocab, np.float32) if want_logits else None
+        nxt = C.c_int32(0)
+        _check(lib().ns_llama_eval_seq(self.h, seq, _np_ptr(t), t.size, n_past, _np_ptr(logits) if want_logits else None,
+                                       C.byref(nxt)), "ns_llama_eval_seq")
+        return logits, int(nxt.value)
+
+    def decode_batch(self, seqs, tokens, n_past, want_logits=True):
+        """one new token for each of the distinct sequences `seqs` in one forward pass -> (logits [n][n_vocab] or None, picks [n])"""
+        s, t, p = (np.ascontiguousarray(a, np.int32) for a in (seqs, tokens, n_past))
+        n = s.size
+        logits = np.empty((n, self.hp.n_vocab), np.float32) if want_logits else None
+        nxt = np.empty(n, np.int32)
+        _check(lib().ns_llama_decode_batch(self.h, n, _np_ptr(s), _np_ptr(t), _np_ptr(p), _np_ptr(logits) if want_logits else None,
+                                           _np_ptr(nxt)), "ns_llama_decode_batch")
+        return logits, nxt
+
+    def generate_batch(self, seqs, first_tokens, n_past, n_new: int) -> np.ndarray:
+        """greedy generation of n_new tokens for each sequence, picks fed back on the device -> [n][n_new]"""
+        s, t, p = (np.ascontiguousarray(a, np.int32) for a in (seqs, first_tokens, n_past))
+        out = np.empty((s.size, n_new), np.int32)
+        _check(lib().ns_llama_generate_batch(self.h, s.size, _np_ptr(s), _np_ptr(t), _np_ptr(p), n_new, _np_ptr(out)),
+               "ns_llama_generate_batch")
+        return out
+
     def close(self):
         if self.h:
             lib().ns_llama_free(self.h)
@@ -508,3 +548,12 @@ class Llama:
             self.close()
         except Exception:
             pass
+
+
+def attention_batch(q_ptr: int, k_ptr: int, v_ptr: int, kc_ptr: int, vc_ptr: int, n_seq: int, seqs, n_past, n_head: int, n_head_kv: int,
+                    hd: int, n_ctx: int, out_ptr: int, ws_ptr: int, rope_theta=10000.0, rope_scale=1.0, queue=None) -> int:
+    """ns_llama_attention_batch on device pointers (one layer's batched decode attention); returns the status code"""
+    s, p = np.ascontiguousarray(seqs, np.int32), np.ascontiguousarray(n_past, np.int32)
+    return lib().ns_llama_attention_batch(C.c_void_p(q_ptr), C.c_void_p(k_ptr), C.c_void_p(v_ptr), C.c_void_p(kc_ptr), C.c_void_p(vc_ptr),
+                                          n_seq, s.size, _np_ptr(s), _np_ptr(p), n_head, n_head_kv, hd, n_ctx, rope_theta, rope_scale,
+                                          C.c_void_p(out_ptr), C.c_void_p(ws_ptr), queue)

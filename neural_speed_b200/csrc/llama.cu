@@ -34,13 +34,14 @@ struct Layer {
 
 constexpr int kAttnThreads = 128;
 
-// x[t][:] = table[token[t]][:]
+// x[t][:] = table[token[t * TSTRIDE]][:]   (TSTRIDE 4: the token slot of each row's device state in a batched step)
+template <int TSTRIDE>
 __global__ void __launch_bounds__(256) embed_kernel(const float* __restrict__ table, const int* __restrict__ tokens, int n_embd,
                                                     int n_vocab, float* __restrict__ x) {
   pdl_launch_dependents();
   pdl_wait();
   const int t = blockIdx.y;
-  int tok = tokens[t];
+  int tok = tokens[t * TSTRIDE];
   tok = tok < 0 ? 0 : (tok >= n_vocab ? n_vocab - 1 : tok);
   const float4* src = (const float4*)(table + (size_t)tok * n_embd);
   float4* dst = (float4*)(x + (size_t)t * n_embd);
@@ -388,6 +389,11 @@ __global__ void __launch_bounds__(kAW * 32) attn_fast_kernel(const float* __rest
 // with v in slot n_keep + (n_total - n_ctx) mod (n_ctx - n_keep), inside whichever range holds it; then every staged K row at or
 // past n_keep, the new one included, is rotated one position back with the fp16 shift table (ne_layers.c:9514-9526), scored
 // and written back with one bulk store; attention covers all n_ctx slots with no mask.
+//
+// BATCH = true: one new token for each of n sequences (continuous batching, llama.cpp:414-489 run per request), grid
+// (n_head, ranges, n).  CTA z serves row z: its position is state[4 z + 1] (the row's {token, n_past, n_recorded, pick}), its
+// KV block seqs[z] ([n_seq][n_head_kv][n_ctx][hd] per layer), and its q / k / v / out rows, partials and tickets are row z's.
+// Everything after those offsets is the RING = false kernel's code, so each row's arithmetic is the single-sequence step's.
 constexpr int kSplitKeys = 256;
 constexpr int kDW = 16;  // warps per CTA
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -399,12 +405,14 @@ static constexpr size_t attn_decode_smem() {
 struct ShiftTable {
   __half2 cs[64];
 };
-template <int HD, bool RING>
+template <int HD, bool RING, bool BATCH = false>
 __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __restrict__ q, const float* __restrict__ knew,
                                                             const float* __restrict__ vnew, __half* __restrict__ kc, __half* __restrict__ vc,
                                                             const int* __restrict__ state, float* __restrict__ out, float* __restrict__ part_ws,
                                                             unsigned* __restrict__ tickets, int n_head, int n_head_kv, int n_ctx, int nsplit,
-                                                            float scale, float theta_scale, float freq_scale, int n_keep, const ShiftTable tab) {
+                                                            float scale, float theta_scale, float freq_scale, int n_keep, const ShiftTable tab,
+                                                            const int* __restrict__ seqs) {
+  static_assert(!(RING && BATCH), "the ring serves one sequence");
   constexpr int EPL = HD / 32;
   extern __shared__ __align__(128) unsigned char smraw[];
   __half* Kt = reinterpret_cast<__half*>(smraw);  // [kSplitKeys][HD]
@@ -427,11 +435,23 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   const int hk = RING ? (int)blockIdx.x : (int)blockIdx.x / group;
   const int h0 = RING ? hk * group : (int)blockIdx.x;  // query heads h0 .. h0 + nh - 1
   const int nh = RING ? group : 1;
-  const int pos = state[1];
+  const int row = BATCH ? (int)blockIdx.z : 0;
+  const int pos = state[4 * row + 1];
   const bool wrapped = RING && pos >= n_ctx;
   const int len = min(pos + 1, n_ctx);
   const int nact = (len + kSplitKeys - 1) / kSplitKeys;
   if (split >= nact) return;
+  if (BATCH) {  // the row's KV block, activations, partials and tickets (the sequence ids, like the positions, precede this step)
+    const size_t blk = (size_t)seqs[row] * n_head_kv * n_ctx * HD;
+    kc += blk;
+    vc += blk;
+    q += (size_t)row * n_head * HD;
+    knew += (size_t)row * n_head_kv * HD;
+    vnew += (size_t)row * n_head_kv * HD;
+    out += (size_t)row * n_head * HD;
+    part_ws += (size_t)row * n_head * nsplit * (HD + 2);
+    tickets += (size_t)row * n_head;
+  }
   const int i0 = split * kSplitKeys, i1 = min(len, i0 + kSplitKeys);
   const int slot = wrapped ? n_keep + (pos - n_ctx) % (n_ctx - n_keep) : pos;  // cache row of the token being evaluated
   const bool has_new = wrapped ? slot >= i0 && slot < i1 : (i1 == len) && pos < n_ctx;  // ... sits in this range
@@ -849,6 +869,8 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
 // greedy pick: index of the maximum, lowest index on ties (model_utils.cpp:2963-2985); also advances the device-side
 // position.  kArgmaxBlocks CTAs scan slices (all loads in flight at once); the last CTA to finish (ticket) merges the
 // partial results.  state[3] = pick; when `advance`: state[0] = pick, state[1] += n_tokens, record[state[2]++] = pick.
+// BATCH: grid row y (one per sequence) does the same for logits row y with state + 4 y, record + y * rec_stride, its own partial
+// slots and its own ticket (the single-sequence instantiation keeps row 0 at compile time).
 constexpr int kArgmaxBlocks = 32;
 __device__ __forceinline__ void argmax_merge(float& best, int& bi, float ov, int oi) {
   if (ov > best || (ov == best && oi < bi)) {
@@ -856,11 +878,19 @@ __device__ __forceinline__ void argmax_merge(float& best, int& bi, float ov, int
     bi = oi;
   }
 }
+template <bool BATCH>
 __global__ void __launch_bounds__(256) argmax_kernel(const float* __restrict__ logits, int n, int* __restrict__ state, int n_tokens,
-                                                     int advance, int* __restrict__ record, float* __restrict__ pval, int* __restrict__ pidx,
-                                                     unsigned* __restrict__ ticket) {
+                                                     int advance, int* __restrict__ record, int rec_stride, float* __restrict__ pval,
+                                                     int* __restrict__ pidx, unsigned* __restrict__ ticket) {
   pdl_launch_dependents();
   pdl_wait();
+  const int row = BATCH ? (int)blockIdx.y : 0;
+  logits += (size_t)row * n;
+  state += 4 * row;
+  if (record) record += (size_t)row * rec_stride;
+  pval += row * kArgmaxBlocks;
+  pidx += row * kArgmaxBlocks;
+  ticket += row;
   const int per = (n + kArgmaxBlocks - 1) / kArgmaxBlocks;
   const int lo = blockIdx.x * per, hi = min(n, lo + per);
   float best = -INFINITY;
@@ -977,6 +1007,44 @@ struct Ring {
   int n_keep;
   ShiftTable tab;
 };
+static int grant_decode_smem(AttnAttr& attr) {
+  if (attr.decode) return NS_OK;
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<128>()));
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<64>()));
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<128>()));
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<64>()));
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)attn_decode_smem<128>()));
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)attn_decode_smem<64>()));
+  attr.decode = true;
+  return NS_OK;
+}
+
+// Batched decode attention: one new token for each of n sequences, one launch (attn_decode_kernel<HD, false, true>).  rstate:
+// [n][4] row states (n_past in slot 1), seqs [n] KV block per row, caches [n_seq][n_head_kv][n_ctx][hd] fp16, q / out
+// [n][n_head * hd], k / v [n][n_head_kv * hd], part [n][n_head][ranges][hd + 2], tickets [n][n_head].  hd 64 / 128 only.
+static int launch_attention_batch(const float* q, const float* k, const float* v, __half* kc, __half* vc, const int* rstate,
+                                  const int* seqs, float* out, float* part, unsigned* tickets, int n, int n_head, int n_head_kv, int hd,
+                                  int n_ctx, float rope_theta, float rope_scale, AttnAttr& attr, cudaStream_t st) {
+  if (hd != 64 && hd != 128) {
+    ns_set_error("ns_llama: the batched decode attention needs head size 64 or 128, got %d", hd);
+    return NS_E_UNSUPPORTED;
+  }
+  if (int rc = grant_decode_smem(attr)) return rc;
+  const float theta_scale = powf(rope_theta, -2.0f / (float)hd);  // as launch_attention
+  const float freq_scale = 1.f / rope_scale;
+  const float attn_scale = 1.0f / sqrtf((float)hd);
+  const int nsplit = attn_ranges(n_ctx);
+  auto kern = hd == 128 ? attn_decode_kernel<128, false, true> : attn_decode_kernel<64, false, true>;
+  NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)n_head, (unsigned)nsplit, (unsigned)n), dim3(kDW * 32),
+                            hd == 128 ? attn_decode_smem<128>() : attn_decode_smem<64>(), st, q, k,
+                            v, kc, vc, rstate, out, part, tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale, theta_scale, freq_scale,
+                            -1, ShiftTable{}, seqs));
+  ns_count_launch();
+  return NS_OK;
+}
+
 static int launch_attention(int kind, float* q, const float* k, const float* v, __half* kc, __half* vc, const int* state, float* out,
                             float* part, unsigned* tickets, int n_head, int n_head_kv, int hd, int n_ctx, int m, float rope_theta,
                             float rope_scale, AttnAttr& attr, cudaStream_t st, const Ring* ring = nullptr) {
@@ -997,13 +1065,7 @@ static int launch_attention(int kind, float* q, const float* k, const float* v, 
   }
   if (kind == NS_ATTN_SPLIT_DECODE) {
     // rope + KV append + attention in one launch, K / V staged by TMA, the context split over CTAs
-    if (!attr.decode) {
-      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<128>()));
-      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<64>()));
-      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<128>()));
-      NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_decode_smem<64>()));
-      attr.decode = true;
-    }
+    if (int rc = grant_decode_smem(attr)) return rc;
     const int nsplit = attn_ranges(n_ctx);
     const size_t dsm = hd == 128 ? attn_decode_smem<128>() : attn_decode_smem<64>();
     auto kern = ring ? (hd == 128 ? attn_decode_kernel<128, true> : attn_decode_kernel<64, true>)
@@ -1011,7 +1073,7 @@ static int launch_attention(int kind, float* q, const float* k, const float* v, 
     const unsigned gx = (unsigned)(ring ? n_head_kv : n_head);  // ring: one CTA per (kv head, range)
     NS_CUDA_TRY(ns_launch_pdl(kern, dim3(gx, (unsigned)nsplit), dim3(kDW * 32), dsm, st, (const float*)q, k, v, kc, vc, state, out, part,
                               tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale, theta_scale, freq_scale, ring ? ring->n_keep : -1,
-                              ring ? ring->tab : ShiftTable{}));
+                              ring ? ring->tab : ShiftTable{}, (const int*)nullptr));
     ns_count_launch();
     return NS_OK;
   }
@@ -1101,6 +1163,77 @@ extern "C" int ns_llama_attention_ring(float* q, const float* k, const float* v,
                           st, &ring);
 }
 
+// Checks the rows of a batched call: 1 <= n <= n_seq, every id in [0, n_seq) and distinct, 0 <= n_past[i], n_past[i] + steps <= n_ctx
+static int check_rows(const char* who, int n_seq, int n, const int* seq, const int* n_past, int steps, int n_ctx) {
+  if (n < 1 || n > n_seq) {
+    ns_set_error("%s: n %d outside [1, n_seq %d]", who, n, n_seq);
+    return NS_E_INVALID;
+  }
+  unsigned long long seen = 0;  // n_seq <= 32
+  for (int i = 0; i < n; ++i) {
+    if (seq[i] < 0 || seq[i] >= n_seq) {
+      ns_set_error("%s: sequence id %d outside [0, %d)", who, seq[i], n_seq);
+      return NS_E_INVALID;
+    }
+    if (seen >> seq[i] & 1ull) {
+      ns_set_error("%s: sequence id %d appears twice", who, seq[i]);
+      return NS_E_INVALID;
+    }
+    seen |= 1ull << seq[i];
+    if (n_past[i] < 0 || n_past[i] + steps > n_ctx) {
+      ns_set_error("%s: sequence %d: n_past %d + %d steps outside n_ctx %d", who, seq[i], n_past[i], steps, n_ctx);
+      return NS_E_INVALID;
+    }
+  }
+  return NS_OK;
+}
+
+// Workspace of ns_llama_attention_batch: int rows[n][4] (slot 1 = n_past) | int seq[n], padded to 16 bytes | unsigned
+// tickets[n][n_head], padded to 16 bytes | float partials[n][n_head][ceil(n_ctx / 256)][hd + 2]
+static size_t attnb_ws_seq_offset(int n) { return (size_t)n * 4 * sizeof(int); }
+static size_t attnb_ws_tickets_offset(int n) { return attnb_ws_seq_offset(n) + ((size_t)n * sizeof(int) + 15) / 16 * 16; }
+static size_t attnb_ws_part_offset(int n, int n_head) {
+  return attnb_ws_tickets_offset(n) + ((size_t)n * n_head * sizeof(unsigned) + 15) / 16 * 16;
+}
+
+extern "C" size_t ns_llama_attention_batch_workspace_bytes(int n, int n_head, int hd, int n_ctx) {
+  if (n <= 0 || n_head <= 0 || hd <= 0 || n_ctx <= 0) return 0;
+  return attnb_ws_part_offset(n, n_head) + (size_t)n * n_head * attn_ranges(n_ctx) * (hd + 2) * sizeof(float);
+}
+
+extern "C" int ns_llama_attention_batch(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n, const int* seq,
+                                        const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx, float rope_theta,
+                                        float rope_scale, float* out, void* ws, void* queue) {
+  if (int rc = ns_ensure_device()) return rc;
+  if (!q || !k || !v || !kc || !vc || !seq || !n_past || !out || !ws || n_seq < 1 || n_seq > 32 || n_head <= 0 || n_head_kv <= 0 ||
+      n_head % n_head_kv || hd <= 0 || hd % 2 || n_ctx <= 0 || !(rope_theta > 0.f) || !(rope_scale > 0.f)) {
+    ns_set_error("ns_llama_attention_batch: invalid arguments (n_seq=%d n=%d n_head=%d n_head_kv=%d hd=%d n_ctx=%d)", n_seq, n, n_head,
+                 n_head_kv, hd, n_ctx);
+    return NS_E_INVALID;
+  }
+  if (int rc = check_rows("ns_llama_attention_batch", n_seq, n, seq, n_past, 1, n_ctx)) return rc;
+  if (hd != 64 && hd != 128) {
+    ns_set_error("ns_llama_attention_batch: head size %d (the batched decode attention takes 64 or 128)", hd);
+    return NS_E_UNSUPPORTED;
+  }
+  cudaStream_t st = ns_stream_of(queue);
+  char* w = static_cast<char*>(ws);
+  std::vector<int> rows((size_t)n * 5, 0);
+  for (int i = 0; i < n; ++i) {
+    rows[(size_t)4 * i + 1] = n_past[i];
+    rows[(size_t)4 * n + i] = seq[i];
+  }
+  NS_CUDA_TRY(cudaMemcpyAsync(w, rows.data(), rows.size() * sizeof(int), cudaMemcpyHostToDevice, st));  // pageable: staged now
+  AttnAttr attr;
+  return launch_attention_batch(q, k, v, static_cast<__half*>(kc), static_cast<__half*>(vc), reinterpret_cast<const int*>(w),
+                                reinterpret_cast<const int*>(w + attnb_ws_seq_offset(n)), out,
+                                reinterpret_cast<float*>(w + attnb_ws_part_offset(n, n_head)),
+                                reinterpret_cast<unsigned*>(w + attnb_ws_tickets_offset(n)), n, n_head, n_head_kv, hd, n_ctx, rope_theta,
+                                rope_scale, attr, st);
+}
+
+constexpr int kMaxSeq = 32;  // KV blocks of one context (ns_llama_set_sequences)
+
 struct ns_llama {
   ns_llama_hparams hp;
   cudaStream_t st;
@@ -1109,17 +1242,20 @@ struct ns_llama {
   float* out_norm = nullptr;
   const ns_weight* output = nullptr;
   std::vector<void*> owned;  // device allocations freed with the context
-  __half *kc = nullptr, *vc = nullptr;
+  int n_seq = 0;             // KV blocks: ns_llama_set_sequences (1 from ns_llama_create)
+  __half *kc = nullptr, *vc = nullptr;  // [n_layer][n_seq][n_head_kv][n_ctx][hd] fp16
   int* state = nullptr;   // device: {token, n_past, n_recorded, last_pick}
   int* tokens = nullptr;  // device: prompt tokens of the current eval
   int* record = nullptr;  // device: generated tokens
-  float* am_val = nullptr;  // argmax partials
+  int* bstate = nullptr;  // device, batched steps: [kMaxSeq][4] row states as `state` | [kMaxSeq] KV block of each row
+  int* brecord = nullptr;   // device, batched steps: [n_seq][n_ctx] picks of each row
+  float* am_val = nullptr;  // argmax partials: [kMaxSeq][kArgmaxBlocks]
   int* am_idx = nullptr;
-  unsigned* am_ticket = nullptr;
+  unsigned* am_ticket = nullptr;  // [kMaxSeq]
   int m_cap = 0;
   AttnAttr attn_attr;                   // dynamic shared memory already granted to the attention kernels on this context's device
-  float* attn_part = nullptr;           // split-context decode attention: [n_head][nsplit][hd + 2] partials
-  unsigned* attn_tickets = nullptr;     // [n_head]
+  float* attn_part = nullptr;           // split-context decode attention: [n_seq][n_head][nsplit][hd + 2] partials
+  unsigned* attn_tickets = nullptr;     // [n_seq][n_head]
   int attn_nsplit = 0;
   int exact_prefill = 0;               // ns_llama_set_exact_prefill
   bool streaming = false;              // ns_llama_set_streaming: ring.n_keep sink slots, ring.tab the shift table
@@ -1131,8 +1267,11 @@ struct ns_llama {
   size_t ws_bytes = 0;
   cudaGraphExec_t decode_exec = nullptr;
   cudaGraph_t decode_graph = nullptr;
+  cudaGraphExec_t batch_exec[kMaxSeq + 1] = {};  // one batched step of n rows, captured on first use
+  cudaGraph_t batch_graph[kMaxSeq + 1] = {};
   int* h_state = nullptr;  // pinned host staging
-  float* h_logits = nullptr;
+  int* h_bstate = nullptr;  // [kMaxSeq * 5]
+  float* h_logits = nullptr;  // [n_seq][n_vocab]
 };
 
 static void* dev_alloc(ns_llama* c, size_t bytes) {
@@ -1154,6 +1293,57 @@ static void dev_free(ns_llama* c, void* p) {
       cudaFree(p);
       return;
     }
+}
+
+// captured graphs hold pointers to the weights, norms, buffers and KV blocks: dropped whenever one of those changes
+static void drop_graphs(ns_llama* c) {
+  if (c->decode_exec) {
+    cudaGraphExecDestroy(c->decode_exec);
+    cudaGraphDestroy(c->decode_graph);
+    c->decode_exec = nullptr;
+    c->decode_graph = nullptr;
+  }
+  for (int n = 0; n <= kMaxSeq; ++n)
+    if (c->batch_exec[n]) {
+      cudaGraphExecDestroy(c->batch_exec[n]);
+      cudaGraphDestroy(c->batch_graph[n]);
+      c->batch_exec[n] = nullptr;
+      c->batch_graph[n] = nullptr;
+    }
+}
+
+// (re)allocates everything sized by the number of KV blocks -- caches, logits, decode-attention partials and tickets, batch
+// record -- and zeroes the caches and tickets.  On failure n_seq is 0 and every eval refuses to run.
+static int alloc_sequences(ns_llama* c, int n_seq) {
+  const ns_llama_hparams& hp = c->hp;
+  const int hd = hp.n_embd / hp.n_head;
+  void* old[6] = {c->kc, c->vc, c->logits, c->attn_part, c->attn_tickets, c->brecord};
+  for (void* p : old) dev_free(c, p);
+  c->kc = c->vc = nullptr;
+  c->logits = c->attn_part = nullptr;
+  c->attn_tickets = nullptr;
+  c->brecord = nullptr;
+  if (c->h_logits) cudaFreeHost(c->h_logits);
+  c->h_logits = nullptr;
+  c->n_seq = 0;
+  const size_t kv_elems = (size_t)n_seq * hp.n_layer * hp.n_head_kv * hp.n_ctx * hd;
+  c->attn_nsplit = attn_ranges(hp.n_ctx);
+  c->kc = (__half*)dev_alloc(c, kv_elems * 2);
+  c->vc = (__half*)dev_alloc(c, kv_elems * 2);
+  c->logits = (float*)dev_alloc(c, (size_t)n_seq * hp.n_vocab * 4);
+  c->attn_part = (float*)dev_alloc(c, (size_t)n_seq * hp.n_head * c->attn_nsplit * (hd + 2) * sizeof(float));
+  c->attn_tickets = (unsigned*)dev_alloc(c, (size_t)n_seq * hp.n_head * sizeof(unsigned));
+  c->brecord = (int*)dev_alloc(c, (size_t)n_seq * hp.n_ctx * sizeof(int));
+  if (!c->kc || !c->vc || !c->logits || !c->attn_part || !c->attn_tickets || !c->brecord) return NS_E_CUDA;
+  if (!ns_cuda_ok(cudaMallocHost((void**)&c->h_logits, (size_t)n_seq * hp.n_vocab * 4), "cudaMallocHost")) {
+    c->h_logits = nullptr;
+    return NS_E_CUDA;
+  }
+  NS_CUDA_TRY(cudaMemsetAsync(c->attn_tickets, 0, (size_t)n_seq * hp.n_head * sizeof(unsigned), c->st));
+  NS_CUDA_TRY(cudaMemsetAsync(c->kc, 0, kv_elems * 2, c->st));
+  NS_CUDA_TRY(cudaMemsetAsync(c->vc, 0, kv_elems * 2, c->st));
+  c->n_seq = n_seq;
+  return NS_OK;
 }
 
 extern "C" ns_llama* ns_llama_create(const ns_llama_hparams* hp, void* queue) {
@@ -1180,30 +1370,20 @@ extern "C" ns_llama* ns_llama_create(const ns_llama_hparams* hp, void* queue) {
       return nullptr;
     }
   }
-  const size_t kv_elems = (size_t)hp->n_layer * hp->n_head_kv * hp->n_ctx * hd;
-  c->kc = (__half*)dev_alloc(c, kv_elems * 2);
-  c->vc = (__half*)dev_alloc(c, kv_elems * 2);
   c->state = (int*)dev_alloc(c, 4 * sizeof(int));
   c->tokens = (int*)dev_alloc(c, (size_t)hp->n_ctx * sizeof(int));
   c->record = (int*)dev_alloc(c, (size_t)hp->n_ctx * sizeof(int));
-  c->logits = (float*)dev_alloc(c, (size_t)hp->n_vocab * 4);
-  c->am_val = (float*)dev_alloc(c, 64 * sizeof(float));
-  c->am_idx = (int*)dev_alloc(c, 64 * sizeof(int));
-  c->am_ticket = (unsigned*)dev_alloc(c, sizeof(unsigned));
-  if (c->am_ticket) cudaMemsetAsync(c->am_ticket, 0, sizeof(unsigned), c->st);
-  c->attn_nsplit = attn_ranges(hp->n_ctx);
-  c->attn_part = (float*)dev_alloc(c, (size_t)hp->n_head * c->attn_nsplit * (hd + 2) * sizeof(float));
-  c->attn_tickets = (unsigned*)dev_alloc(c, (size_t)hp->n_head * sizeof(unsigned));
-  if (c->attn_tickets) cudaMemsetAsync(c->attn_tickets, 0, (size_t)hp->n_head * sizeof(unsigned), c->st);
-  if (!c->kc || !c->vc || !c->state || !c->tokens || !c->record || !c->logits || !c->am_val || !c->am_idx || !c->am_ticket ||
-      !c->attn_part || !c->attn_tickets ||
+  c->bstate = (int*)dev_alloc(c, (size_t)kMaxSeq * 5 * sizeof(int));
+  c->am_val = (float*)dev_alloc(c, (size_t)kMaxSeq * kArgmaxBlocks * sizeof(float));
+  c->am_idx = (int*)dev_alloc(c, (size_t)kMaxSeq * kArgmaxBlocks * sizeof(int));
+  c->am_ticket = (unsigned*)dev_alloc(c, kMaxSeq * sizeof(unsigned));
+  if (c->am_ticket) cudaMemsetAsync(c->am_ticket, 0, kMaxSeq * sizeof(unsigned), c->st);
+  if (!c->state || !c->tokens || !c->record || !c->bstate || !c->am_val || !c->am_idx || !c->am_ticket ||
       cudaMallocHost((void**)&c->h_state, 4 * sizeof(int)) != cudaSuccess ||
-      cudaMallocHost((void**)&c->h_logits, (size_t)hp->n_vocab * 4) != cudaSuccess) {
+      cudaMallocHost((void**)&c->h_bstate, (size_t)kMaxSeq * 5 * sizeof(int)) != cudaSuccess || alloc_sequences(c, 1)) {
     ns_llama_free(c);
     return nullptr;
   }
-  cudaMemsetAsync(c->kc, 0, kv_elems * 2, c->st);
-  cudaMemsetAsync(c->vc, 0, kv_elems * 2, c->st);
   cudaMemsetAsync(c->state, 0, 4 * sizeof(int), c->st);
   return c;
 }
@@ -1211,10 +1391,10 @@ extern "C" ns_llama* ns_llama_create(const ns_llama_hparams* hp, void* queue) {
 extern "C" void ns_llama_free(ns_llama* c) {
   if (!c) return;
   cudaStreamSynchronize(c->st);
-  if (c->decode_exec) cudaGraphExecDestroy(c->decode_exec);
-  if (c->decode_graph) cudaGraphDestroy(c->decode_graph);
+  drop_graphs(c);
   for (void* p : c->owned) cudaFree(p);
   if (c->h_state) cudaFreeHost(c->h_state);
+  if (c->h_bstate) cudaFreeHost(c->h_bstate);
   if (c->h_logits) cudaFreeHost(c->h_logits);
   delete c;
 }
@@ -1237,13 +1417,8 @@ extern "C" int ns_llama_set_f32(ns_llama* c, int tensor, int layer, const float*
                        : tensor == NS_LT_OUT_NORM ? (const float**)&c->out_norm
                        : tensor == NS_LT_ATTN_NORM ? &c->layers[layer].attn_norm
                                                    : &c->layers[layer].ffn_norm;
-  if (*slot) {  // set twice: the captured decode graph holds the old pointer
-    if (c->decode_exec) {
-      cudaGraphExecDestroy(c->decode_exec);
-      cudaGraphDestroy(c->decode_graph);
-      c->decode_exec = nullptr;
-      c->decode_graph = nullptr;
-    }
+  if (*slot) {  // set twice: the captured graphs hold the old pointer
+    drop_graphs(c);
     dev_free(c, (void*)*slot);
   }
   *slot = d;
@@ -1276,12 +1451,7 @@ extern "C" int ns_llama_set_weight(ns_llama* c, int tensor, int layer, const ns_
                            : tensor == NS_LT_WO ? &l.wo : tensor == NS_LT_W1 ? &l.w1 : tensor == NS_LT_W2 ? &l.w2 : &l.w3;
     *slot = w;
   }
-  if (c->decode_exec) {  // weights changed: the captured graph holds stale pointers
-    cudaGraphExecDestroy(c->decode_exec);
-    cudaGraphDestroy(c->decode_graph);
-    c->decode_exec = nullptr;
-    c->decode_graph = nullptr;
-  }
+  drop_graphs(c);  // weights changed: the captured graphs hold stale pointers
   return NS_OK;
 }
 
@@ -1319,16 +1489,15 @@ static int ensure_buffers(ns_llama* c, int m) {
   c->ws_bytes = wsb;
   if (!c->x || !c->xn || !c->qkv || !c->attn || !c->tmp || !c->ws) return NS_E_CUDA;
   c->m_cap = m;
-  if (c->decode_exec) {
-    cudaGraphExecDestroy(c->decode_exec);
-    cudaGraphDestroy(c->decode_graph);
-    c->decode_exec = nullptr;
-    c->decode_graph = nullptr;
-  }
+  drop_graphs(c);
   return NS_OK;
 }
 
 static int check_complete(const ns_llama* c) {
+  if (c->n_seq < 1) {
+    ns_set_error("ns_llama: no KV cache (a failed ns_llama_set_sequences)");
+    return NS_E_INVALID;
+  }
   if (!c->tok_embd || !c->out_norm || !c->output) {
     ns_set_error("ns_llama: tok_embeddings / output norm / output weight not set");
     return NS_E_INVALID;
@@ -1344,21 +1513,25 @@ static int check_complete(const ns_llama* c) {
 }
 
 // enqueue the whole forward pass for m new tokens (ids in c->tokens[0..m) or, when from_state, the single id in
-// state[0]); position base = state[1].  Leaves logits of the LAST token in c->logits and the greedy pick in state[3].
-static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int* record, bool ring) {
+// state[0]); position base = state[1]; KV block `seq`.  Leaves logits of the LAST token in c->logits and the greedy pick in
+// state[3].  batch: m rows of m different sequences instead (row i: token and position in bstate[4 i ..], KV block
+// bstate[4 kMaxSeq + i]), logits and argmax of every row, picks recorded in brecord [row][n_ctx].
+static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int* record, bool ring, int seq = 0, bool batch = false) {
   const ns_llama_hparams& hp = c->hp;
   cudaStream_t st = c->st;
   const int E = hp.n_embd, hd = E / hp.n_head, kvd = hd * hp.n_head_kv;
   float* q = c->qkv;
   float* k = q + (size_t)m * E;
   float* v = k + (size_t)m * kvd;
-  NS_CUDA_TRY(ns_launch_pdl(embed_kernel, dim3((unsigned)((E / 4 + 255) / 256), (unsigned)m), dim3(256), 0, st, (const float*)c->tok_embd,
-                            (const int*)(from_state ? c->state : c->tokens), E, hp.n_vocab, c->x));
+  const int* toks = batch ? c->bstate : from_state ? c->state : c->tokens;
+  NS_CUDA_TRY(ns_launch_pdl(batch ? embed_kernel<4> : embed_kernel<1>, dim3((unsigned)((E / 4 + 255) / 256), (unsigned)m), dim3(256), 0, st,
+                            (const float*)c->tok_embd, toks, E, hp.n_vocab, c->x));
   ns_count_launch();
+  const size_t blk = (size_t)hp.n_head_kv * hp.n_ctx * hd;  // one sequence's cache of one layer
   for (int il = 0; il < hp.n_layer; ++il) {
     const Layer& L = c->layers[il];
-    __half* kc = c->kc + (size_t)il * hp.n_head_kv * hp.n_ctx * hd;
-    __half* vc = c->vc + (size_t)il * hp.n_head_kv * hp.n_ctx * hd;
+    __half* kc = c->kc + ((size_t)il * c->n_seq + (batch ? 0 : seq)) * blk;
+    __half* vc = c->vc + ((size_t)il * c->n_seq + (batch ? 0 : seq)) * blk;
     // Decode rows: the attention RMSNorm (llama.cpp:205-210) rides in the activation quantiser of the Q/K/V launch(es) -- every
     // CTA reads the whole row anyway -- instead of a one-CTA kernel and a launch boundary of its own.
     const ns_weight* qkvw[3] = {L.wq, L.wk, L.wv};
@@ -1380,10 +1553,15 @@ static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int
           return rc;
     }
     static const int dbg_skip = getenv("NS_LLAMA_DEBUG_SKIP") ? atoi(getenv("NS_LLAMA_DEBUG_SKIP")) : 0;  // timing experiments only
-    if (!(m == 1 && (dbg_skip & 1)))  // (else results are wrong: the attention launch is left out to measure what it costs)
+    if (batch) {
+      if (int rc = launch_attention_batch(q, k, v, kc, vc, c->bstate, c->bstate + 4 * kMaxSeq, c->attn, c->attn_part, c->attn_tickets, m,
+                                          hp.n_head, hp.n_head_kv, hd, hp.n_ctx, hp.rope_theta, hp.rope_scale, c->attn_attr, st))
+        return rc;
+    } else if (!(m == 1 && (dbg_skip & 1))) {  // (else results are wrong: the attention launch is left out to measure what it costs)
       if (int rc = launch_attention(NS_ATTN_AUTO, q, k, v, kc, vc, c->state, c->attn, c->attn_part, c->attn_tickets, hp.n_head, hp.n_head_kv,
                                     hd, hp.n_ctx, m, hp.rope_theta, hp.rope_scale, c->attn_attr, st, ring ? &c->ring : nullptr))
         return rc;
+    }
     // inpFF = wo * attn + inpSA, written over x (every row is read by its own output only after the matmul finished)
     if (int rc = ns_mul_mat_engine(L.wo, c->attn, E, c->xn, E, m, c->x, c->ws, st, nullptr, 0.f)) return rc;
     // xn now holds inpFF; FFN + residual back into x, the FFN RMSNorm folded into the gate/up launch where that is a ring GEMV,
@@ -1396,19 +1574,45 @@ static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int
       if (int rc = ns_ffn_silu_residual(L.w1, L.w2, L.w3, c->attn, E, c->tmp, c->x, E, m, c->xn, c->ws, st, nullptr, 0.f, 1)) return rc;
     }
   }
-  // logits of the last token only (model_eval keeps the last row unless logits_all)
+  // logits of the last token only (model_eval keeps the last row unless logits_all); a batched step: of every row, each being
+  // its sequence's last token (llama.cpp:745-758)
+  const int rows = batch ? m : 1;
+  const float* xl = c->x + (size_t)(m - rows) * E;
   const ns_weight* outw[1] = {c->output};
-  if (ns_rmsnorm_fusable(outw, 1, 1)) {
-    if (int rc = ns_rmsnorm_mul_mat(c->output, c->x + (size_t)(m - 1) * E, E, c->out_norm, hp.norm_eps, c->logits, hp.n_vocab, 1, nullptr,
-                                    c->ws, (void*)st))
+  if (ns_rmsnorm_fusable(outw, 1, rows)) {
+    if (int rc = ns_rmsnorm_mul_mat(c->output, xl, E, c->out_norm, hp.norm_eps, c->logits, hp.n_vocab, rows, nullptr, c->ws, (void*)st))
       return rc;
   } else {
-    if (int rc = launch_rmsnorm(c->x + (size_t)(m - 1) * E, c->out_norm, c->xn, 1, E, hp.norm_eps, st)) return rc;
-    if (int rc = ns_mul_mat(c->output, c->xn, E, c->logits, hp.n_vocab, 1, nullptr, nullptr, 0, c->ws, (void*)st)) return rc;
+    if (int rc = launch_rmsnorm(xl, c->out_norm, c->xn, rows, E, hp.norm_eps, st)) return rc;
+    if (int rc = ns_mul_mat(c->output, c->xn, E, c->logits, hp.n_vocab, rows, nullptr, nullptr, 0, c->ws, (void*)st)) return rc;
   }
-  NS_CUDA_TRY(ns_launch_pdl(argmax_kernel, dim3((unsigned)kArgmaxBlocks), dim3(256), 0, st, (const float*)c->logits, hp.n_vocab, c->state, m,
-                            advance, record, c->am_val, c->am_idx, c->am_ticket));
+  NS_CUDA_TRY(ns_launch_pdl(batch ? argmax_kernel<true> : argmax_kernel<false>, dim3((unsigned)kArgmaxBlocks, (unsigned)rows), dim3(256), 0, st, (const float*)c->logits,
+                            hp.n_vocab, batch ? c->bstate : c->state, batch ? 1 : m, advance, record, hp.n_ctx, c->am_val, c->am_idx,
+                            c->am_ticket));
   ns_count_launch();
+  return NS_OK;
+}
+
+static int ensure_batch_graph(ns_llama* c, int n) {
+  if (c->batch_exec[n]) return NS_OK;
+  // as ensure_decode_graph: one eager pass that does not advance the rows (it writes the K/V rows the captured pass rewrites
+  // with the same values), then the capture
+  if (int rc = enqueue_forward(c, n, true, 0, nullptr, false, 0, true)) return rc;
+  NS_CUDA_TRY(cudaStreamSynchronize(c->st));
+  NS_CUDA_TRY(cudaStreamBeginCapture(c->st, cudaStreamCaptureModeThreadLocal));
+  int rc = enqueue_forward(c, n, true, 1, c->brecord, false, 0, true);
+  cudaGraph_t g = nullptr;
+  cudaError_t e = cudaStreamEndCapture(c->st, &g);
+  if (rc) {
+    if (g) cudaGraphDestroy(g);
+    return rc;
+  }
+  if (!ns_cuda_ok(e, "cudaStreamEndCapture") || !g) return NS_E_CUDA;
+  if (!ns_cuda_ok(cudaGraphInstantiate(&c->batch_exec[n], g, 0), "cudaGraphInstantiate")) {
+    cudaGraphDestroy(g);
+    return NS_E_CUDA;
+  }
+  c->batch_graph[n] = g;
   return NS_OK;
 }
 
@@ -1444,20 +1648,16 @@ extern "C" int ns_llama_set_exact_prefill(ns_llama* c, int on) {
   return NS_OK;
 }
 
-static void drop_decode_graph(ns_llama* c) {
-  if (!c->decode_exec) return;
-  cudaGraphExecDestroy(c->decode_exec);
-  cudaGraphDestroy(c->decode_graph);
-  c->decode_exec = nullptr;
-  c->decode_graph = nullptr;
-}
-
 extern "C" int ns_llama_set_streaming(ns_llama* c, int n_keep) {
   if (!c || n_keep < -1 || n_keep >= c->hp.n_ctx) {
     ns_set_error("ns_llama_set_streaming: n_keep %d outside [-1, n_ctx)", n_keep);
     return NS_E_INVALID;
   }
   const int hd = c->hp.n_embd / c->hp.n_head;
+  if (n_keep >= 0 && c->n_seq > 1) {
+    ns_set_error("ns_llama_set_streaming: %d sequences (the ring serves one; llama.cpp:104 forbids the pair)", c->n_seq);
+    return NS_E_UNSUPPORTED;
+  }
   if (n_keep >= 0 && c->hp.rope_scale != 1.f) {
     ns_set_error("ns_llama_set_streaming: rope_scale %g != 1 (the reference's positions and shift table disagree)", c->hp.rope_scale);
     return NS_E_UNSUPPORTED;
@@ -1467,7 +1667,7 @@ extern "C" int ns_llama_set_streaming(ns_llama* c, int n_keep) {
     return NS_E_UNSUPPORTED;
   }
   NS_CUDA_TRY(cudaStreamSynchronize(c->st));  // nothing in flight replays the graph dropped below
-  drop_decode_graph(c);
+  drop_graphs(c);
   c->streaming = n_keep >= 0;
   c->ring = Ring{n_keep, c->streaming ? shift_table(hd, c->hp.rope_theta) : ShiftTable{}};
   c->wrapped = false;
@@ -1500,12 +1700,9 @@ static void advance_position(ns_llama* c, int n_past, int n) {
   c->wrapped = c->streaming && ((c->wrapped && n_past > c->ring.n_keep) || n_past + n > c->hp.n_ctx);
 }
 
-extern "C" int ns_llama_eval(ns_llama* c, const int32_t* tokens, int n_tokens, int n_past, float* logits_host, int32_t* next_token) {
-  if (int rc = ns_ensure_device()) return rc;
-  if (!c || !tokens || n_tokens <= 0 || n_past < 0) {
-    ns_set_error("ns_llama_eval: invalid arguments (n_tokens=%d n_past=%d n_ctx=%d)", n_tokens, n_past, c ? c->hp.n_ctx : 0);
-    return NS_E_INVALID;
-  }
+// ns_llama_eval on KV block `seq`: block 0 one-token steps replay the decode graph, every other step (prompts, and single
+// tokens of the other blocks, whose graph would bake in the block) runs the same kernels eagerly
+static int eval_block(ns_llama* c, int seq, const int32_t* tokens, int n_tokens, int n_past, float* logits_host, int32_t* next_token) {
   if (c->streaming && n_tokens > 1 && n_past + n_tokens > c->hp.n_ctx) {
     // the reference masks a multi-token step in slot order, which means nothing in ring order (llama.cpp:467, a TODO there)
     ns_set_error("ns_llama_eval: %d tokens past n_ctx %d: the ring takes one token per step", n_tokens, c->hp.n_ctx);
@@ -1518,7 +1715,7 @@ extern "C" int ns_llama_eval(ns_llama* c, const int32_t* tokens, int n_tokens, i
     for (int t0 = 0; t0 < n_tokens; t0 += 32) {
       const int nt = n_tokens - t0 < 32 ? n_tokens - t0 : 32;
       const bool last = t0 + nt == n_tokens;
-      if (int rc = ns_llama_eval(c, tokens + t0, nt, n_past + t0, last ? logits_host : nullptr, last ? next_token : nullptr)) return rc;
+      if (int rc = eval_block(c, seq, tokens + t0, nt, n_past + t0, last ? logits_host : nullptr, last ? next_token : nullptr)) return rc;
     }
     return NS_OK;
   }
@@ -1530,12 +1727,12 @@ extern "C" int ns_llama_eval(ns_llama* c, const int32_t* tokens, int n_tokens, i
   c->h_state[2] = 0;
   c->h_state[3] = 0;
   NS_CUDA_TRY(cudaMemcpyAsync(c->state, c->h_state, 4 * sizeof(int), cudaMemcpyHostToDevice, st));
-  if (n_tokens == 1) {
+  if (n_tokens == 1 && seq == 0) {
     if (int rc = ensure_decode_graph(c)) return rc;
     NS_CUDA_TRY(cudaGraphLaunch(c->decode_exec, st));
   } else {
     NS_CUDA_TRY(cudaMemcpyAsync(c->tokens, tokens, (size_t)n_tokens * sizeof(int), cudaMemcpyHostToDevice, st));
-    if (int rc = enqueue_forward(c, n_tokens, false, 1, nullptr, false)) return rc;
+    if (int rc = enqueue_forward(c, n_tokens, false, 1, nullptr, false, seq)) return rc;
   }
   if (logits_host) NS_CUDA_TRY(cudaMemcpyAsync(c->h_logits, c->logits, (size_t)c->hp.n_vocab * 4, cudaMemcpyDeviceToHost, st));
   NS_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->state, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1543,6 +1740,117 @@ extern "C" int ns_llama_eval(ns_llama* c, const int32_t* tokens, int n_tokens, i
   if (logits_host) memcpy(logits_host, c->h_logits, (size_t)c->hp.n_vocab * 4);
   if (next_token) *next_token = c->h_state[3];
   advance_position(c, n_past, n_tokens);
+  return NS_OK;
+}
+
+extern "C" int ns_llama_eval(ns_llama* c, const int32_t* tokens, int n_tokens, int n_past, float* logits_host, int32_t* next_token) {
+  if (int rc = ns_ensure_device()) return rc;
+  if (!c || !tokens || n_tokens <= 0 || n_past < 0) {
+    ns_set_error("ns_llama_eval: invalid arguments (n_tokens=%d n_past=%d n_ctx=%d)", n_tokens, n_past, c ? c->hp.n_ctx : 0);
+    return NS_E_INVALID;
+  }
+  return eval_block(c, 0, tokens, n_tokens, n_past, logits_host, next_token);
+}
+
+extern "C" int ns_llama_eval_seq(ns_llama* c, int seq, const int32_t* tokens, int n_tokens, int n_past, float* logits_host,
+                                 int32_t* next_token) {
+  if (int rc = ns_ensure_device()) return rc;
+  if (!c || !tokens || n_tokens <= 0 || n_past < 0) {
+    ns_set_error("ns_llama_eval_seq: invalid arguments (n_tokens=%d n_past=%d n_ctx=%d)", n_tokens, n_past, c ? c->hp.n_ctx : 0);
+    return NS_E_INVALID;
+  }
+  if (seq < 0 || seq >= c->n_seq) {
+    ns_set_error("ns_llama_eval_seq: sequence id %d outside [0, %d)", seq, c->n_seq);
+    return NS_E_INVALID;
+  }
+  return eval_block(c, seq, tokens, n_tokens, n_past, logits_host, next_token);
+}
+
+// 1 <= n_seq <= 32 KV blocks: every block restarts empty
+extern "C" int ns_llama_set_sequences(ns_llama* c, int n_seq) {
+  if (!c || n_seq < 1 || n_seq > kMaxSeq) {
+    ns_set_error("ns_llama_set_sequences: n_seq %d outside [1, %d]", n_seq, kMaxSeq);
+    return NS_E_INVALID;
+  }
+  const int hd = c->hp.n_embd / c->hp.n_head;
+  if (n_seq > 1 && c->streaming) {
+    ns_set_error("ns_llama_set_sequences: %d sequences with streaming on (llama.cpp:104 forbids the pair)", n_seq);
+    return NS_E_UNSUPPORTED;
+  }
+  if (n_seq > 1 && hd != 64 && hd != 128) {
+    ns_set_error("ns_llama_set_sequences: head size %d (the batched decode attention takes 64 or 128)", hd);
+    return NS_E_UNSUPPORTED;
+  }
+  NS_CUDA_TRY(cudaStreamSynchronize(c->st));  // nothing in flight uses the blocks or graphs released below
+  drop_graphs(c);
+  c->n_total = 0;
+  c->wrapped = false;
+  return alloc_sequences(c, n_seq);
+}
+
+// argument checks and the rows' device state of a batched call (no launch when the call is refused)
+static int start_batch(ns_llama* c, const char* who, int n, const int* seq, const int32_t* tokens, const int* n_past, int steps) {
+  if (!c || !seq || !tokens || !n_past) {
+    ns_set_error("%s: null pointer", who);
+    return NS_E_INVALID;
+  }
+  if (steps <= 0) {
+    ns_set_error("%s: %d steps", who, steps);
+    return NS_E_INVALID;
+  }
+  if (int rc = check_rows(who, c->n_seq, n, seq, n_past, steps, c->hp.n_ctx)) return rc;
+  const int hd = c->hp.n_embd / c->hp.n_head;
+  if (hd != 64 && hd != 128) {
+    ns_set_error("%s: head size %d (the batched decode attention takes 64 or 128)", who, hd);
+    return NS_E_UNSUPPORTED;
+  }
+  if (c->streaming) {
+    ns_set_error("%s: streaming is on (the ring serves ns_llama_eval / ns_llama_generate only)", who);
+    return NS_E_UNSUPPORTED;
+  }
+  if (int rc = check_complete(c)) return rc;
+  if (int rc = ensure_buffers(c, n)) return rc;
+  for (int i = 0; i < kMaxSeq; ++i) {
+    int* r = c->h_bstate + 4 * i;
+    r[0] = i < n ? tokens[i] : 0;
+    r[1] = i < n ? n_past[i] : 0;
+    r[2] = r[3] = 0;
+    c->h_bstate[4 * kMaxSeq + i] = i < n ? seq[i] : 0;
+  }
+  NS_CUDA_TRY(cudaMemcpyAsync(c->bstate, c->h_bstate, (size_t)kMaxSeq * 5 * sizeof(int), cudaMemcpyHostToDevice, c->st));
+  return ensure_batch_graph(c, n);
+}
+
+extern "C" int ns_llama_decode_batch(ns_llama* c, int n, const int* seq, const int32_t* tokens, const int* n_past, float* logits_host,
+                                     int32_t* next_tokens) {
+  if (int rc = ns_ensure_device()) return rc;
+  if (int rc = start_batch(c, "ns_llama_decode_batch", n, seq, tokens, n_past, 1)) return rc;
+  cudaStream_t st = c->st;
+  const size_t nl = (size_t)n * c->hp.n_vocab;
+  NS_CUDA_TRY(cudaGraphLaunch(c->batch_exec[n], st));
+  if (logits_host) NS_CUDA_TRY(cudaMemcpyAsync(c->h_logits, c->logits, nl * 4, cudaMemcpyDeviceToHost, st));
+  NS_CUDA_TRY(cudaMemcpyAsync(c->h_bstate, c->bstate, (size_t)n * 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
+  NS_CUDA_TRY(cudaStreamSynchronize(st));
+  if (logits_host) memcpy(logits_host, c->h_logits, nl * 4);
+  if (next_tokens)
+    for (int i = 0; i < n; ++i) next_tokens[i] = c->h_bstate[4 * i + 3];
+  return NS_OK;
+}
+
+extern "C" int ns_llama_generate_batch(ns_llama* c, int n, const int* seq, const int32_t* first_tokens, const int* n_past, int n_new,
+                                       int32_t* out_tokens) {
+  if (int rc = ns_ensure_device()) return rc;
+  if (!out_tokens) {
+    ns_set_error("ns_llama_generate_batch: null pointer");
+    return NS_E_INVALID;
+  }
+  if (int rc = start_batch(c, "ns_llama_generate_batch", n, seq, first_tokens, n_past, n_new)) return rc;
+  cudaStream_t st = c->st;
+  for (int i = 0; i < n_new; ++i) NS_CUDA_TRY(cudaGraphLaunch(c->batch_exec[n], st));
+  // row r's picks: brecord[r][0 .. n_new) (n_past + n_new <= n_ctx)
+  NS_CUDA_TRY(cudaMemcpy2DAsync(out_tokens, (size_t)n_new * sizeof(int), c->brecord, (size_t)c->hp.n_ctx * sizeof(int),
+                                (size_t)n_new * sizeof(int), (size_t)n, cudaMemcpyDeviceToHost, st));
+  NS_CUDA_TRY(cudaStreamSynchronize(st));
   return NS_OK;
 }
 
@@ -1578,5 +1886,5 @@ extern "C" int ns_llama_generate(ns_llama* c, int32_t first_token, int n_past, i
 
 extern "C" unsigned long long ns_llama_kv_bytes(const ns_llama* c) {
   if (!c) return 0;
-  return (unsigned long long)2 * c->hp.n_layer * c->hp.n_head_kv * c->hp.n_ctx * (c->hp.n_embd / c->hp.n_head) * 2;
+  return (unsigned long long)2 * c->n_seq * c->hp.n_layer * c->hp.n_head_kv * c->hp.n_ctx * (c->hp.n_embd / c->hp.n_head) * 2;
 }
