@@ -364,6 +364,29 @@ NS_API int ns_llama_decode_batch(ns_llama* ctx, int n, const int* seq, const int
  * n_past[i] + n_new <= n_ctx; argument rules as ns_llama_decode_batch */
 NS_API int ns_llama_generate_batch(ns_llama* ctx, int n, const int* seq, const int32_t* first_tokens, const int* n_past,
                                    int n_new, int32_t* out_tokens);
+/* One forward pass over n segments of n DISTINCT sequences (model_eval with n_input inputs, llama.cpp:53-90, 329-460, 745-758).
+ * Segment i is n_tokens[i] >= 1 tokens of sequence seq[i], appended at positions n_past[i] ..; tokens holds all segments back to
+ * back (T = sum n_tokens rows).  logits_host (nullable) [n][n_vocab]: each segment's LAST token, in the caller's order;
+ * next_tokens (nullable) [n]: greedy picks.  New prompts, prompt chunks at n_past > 0 and the decode tokens of running
+ * sequences share one pass: every matmul reads its weights once for all T rows.
+ * Every matmul node is routed by ns_route at T rows, as a prompt of T tokens is (so a decode token in a pass of T > 32 rows takes
+ * the bf16 wgmma GEMM for that step); the one-token segments' attention is ns_llama_decode_batch's, each longer segment's is
+ * the tensor-core prompt attention (NS_ATTN_MMA) on its block, bit for bit -- also for 2 .. 7 tokens, where ns_llama_eval_seq
+ * takes NS_ATTN_ROWS.  When every segment has one token the call is ns_llama_decode_batch (its captured graph); other passes
+ * run eagerly.  NS_E_INVALID (nothing launched) for n outside [1, n_seq], a sequence id outside [0, n_seq) or given twice,
+ * n_tokens[i] < 1, n_past[i] < 0 or n_past[i] + n_tokens[i] > n_ctx, T > 4096 rows (a fixed cap per call: chunk longer
+ * prompts), null pointers; NS_E_UNSUPPORTED with streaming on, a head size other than 64 / 128, or exact-prefill mode with
+ * T > 32 (its integer block sums hold up to 32 rows). */
+NS_API int ns_llama_eval_batch(ns_llama* ctx, int n, const int* seq, const int* n_tokens, const int32_t* tokens,
+                               const int* n_past, float* logits_host, int32_t* next_tokens);
+/* The host plan of ns_llama_eval_batch on its own (no device needed): the argument rules above that return NS_E_INVALID, for a
+ * context of n_seq KV blocks of n_ctx positions, and the layout of the pass.  Internal order: the one-token segments first,
+ * then the longer ones, each group in the caller's order.  order [n]: caller index of internal segment j; rows [T][2]:
+ * {position, KV block} of internal row r; tiles [>= T / 64 + n][5]: one entry per 64 query rows of each multi-token segment,
+ * {segment's first row counted from internal row d, its length, its n_past, its block, the tile's first query row inside the
+ * segment}; counts [3] = {T, d = number of one-token segments, number of tile entries}. */
+NS_API int ns_llama_batch_plan(int n_seq, int n_ctx, int n, const int* seq, const int* n_tokens, const int* n_past, int* order,
+                               int* rows, int* tiles, int* counts);
 NS_API unsigned long long ns_llama_kv_bytes(const ns_llama* ctx); /* all n_seq blocks */
 /* One layer's attention of the eval step on its own, for parity tests: RoPE (mode 0, angle = p * rope_theta^(-2i/hd) / rope_scale)
  * of q [m][n_head * hd] in place and of the m new rows k [m][n_head_kv * hd] at positions n_past .. n_past + m - 1, k and v appended
@@ -404,6 +427,16 @@ NS_API size_t ns_llama_attention_batch_workspace_bytes(int n, int n_head, int hd
 NS_API int ns_llama_attention_batch(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n,
                                     const int* seq, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
                                     float rope_theta, float rope_scale, float* out, void* ws, void* queue);
+/* One layer's ragged prompt attention on its own, for parity tests (as one ns_llama_attention(NS_ATTN_MMA) call per segment on
+ * that segment's block): segment i is n_tokens[i] >= 1 rows of sequence seq[i] at positions n_past[i] .., the segments back to
+ * back in the caller's order (T = sum n_tokens rows).  q [T][n_head * hd] is rotated in place, k / v [T][n_head_kv * hd] are
+ * rotated / appended to the caches [n_seq][n_head_kv][n_ctx][hd] fp16, out [T][n_head * hd].  Argument rules of
+ * ns_llama_eval_batch (NS_E_INVALID, nothing launched), hd 64 / 128 (else NS_E_UNSUPPORTED).  ws: device workspace of
+ * ns_llama_attention_ragged_workspace_bytes(n, T) bytes: int rows[T][2] | int tiles[T / 64 + n][5], written by the call. */
+NS_API size_t ns_llama_attention_ragged_workspace_bytes(int n, int n_rows);
+NS_API int ns_llama_attention_ragged(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n, const int* seq,
+                                     const int* n_tokens, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
+                                     float rope_theta, float rope_scale, float* out, void* ws, void* queue);
 
 /* ---- tensor-parallel exchange step over NVLink peer memory (SURVEY 8e) --------------------------------------------
  * One-shot sum all-reduce replacing reduce_add / ne_all_reduce (core/parallel_context.cpp:47, ne_layers.c:5466) for the

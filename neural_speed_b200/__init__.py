@@ -62,6 +62,7 @@ EXPORTS = [
     "ns_llama_set_streaming", "ns_llama_kv_bytes", "ns_llama_attention_workspace_bytes", "ns_llama_attention", "ns_llama_attention_ring",
     "ns_llama_set_sequences", "ns_llama_eval_seq", "ns_llama_decode_batch", "ns_llama_generate_batch",
     "ns_llama_attention_batch_workspace_bytes", "ns_llama_attention_batch",
+    "ns_llama_eval_batch", "ns_llama_batch_plan", "ns_llama_attention_ragged_workspace_bytes", "ns_llama_attention_ragged",
     "ns_comm_handle_bytes", "ns_comm_create", "ns_comm_get_handle", "ns_comm_open_peers", "ns_comm_link_local", "ns_comm_all_reduce_f32",
     "ns_comm_status", "ns_comm_free",
 ]
@@ -195,6 +196,11 @@ def lib() -> C.CDLL:
     L.ns_llama_attention_batch_workspace_bytes.restype = sz
     L.ns_llama_attention_batch_workspace_bytes.argtypes = [i, i, i, i]
     L.ns_llama_attention_batch.argtypes = [vp, vp, vp, vp, vp, i, i, vp, vp, i, i, i, i, C.c_float, C.c_float, vp, vp, vp]
+    L.ns_llama_eval_batch.argtypes = [vp, i, vp, vp, vp, vp, vp, vp]
+    L.ns_llama_batch_plan.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp]
+    L.ns_llama_attention_ragged_workspace_bytes.restype = sz
+    L.ns_llama_attention_ragged_workspace_bytes.argtypes = [i, i]
+    L.ns_llama_attention_ragged.argtypes = [vp, vp, vp, vp, vp, i, i, vp, vp, vp, i, i, i, i, C.c_float, C.c_float, vp, vp, vp]
     L.ns_comm_handle_bytes.restype = sz
     L.ns_comm_create.restype = vp
     L.ns_comm_create.argtypes = [i, i, sz, vp]
@@ -530,6 +536,20 @@ class Llama:
                                            _np_ptr(nxt)), "ns_llama_decode_batch")
         return logits, nxt
 
+    def eval_batch(self, seqs, token_lists, n_past, want_logits=True):
+        """one forward pass over a token segment of each of the distinct sequences `seqs` (new prompts, prompt chunks and decode
+        tokens together) -> (logits of each segment's last token [n][n_vocab] or None, picks [n])"""
+        s, p = (np.ascontiguousarray(a, np.int32) for a in (seqs, n_past))
+        parts = [np.asarray(x, np.int32).ravel() for x in token_lists]
+        lens = np.array([x.size for x in parts], np.int32)
+        t = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0, np.int32))
+        n = s.size
+        logits = np.empty((n, self.hp.n_vocab), np.float32) if want_logits else None
+        nxt = np.empty(n, np.int32)
+        _check(lib().ns_llama_eval_batch(self.h, n, _np_ptr(s), _np_ptr(lens), _np_ptr(t), _np_ptr(p),
+                                         _np_ptr(logits) if want_logits else None, _np_ptr(nxt)), "ns_llama_eval_batch")
+        return logits, nxt
+
     def generate_batch(self, seqs, first_tokens, n_past, n_new: int) -> np.ndarray:
         """greedy generation of n_new tokens for each sequence, picks fed back on the device -> [n][n_new]"""
         s, t, p = (np.ascontiguousarray(a, np.int32) for a in (seqs, first_tokens, n_past))
@@ -557,3 +577,28 @@ def attention_batch(q_ptr: int, k_ptr: int, v_ptr: int, kc_ptr: int, vc_ptr: int
     return lib().ns_llama_attention_batch(C.c_void_p(q_ptr), C.c_void_p(k_ptr), C.c_void_p(v_ptr), C.c_void_p(kc_ptr), C.c_void_p(vc_ptr),
                                           n_seq, s.size, _np_ptr(s), _np_ptr(p), n_head, n_head_kv, hd, n_ctx, rope_theta, rope_scale,
                                           C.c_void_p(out_ptr), C.c_void_p(ws_ptr), queue)
+
+
+def attention_ragged(q_ptr: int, k_ptr: int, v_ptr: int, kc_ptr: int, vc_ptr: int, n_seq: int, seqs, n_tokens, n_past, n_head: int,
+                     n_head_kv: int, hd: int, n_ctx: int, out_ptr: int, ws_ptr: int, rope_theta=10000.0, rope_scale=1.0, queue=None) -> int:
+    """ns_llama_attention_ragged on device pointers (one layer's ragged prompt attention); returns the status code"""
+    s, t, p = (np.ascontiguousarray(a, np.int32) for a in (seqs, n_tokens, n_past))
+    return lib().ns_llama_attention_ragged(C.c_void_p(q_ptr), C.c_void_p(k_ptr), C.c_void_p(v_ptr), C.c_void_p(kc_ptr), C.c_void_p(vc_ptr),
+                                           n_seq, s.size, _np_ptr(s), _np_ptr(t), _np_ptr(p), n_head, n_head_kv, hd, n_ctx, rope_theta,
+                                           rope_scale, C.c_void_p(out_ptr), C.c_void_p(ws_ptr), queue)
+
+
+def batch_plan(n_seq: int, n_ctx: int, seqs, n_tokens, n_past):
+    """ns_llama_batch_plan (host only) -> (status, plan): plan = dict(order [n], rows [T][2] {position, block}, d, tiles [k][5])
+    on success, None on a refused call (the reason in last_error())"""
+    s, t, p = (np.ascontiguousarray(a, np.int32) for a in (seqs, n_tokens, n_past))
+    T = int(np.clip(t, 0, None).sum()) if t.size else 0
+    order = np.zeros(max(s.size, 1), np.int32)
+    rows = np.zeros((max(T, 1), 2), np.int32)
+    tiles = np.zeros((T // 64 + s.size + 1, 5), np.int32)
+    counts = np.zeros(3, np.int32)
+    rc = lib().ns_llama_batch_plan(n_seq, n_ctx, s.size, _np_ptr(s), _np_ptr(t), _np_ptr(p), _np_ptr(order), _np_ptr(rows), _np_ptr(tiles),
+                                   _np_ptr(counts))
+    if rc != 0:
+        return rc, None
+    return rc, dict(order=order[:s.size], rows=rows[:counts[0]], d=int(counts[1]), tiles=tiles[:counts[2]])

@@ -20,6 +20,7 @@
 // rounded to fp16 (table_exp_f16, ne_layers.c:8933-8937); rms_norm as kernel_ref.h:2199-2225.
 #include <cuda_fp16.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "nsb.cuh"
@@ -97,13 +98,24 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const float* __restrict__ 
 
 // rope (mode 0) on q and k of every new token + append k,v to the fp16 cache.
 // grid (n_head + n_head_kv, n_tokens), hd/2 threads.  pos = state[1] + t.
+// RAGGED: the rows belong to segments of several sequences (ns_llama_eval_batch); row t takes its position and its KV block
+// ([n_seq][n_head_kv][n_ctx][hd]) from rows[2 t], rows[2 t + 1] instead.
+template <bool RAGGED = false>
 __global__ void rope_kv_kernel(float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk, const float* __restrict__ v, int ldv,
                                __half* __restrict__ kc, __half* __restrict__ vc, const int* __restrict__ state, int n_head, int n_head_kv,
-                               int hd, int n_ctx, float theta_scale, float freq_scale) {
+                               int hd, int n_ctx, float theta_scale, float freq_scale, const int* __restrict__ rows) {
   pdl_launch_dependents();
   pdl_wait();
   const int h = blockIdx.x, t = blockIdx.y, i = threadIdx.x;  // pair index
-  const int pos = state[1] + t;
+  int pos;
+  if (RAGGED) {
+    pos = rows[2 * t];
+    const size_t blk = (size_t)rows[2 * t + 1] * n_head_kv * n_ctx * hd;
+    kc += blk;
+    vc += blk;
+  } else {
+    pos = state[1] + t;
+  }
   // theta_base = p; repeated `theta_base *= theta_scale` (ne_layers.c:9321,9385): keep the same sequence of roundings
   float theta = (float)pos;
   for (int j = 0; j < i; ++j) theta *= theta_scale;
@@ -703,7 +715,13 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
 // CTA = 64 query rows of one head (4 warps x 16 rows); K / V tiles of 64 keys staged in shared memory with 16-byte padded rows
 // (conflict-free 32-bit B-fragment loads for K, ldmatrix.trans for V); every q-tile of a head re-reads that head's K / V through L2.
 // Bound: tensor pipe / shared-memory bandwidth (K and V of one head are 0.5 MB at 2048 positions -- L2 resident).
+//
+// RAGGED: the query rows are segments of several sequences (ns_llama_eval_batch, llama.cpp:414-489 run per input), grid
+// (tiles, n_head).  CTA x reads tiles[5 x] = {segment's first row, its length, its n_past, its KV block, the tile's first query row
+// inside the segment}, offsets q / out by the first row and kc / vc by the block, and takes pos0 = n_past, m = length.  Everything
+// after those offsets is the single-sequence code, so each segment is bit-identical to a launch of its own.
 constexpr int kAttnMmaRows = 64, kAttnMmaKeys = 64;
+constexpr int kTileInts = 5;  // ints per entry of the ragged tile table
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   const __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&h);
@@ -713,10 +731,11 @@ __device__ __forceinline__ void mma_f16_16816(float (&c)[4], const uint32_t (&a)
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-template <int HD>
+template <int HD, bool RAGGED = false>
 __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__ q, int ldq, const __half* __restrict__ kc,
                                                        const __half* __restrict__ vc, const int* __restrict__ state, float* __restrict__ out,
-                                                       int ldo, int n_head, int n_head_kv, int n_ctx, int m, float scale) {
+                                                       int ldo, int n_head, int n_head_kv, int n_ctx, int m, float scale,
+                                                       const int* __restrict__ tiles) {
   constexpr int LD = HD + 8;  // halves per shared-memory row: 16 bytes of padding rotate the banks by 4 words per row
   constexpr int KS = HD / 16, NT = HD / 8;
   __shared__ __align__(16) __half Ks[kAttnMmaKeys * LD];
@@ -725,8 +744,21 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
   pdl_wait();
   const int h = blockIdx.y, hk = h / (n_head / n_head_kv);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t4 = lane & 3;
-  const int pos0 = state[1];
-  const int q0 = blockIdx.x * kAttnMmaRows;
+  int pos0, q0;
+  if (RAGGED) {
+    const int* tl = tiles + kTileInts * blockIdx.x;
+    q += (size_t)tl[0] * ldq;
+    out += (size_t)tl[0] * ldo;
+    const size_t blk = (size_t)tl[3] * n_head_kv * n_ctx * HD;
+    kc += blk;
+    vc += blk;
+    m = tl[1];
+    pos0 = tl[2];
+    q0 = tl[4];
+  } else {
+    pos0 = state[1];
+    q0 = blockIdx.x * kAttnMmaRows;
+  }
   const int row0 = q0 + warp * 16 + g, row1 = row0 + 8;  // this thread's two query rows (token indices of the batch)
   const int total = min(pos0 + m, n_ctx);                // keys that exist
   const __half* kh = kc + (size_t)hk * n_ctx * HD;
@@ -937,6 +969,16 @@ __global__ void __launch_bounds__(256) argmax_kernel(const float* __restrict__ l
   }
 }
 
+// dst[j][:] = x[src[j]][:]   (the last row of each segment of ns_llama_eval_batch, gathered for the lm_head); grid (blocks, n)
+__global__ void __launch_bounds__(256) gather_rows_kernel(const float* __restrict__ x, const int* __restrict__ src, int n_embd,
+                                                          float* __restrict__ dst) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const float4* s = (const float4*)(x + (size_t)src[blockIdx.y] * n_embd);
+  float4* d = (float4*)(dst + (size_t)blockIdx.y * n_embd);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_embd / 4; i += gridDim.x * blockDim.x) d[i] = s[i];
+}
+
 }  // namespace
 
 // ---- one layer's attention: RoPE of q and of the m new k rows at positions state[1] + t, fp16 KV append, causal attention ------
@@ -1084,14 +1126,14 @@ static int launch_attention(int kind, float* q, const float* k, const float* v, 
     ns_count_launch();
     return NS_OK;
   }
-  NS_CUDA_TRY(ns_launch_pdl(rope_kv_kernel, dim3((unsigned)(n_head + n_head_kv), (unsigned)m), dim3((unsigned)(hd / 2)), 0, st, q, ldq, k,
-                            ldk, v, ldk, kc, vc, state, n_head, n_head_kv, hd, n_ctx, theta_scale, freq_scale));
+  NS_CUDA_TRY(ns_launch_pdl(rope_kv_kernel<false>, dim3((unsigned)(n_head + n_head_kv), (unsigned)m), dim3((unsigned)(hd / 2)), 0, st, q,
+                            ldq, k, ldk, v, ldk, kc, vc, state, n_head, n_head_kv, hd, n_ctx, theta_scale, freq_scale, (const int*)nullptr));
   ns_count_launch();
   if (kind == NS_ATTN_MMA) {  // causal attention on the tensor cores, 64 query rows per CTA
     auto kern = hd == 128 ? attn_mma_kernel<128> : attn_mma_kernel<64>;
     NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)((m + kAttnMmaRows - 1) / kAttnMmaRows), (unsigned)n_head), dim3(128), 0, st,
                               (const float*)q, ldq, (const __half*)kc, (const __half*)vc, state, out, ldq, n_head, n_head_kv, n_ctx, m,
-                              attn_scale));
+                              attn_scale, (const int*)nullptr));
   } else if (kind == NS_ATTN_ROWS) {
     auto kern = hd == 128 ? attn_fast_kernel<128, false> : attn_fast_kernel<64, false>;
     NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)n_head, (unsigned)m), dim3(kAW * 32), rows_smem, st, (const float*)q, ldq, k, ldk, v, ldk,
@@ -1232,7 +1274,160 @@ extern "C" int ns_llama_attention_batch(float* q, const float* k, const float* v
                                 rope_scale, attr, st);
 }
 
+// ---- mixed batches: token segments of several sequences in one pass (ns_llama_eval_batch) ------------------------------------
+constexpr int kMaxBatchRows = 4096;  // rows of one pass over segments; the caller chunks longer prompts
+
+// Checks the segments of a ragged call: the ids and n_past as check_rows, then 1 <= n_tokens[i], n_past[i] + n_tokens[i] <= n_ctx
+// and at most kMaxBatchRows rows in all.  *total = the number of rows.
+static int check_segments(const char* who, int n_seq, int n_ctx, int n, const int* seq, const int* n_tokens, const int* n_past, int* total) {
+  if (!seq || !n_tokens || !n_past) {
+    ns_set_error("%s: null pointer", who);
+    return NS_E_INVALID;
+  }
+  if (int rc = check_rows(who, n_seq, n, seq, n_past, 1, n_ctx)) return rc;
+  long long rows = 0;
+  for (int i = 0; i < n; ++i) {
+    if (n_tokens[i] < 1) {
+      ns_set_error("%s: segment %d: n_tokens %d < 1", who, i, n_tokens[i]);
+      return NS_E_INVALID;
+    }
+    if (n_tokens[i] > n_ctx - n_past[i]) {
+      ns_set_error("%s: sequence %d: n_past %d + %d tokens outside n_ctx %d", who, seq[i], n_past[i], n_tokens[i], n_ctx);
+      return NS_E_INVALID;
+    }
+    rows += n_tokens[i];
+  }
+  if (rows > kMaxBatchRows) {
+    ns_set_error("%s: %lld rows in one pass, at most %d (chunk longer prompts)", who, rows, kMaxBatchRows);
+    return NS_E_INVALID;
+  }
+  *total = (int)rows;
+  return NS_OK;
+}
+
+// Row layout of segments order[0 .. n) placed back to back: first[j] = first row of segment order[j], rows[2 r] / rows[2 r + 1] =
+// position / KV block of row r; the segments from j0 on also get one tile entry per 64 query rows {first row counted from the
+// first row of segment order[j0], length, n_past, block, the tile's first query row inside the segment} (attn_mma_kernel<RAGGED>).
+static void lay_out_segments(const std::vector<int>& order, int j0, const int* seq, const int* n_tokens, const int* n_past,
+                             std::vector<int>& first, std::vector<int>& rows, std::vector<int>& tiles) {
+  first.assign(order.size(), 0);
+  rows.clear();
+  tiles.clear();
+  int r = 0, r0 = 0;
+  for (size_t j = 0; j < order.size(); ++j) {
+    const int i = order[j];
+    if ((int)j == j0) r0 = r;
+    first[j] = r;
+    for (int t = 0; t < n_tokens[i]; ++t) rows.insert(rows.end(), {n_past[i] + t, seq[i]});
+    if ((int)j >= j0)
+      for (int q0 = 0; q0 < n_tokens[i]; q0 += kAttnMmaRows) tiles.insert(tiles.end(), {r - r0, n_tokens[i], n_past[i], seq[i], q0});
+    r += n_tokens[i];
+  }
+}
+
+// The plan of ns_llama_eval_batch: internal order = the one-token segments, then the longer ones, each group in the caller's order.
+// Rows 0 .. d - 1 take the batched decode attention, rows d .. T - 1 the ragged prompt attention (tile rows counted from row d).
+struct BatchPlan {
+  int T = 0, d = 0;
+  std::vector<int> order, first, rows, tiles;
+};
+
+static int plan_batch(const char* who, int n_seq, int n_ctx, int n, const int* seq, const int* n_tokens, const int* n_past, BatchPlan& p) {
+  if (int rc = check_segments(who, n_seq, n_ctx, n, seq, n_tokens, n_past, &p.T)) return rc;
+  p.order.clear();
+  for (int i = 0; i < n; ++i)
+    if (n_tokens[i] == 1) p.order.push_back(i);
+  p.d = (int)p.order.size();
+  for (int i = 0; i < n; ++i)
+    if (n_tokens[i] > 1) p.order.push_back(i);
+  lay_out_segments(p.order, p.d, seq, n_tokens, n_past, p.first, p.rows, p.tiles);
+  return NS_OK;
+}
+
+extern "C" int ns_llama_batch_plan(int n_seq, int n_ctx, int n, const int* seq, const int* n_tokens, const int* n_past, int* order,
+                                   int* rows, int* tiles, int* counts) {
+  if (!order || !rows || !tiles || !counts) {
+    ns_set_error("ns_llama_batch_plan: null pointer");
+    return NS_E_INVALID;
+  }
+  if (n_seq < 1 || n_seq > 32 || n_ctx <= 0) {
+    ns_set_error("ns_llama_batch_plan: invalid arguments (n_seq=%d n_ctx=%d)", n_seq, n_ctx);
+    return NS_E_INVALID;
+  }
+  BatchPlan p;
+  if (int rc = plan_batch("ns_llama_batch_plan", n_seq, n_ctx, n, seq, n_tokens, n_past, p)) return rc;
+  std::copy(p.order.begin(), p.order.end(), order);
+  std::copy(p.rows.begin(), p.rows.end(), rows);
+  std::copy(p.tiles.begin(), p.tiles.end(), tiles);
+  counts[0] = p.T;
+  counts[1] = p.d;
+  counts[2] = (int)p.tiles.size() / kTileInts;
+  return NS_OK;
+}
+
+// Ragged prompt attention: RoPE + KV append of n_rows rows (rows [n_rows][2] = {position, block}), then attn_mma_kernel<RAGGED> over
+// n_tiles tile entries.  q / out [n_rows][n_head * hd], k / v [n_rows][n_head_kv * hd], caches [n_seq][n_head_kv][n_ctx][hd] fp16.
+static int launch_attention_ragged(float* q, const float* k, const float* v, __half* kc, __half* vc, const int* rows, const int* tiles,
+                                   int n_rows, int n_tiles, float* out, int n_head, int n_head_kv, int hd, int n_ctx, float rope_theta,
+                                   float rope_scale, cudaStream_t st) {
+  if (hd != 64 && hd != 128) {
+    ns_set_error("ns_llama: the ragged prompt attention needs head size 64 or 128, got %d", hd);
+    return NS_E_UNSUPPORTED;
+  }
+  const int ldq = n_head * hd, ldk = n_head_kv * hd;
+  const float theta_scale = powf(rope_theta, -2.0f / (float)hd);  // as launch_attention
+  const float freq_scale = 1.f / rope_scale;
+  const float attn_scale = 1.0f / sqrtf((float)hd);
+  NS_CUDA_TRY(ns_launch_pdl(rope_kv_kernel<true>, dim3((unsigned)(n_head + n_head_kv), (unsigned)n_rows), dim3((unsigned)(hd / 2)), 0, st,
+                            q, ldq, k, ldk, v, ldk, kc, vc, (const int*)nullptr, n_head, n_head_kv, hd, n_ctx, theta_scale, freq_scale,
+                            rows));
+  ns_count_launch();
+  auto kern = hd == 128 ? attn_mma_kernel<128, true> : attn_mma_kernel<64, true>;
+  NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)n_tiles, (unsigned)n_head), dim3(128), 0, st, (const float*)q, ldq, (const __half*)kc,
+                            (const __half*)vc, (const int*)nullptr, out, ldq, n_head, n_head_kv, n_ctx, 0, attn_scale, tiles));
+  ns_count_launch();
+  return NS_OK;
+}
+
+// Workspace of ns_llama_attention_ragged: int rows[n_rows][2] | int tiles[n_rows / 64 + n][5]
+extern "C" size_t ns_llama_attention_ragged_workspace_bytes(int n, int n_rows) {
+  if (n <= 0 || n_rows <= 0) return 0;
+  return ((size_t)2 * n_rows + (size_t)(n_rows / kAttnMmaRows + n) * kTileInts) * sizeof(int);
+}
+
+extern "C" int ns_llama_attention_ragged(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n, const int* seq,
+                                         const int* n_tokens, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
+                                         float rope_theta, float rope_scale, float* out, void* ws, void* queue) {
+  if (int rc = ns_ensure_device()) return rc;
+  if (!q || !k || !v || !kc || !vc || !out || !ws || n_seq < 1 || n_seq > 32 || n_head <= 0 || n_head_kv <= 0 || n_head % n_head_kv ||
+      hd <= 0 || hd % 2 || n_ctx <= 0 || !(rope_theta > 0.f) || !(rope_scale > 0.f)) {
+    ns_set_error("ns_llama_attention_ragged: invalid arguments (n_seq=%d n=%d n_head=%d n_head_kv=%d hd=%d n_ctx=%d)", n_seq, n, n_head,
+                 n_head_kv, hd, n_ctx);
+    return NS_E_INVALID;
+  }
+  int n_rows = 0;
+  if (int rc = check_segments("ns_llama_attention_ragged", n_seq, n_ctx, n, seq, n_tokens, n_past, &n_rows)) return rc;
+  if (hd != 64 && hd != 128) {
+    ns_set_error("ns_llama_attention_ragged: head size %d (the ragged prompt attention takes 64 or 128)", hd);
+    return NS_E_UNSUPPORTED;
+  }
+  std::vector<int> order(n), first, rows, tiles;
+  for (int i = 0; i < n; ++i) order[i] = i;
+  lay_out_segments(order, 0, seq, n_tokens, n_past, first, rows, tiles);
+  cudaStream_t st = ns_stream_of(queue);
+  char* w = static_cast<char*>(ws);
+  // pageable sources: staged before the calls return
+  NS_CUDA_TRY(cudaMemcpyAsync(w, rows.data(), rows.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  NS_CUDA_TRY(cudaMemcpyAsync(w + (size_t)2 * n_rows * sizeof(int), tiles.data(), tiles.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  return launch_attention_ragged(q, k, v, static_cast<__half*>(kc), static_cast<__half*>(vc), reinterpret_cast<const int*>(w),
+                                 reinterpret_cast<const int*>(w + (size_t)2 * n_rows * sizeof(int)), n_rows, (int)tiles.size() / kTileInts,
+                                 out, n_head, n_head_kv, hd, n_ctx, rope_theta, rope_scale, st);
+}
+
 constexpr int kMaxSeq = 32;  // KV blocks of one context (ns_llama_set_sequences)
+constexpr int kPlanTiles = kMaxBatchRows / kAttnMmaRows + kMaxSeq;  // tile entries of one mixed pass, at most
+// device tables of a mixed pass: rows [kMaxBatchRows][2] | tiles [kPlanTiles][kTileInts] | last row of each segment [kMaxSeq]
+constexpr int kPlanInts = 2 * kMaxBatchRows + kPlanTiles * kTileInts + kMaxSeq;
 
 struct ns_llama {
   ns_llama_hparams hp;
@@ -1246,6 +1441,8 @@ struct ns_llama {
   __half *kc = nullptr, *vc = nullptr;  // [n_layer][n_seq][n_head_kv][n_ctx][hd] fp16
   int* state = nullptr;   // device: {token, n_past, n_recorded, last_pick}
   int* tokens = nullptr;  // device: prompt tokens of the current eval
+  int tok_cap = 0;        // ... their capacity: n_ctx, grown to the rows of a larger ns_llama_eval_batch pass
+  int* plan = nullptr;    // device, ns_llama_eval_batch: kPlanInts (allocated on first use)
   int* record = nullptr;  // device: generated tokens
   int* bstate = nullptr;  // device, batched steps: [kMaxSeq][4] row states as `state` | [kMaxSeq] KV block of each row
   int* brecord = nullptr;   // device, batched steps: [n_seq][n_ctx] picks of each row
@@ -1271,6 +1468,7 @@ struct ns_llama {
   cudaGraph_t batch_graph[kMaxSeq + 1] = {};
   int* h_state = nullptr;  // pinned host staging
   int* h_bstate = nullptr;  // [kMaxSeq * 5]
+  int* h_plan = nullptr;      // [kMaxBatchRows] tokens | kPlanInts tables, as `plan` (allocated with it)
   float* h_logits = nullptr;  // [n_seq][n_vocab]
 };
 
@@ -1372,6 +1570,7 @@ extern "C" ns_llama* ns_llama_create(const ns_llama_hparams* hp, void* queue) {
   }
   c->state = (int*)dev_alloc(c, 4 * sizeof(int));
   c->tokens = (int*)dev_alloc(c, (size_t)hp->n_ctx * sizeof(int));
+  c->tok_cap = hp->n_ctx;
   c->record = (int*)dev_alloc(c, (size_t)hp->n_ctx * sizeof(int));
   c->bstate = (int*)dev_alloc(c, (size_t)kMaxSeq * 5 * sizeof(int));
   c->am_val = (float*)dev_alloc(c, (size_t)kMaxSeq * kArgmaxBlocks * sizeof(float));
@@ -1395,6 +1594,7 @@ extern "C" void ns_llama_free(ns_llama* c) {
   for (void* p : c->owned) cudaFree(p);
   if (c->h_state) cudaFreeHost(c->h_state);
   if (c->h_bstate) cudaFreeHost(c->h_bstate);
+  if (c->h_plan) cudaFreeHost(c->h_plan);
   if (c->h_logits) cudaFreeHost(c->h_logits);
   delete c;
 }
@@ -1516,7 +1716,17 @@ static int check_complete(const ns_llama* c) {
 // state[0]); position base = state[1]; KV block `seq`.  Leaves logits of the LAST token in c->logits and the greedy pick in
 // state[3].  batch: m rows of m different sequences instead (row i: token and position in bstate[4 i ..], KV block
 // bstate[4 kMaxSeq + i]), logits and argmax of every row, picks recorded in brecord [row][n_ctx].
-static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int* record, bool ring, int seq = 0, bool batch = false) {
+// mix: m rows of mix->n segments of distinct sequences (ns_llama_eval_batch), ids in c->tokens; rows 0 .. d - 1 are one-token
+// segments (token, position and block in bstate as a batched step), rows d .. m - 1 the longer ones (mix->rows / mix->tiles);
+// logits and argmax (no advance) of each segment's last row, in internal order.
+struct MixedPass {
+  int n, d, n_tiles;
+  const int* rows;   // device [m][2]: {position, KV block}
+  const int* tiles;  // device [n_tiles][kTileInts], rows counted from row d
+  const int* last;   // device [n]: last row of each segment
+};
+static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int* record, bool ring, int seq = 0, bool batch = false,
+                           const MixedPass* mix = nullptr) {
   const ns_llama_hparams& hp = c->hp;
   cudaStream_t st = c->st;
   const int E = hp.n_embd, hd = E / hp.n_head, kvd = hd * hp.n_head_kv;
@@ -1553,7 +1763,17 @@ static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int
           return rc;
     }
     static const int dbg_skip = getenv("NS_LLAMA_DEBUG_SKIP") ? atoi(getenv("NS_LLAMA_DEBUG_SKIP")) : 0;  // timing experiments only
-    if (batch) {
+    if (mix) {  // kc / vc: block 0 of the layer
+      const int d = mix->d;
+      if (d > 0)
+        if (int rc = launch_attention_batch(q, k, v, kc, vc, c->bstate, c->bstate + 4 * kMaxSeq, c->attn, c->attn_part, c->attn_tickets, d,
+                                            hp.n_head, hp.n_head_kv, hd, hp.n_ctx, hp.rope_theta, hp.rope_scale, c->attn_attr, st))
+          return rc;
+      if (int rc = launch_attention_ragged(q + (size_t)d * E, k + (size_t)d * kvd, v + (size_t)d * kvd, kc, vc, mix->rows + 2 * d, mix->tiles,
+                                           m - d, mix->n_tiles, c->attn + (size_t)d * E, hp.n_head, hp.n_head_kv, hd, hp.n_ctx,
+                                           hp.rope_theta, hp.rope_scale, st))
+        return rc;
+    } else if (batch) {
       if (int rc = launch_attention_batch(q, k, v, kc, vc, c->bstate, c->bstate + 4 * kMaxSeq, c->attn, c->attn_part, c->attn_tickets, m,
                                           hp.n_head, hp.n_head_kv, hd, hp.n_ctx, hp.rope_theta, hp.rope_scale, c->attn_attr, st))
         return rc;
@@ -1576,8 +1796,14 @@ static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int
   }
   // logits of the last token only (model_eval keeps the last row unless logits_all); a batched step: of every row, each being
   // its sequence's last token (llama.cpp:745-758)
-  const int rows = batch ? m : 1;
+  const int rows = batch ? m : mix ? mix->n : 1;
   const float* xl = c->x + (size_t)(m - rows) * E;
+  if (mix) {  // each segment's last row, gathered into attn (free after the last layer)
+    NS_CUDA_TRY(ns_launch_pdl(gather_rows_kernel, dim3((unsigned)((E / 4 + 255) / 256), (unsigned)rows), dim3(256), 0, st,
+                              (const float*)c->x, mix->last, E, c->attn));
+    ns_count_launch();
+    xl = c->attn;
+  }
   const ns_weight* outw[1] = {c->output};
   if (ns_rmsnorm_fusable(outw, 1, rows)) {
     if (int rc = ns_rmsnorm_mul_mat(c->output, xl, E, c->out_norm, hp.norm_eps, c->logits, hp.n_vocab, rows, nullptr, c->ws, (void*)st))
@@ -1586,8 +1812,9 @@ static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int
     if (int rc = launch_rmsnorm(xl, c->out_norm, c->xn, rows, E, hp.norm_eps, st)) return rc;
     if (int rc = ns_mul_mat(c->output, c->xn, E, c->logits, hp.n_vocab, rows, nullptr, nullptr, 0, c->ws, (void*)st)) return rc;
   }
-  NS_CUDA_TRY(ns_launch_pdl(batch ? argmax_kernel<true> : argmax_kernel<false>, dim3((unsigned)kArgmaxBlocks, (unsigned)rows), dim3(256), 0, st, (const float*)c->logits,
-                            hp.n_vocab, batch ? c->bstate : c->state, batch ? 1 : m, advance, record, hp.n_ctx, c->am_val, c->am_idx,
+  const bool rowwise = batch || mix;  // a pick per row, in bstate
+  NS_CUDA_TRY(ns_launch_pdl(rowwise ? argmax_kernel<true> : argmax_kernel<false>, dim3((unsigned)kArgmaxBlocks, (unsigned)rows), dim3(256), 0, st, (const float*)c->logits,
+                            hp.n_vocab, rowwise ? c->bstate : c->state, rowwise ? 1 : m, advance, record, hp.n_ctx, c->am_val, c->am_idx,
                             c->am_ticket));
   ns_count_launch();
   return NS_OK;
@@ -1851,6 +2078,89 @@ extern "C" int ns_llama_generate_batch(ns_llama* c, int n, const int* seq, const
   NS_CUDA_TRY(cudaMemcpy2DAsync(out_tokens, (size_t)n_new * sizeof(int), c->brecord, (size_t)c->hp.n_ctx * sizeof(int),
                                 (size_t)n_new * sizeof(int), (size_t)n, cudaMemcpyDeviceToHost, st));
   NS_CUDA_TRY(cudaStreamSynchronize(st));
+  return NS_OK;
+}
+
+// model_eval over n inputs (llama.cpp:53-90, 329-460, 745-758): one pass over the token segments of n distinct sequences
+extern "C" int ns_llama_eval_batch(ns_llama* c, int n, const int* seq, const int* n_tokens, const int32_t* tokens, const int* n_past,
+                                   float* logits_host, int32_t* next_tokens) {
+  const char* who = "ns_llama_eval_batch";
+  if (int rc = ns_ensure_device()) return rc;
+  if (!c || !tokens) {
+    ns_set_error("%s: null pointer", who);
+    return NS_E_INVALID;
+  }
+  BatchPlan p;
+  if (int rc = plan_batch(who, c->n_seq, c->hp.n_ctx, n, seq, n_tokens, n_past, p)) return rc;
+  const int hd = c->hp.n_embd / c->hp.n_head;
+  if (hd != 64 && hd != 128) {
+    ns_set_error("%s: head size %d (the batched decode and ragged prompt attention take 64 or 128)", who, hd);
+    return NS_E_UNSUPPORTED;
+  }
+  if (c->streaming) {
+    ns_set_error("%s: streaming is on (the ring serves ns_llama_eval / ns_llama_generate only; llama.cpp:104)", who);
+    return NS_E_UNSUPPORTED;
+  }
+  if (c->exact_prefill && p.T > 32) {
+    ns_set_error("%s: %d rows in exact-prefill mode (the integer block sums hold up to 32 rows)", who, p.T);
+    return NS_E_UNSUPPORTED;
+  }
+  if (p.d == n) return ns_llama_decode_batch(c, n, seq, tokens, n_past, logits_host, next_tokens);  // its captured graph
+  if (int rc = check_complete(c)) return rc;
+  if (int rc = ensure_buffers(c, p.T)) return rc;
+  cudaStream_t st = c->st;
+  if (!c->plan) {
+    c->plan = (int*)dev_alloc(c, (size_t)kPlanInts * sizeof(int));
+    if (!c->plan) return NS_E_CUDA;
+    if (!ns_cuda_ok(cudaMallocHost((void**)&c->h_plan, (size_t)(kMaxBatchRows + kPlanInts) * sizeof(int)), "cudaMallocHost")) {
+      c->h_plan = nullptr;
+      dev_free(c, c->plan);
+      c->plan = nullptr;
+      return NS_E_CUDA;
+    }
+  }
+  if (p.T > c->tok_cap) {  // nothing captured reads c->tokens: only the eager passes in flight, drained first
+    NS_CUDA_TRY(cudaStreamSynchronize(st));
+    dev_free(c, c->tokens);
+    c->tokens = (int*)dev_alloc(c, (size_t)p.T * sizeof(int));
+    c->tok_cap = c->tokens ? p.T : 0;
+    if (!c->tokens) return NS_E_CUDA;
+  }
+  // staging: ids in internal order | rows | tiles | last rows; the one-token rows' states as a batched step's
+  int* h_tok = c->h_plan;
+  int* h_tab = c->h_plan + kMaxBatchRows;
+  std::vector<int> off(n, 0);  // first id of segment i in `tokens` (caller's order)
+  for (int i = 1; i < n; ++i) off[i] = off[i - 1] + n_tokens[i - 1];
+  for (int j = 0; j < n; ++j) {
+    const int i = p.order[j];
+    memcpy(h_tok + p.first[j], tokens + off[i], (size_t)n_tokens[i] * sizeof(int));
+    h_tab[2 * kMaxBatchRows + kPlanTiles * kTileInts + j] = p.first[j] + n_tokens[i] - 1;
+  }
+  std::copy(p.rows.begin(), p.rows.end(), h_tab);
+  std::copy(p.tiles.begin(), p.tiles.end(), h_tab + 2 * kMaxBatchRows);
+  for (int j = 0; j < kMaxSeq; ++j) {
+    int* r = c->h_bstate + 4 * j;
+    const int i = j < p.d ? p.order[j] : -1;
+    r[0] = i >= 0 ? tokens[off[i]] : 0;
+    r[1] = i >= 0 ? n_past[i] : 0;
+    r[2] = r[3] = 0;
+    c->h_bstate[4 * kMaxSeq + j] = i >= 0 ? seq[i] : 0;
+  }
+  NS_CUDA_TRY(cudaMemcpyAsync(c->tokens, h_tok, (size_t)p.T * sizeof(int), cudaMemcpyHostToDevice, st));
+  NS_CUDA_TRY(cudaMemcpyAsync(c->plan, h_tab, (size_t)kPlanInts * sizeof(int), cudaMemcpyHostToDevice, st));
+  NS_CUDA_TRY(cudaMemcpyAsync(c->bstate, c->h_bstate, (size_t)kMaxSeq * 5 * sizeof(int), cudaMemcpyHostToDevice, st));
+  const MixedPass mix{n, p.d, (int)p.tiles.size() / kTileInts, c->plan, c->plan + 2 * kMaxBatchRows,
+                      c->plan + 2 * kMaxBatchRows + kPlanTiles * kTileInts};
+  if (int rc = enqueue_forward(c, p.T, false, 0, nullptr, false, 0, false, &mix)) return rc;
+  const size_t nv = (size_t)c->hp.n_vocab;
+  if (logits_host) NS_CUDA_TRY(cudaMemcpyAsync(c->h_logits, c->logits, n * nv * 4, cudaMemcpyDeviceToHost, st));
+  NS_CUDA_TRY(cudaMemcpyAsync(c->h_bstate, c->bstate, (size_t)n * 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
+  NS_CUDA_TRY(cudaStreamSynchronize(st));
+  for (int j = 0; j < n; ++j) {  // back to the caller's order
+    const int i = p.order[j];
+    if (logits_host) memcpy(logits_host + (size_t)i * nv, c->h_logits + (size_t)j * nv, nv * 4);
+    if (next_tokens) next_tokens[i] = c->h_bstate[4 * j + 3];
+  }
   return NS_OK;
 }
 
