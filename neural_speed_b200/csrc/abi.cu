@@ -606,14 +606,22 @@ extern "C" int ns_weight_dequant_f32(const ns_weight* w, float* dst_dev, int ld,
 int ns_route(int kind, const ns_weight* const* w, int m, int flags) {
   if (kind == NS_NODE_PLAIN && w[0]->wfmt == NS_W_Q6K) return NS_PATH_Q6K;  // whatever the flags
   const int nw = kind == NS_NODE_QKV ? 3 : (kind == NS_NODE_FFN && w[1]) ? 2 : 1;  // the weights of the node's first launch
+  const int mode = kind == NS_NODE_QKV ? NS_GEMV_CONCAT : nw == 2 ? NS_GEMV_GATE_UP_SILU : NS_GEMV_PLAIN;
+  bool gemv_only = false;
   if (!(flags & (NS_MM_FORCE_GEMV | NS_MM_FORCE_TC)) && ns_gemm_imma_supported(w, nw, m)) {
-    if (kind == NS_NODE_PLAIN) return NS_PATH_IMMA;
-    if (kind == NS_NODE_QKV && w[0]->n % 2 == 0 && w[1]->n % 2 == 0) return NS_PATH_IMMA;  // QKV: q and k need an even n
-    if (kind == NS_NODE_FFN && ns_gemm_imma_supported(&w[2], 1, m)) return NS_PATH_IMMA;  // FFN: gate/up and down both, or neither
+    const bool imma = kind == NS_NODE_PLAIN ||
+                      (kind == NS_NODE_QKV && w[0]->n % 2 == 0 && w[1]->n % 2 == 0) ||  // QKV: q and k need an even n
+                      (kind == NS_NODE_FFN && ns_gemm_imma_supported(&w[2], 1, m));     // FFN: gate/up and down both, or neither
+    if (imma) {
+      if (ns_gemm_imma_planned(w, nw, mode, m) && (kind != NS_NODE_FFN || ns_gemm_imma_planned(&w[2], 1, NS_GEMV_PLAIN, m)))
+        return NS_PATH_IMMA;
+      // a launch the shared-memory planner cannot fit takes GEMV tiles: the same exact block sums, never the bf16 GEMM
+      gemv_only = true;
+    }
   }
   // The tensor-core GEMM has a fixed cost at small m (pipeline fill, split-K epilogue) while GEMV tiles keep the exact-integer
   // numerics: GEMV tiles up to 16 rows (the reference switches from its GEMV to the blocked GEMM at m > 4)
-  bool tc = !(flags & NS_MM_FORCE_GEMV) && (m > 16 || (flags & NS_MM_FORCE_TC)) && ns_gemm_tc_supported(w[0]);
+  bool tc = !gemv_only && !(flags & NS_MM_FORCE_GEMV) && (m > 16 || (flags & NS_MM_FORCE_TC)) && ns_gemm_tc_supported(w[0]);
   if (kind == NS_NODE_QKV)  // one bf16 activation image for all three: equal k, no act-order shuffles
     tc = tc && ns_gemm_tc_supported(w[1]) && ns_gemm_tc_supported(w[2]) && w[1]->k == w[0]->k && w[2]->k == w[0]->k &&
          !w[0]->shuffle && !w[1]->shuffle && !w[2]->shuffle;
@@ -635,7 +643,8 @@ static bool norm_foldable(const ns_weight* const* w, int nw, int m) {
   if (off || m < 1 || m > 2 || nw < 1) return false;
   for (int i = 0; i < nw; ++i)
     if (!w[i] || !ns_gemv_fused_quant_ok(w[i]) || w[i]->k % 8) return false;
-  return !ns_gemm_imma_supported(w, nw, m);
+  const int mode = nw == 3 ? NS_GEMV_CONCAT : nw == 2 ? NS_GEMV_GATE_UP_SILU : NS_GEMV_PLAIN;
+  return !(ns_gemm_imma_supported(w, nw, m) && ns_gemm_imma_planned(w, nw, mode, m));
 }
 
 // kpad: the widest padded input of the node's launches

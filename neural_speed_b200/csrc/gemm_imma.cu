@@ -1,4 +1,4 @@
-// gemm_imma.cu -- batched decode (5..32 activation rows): 4-bit weights x int8 activations on the INTEGER tensor cores.
+// gemm_imma.cu -- batched decode (3..32 activation rows): 4-bit weights x int8 activations on the INTEGER tensor cores.
 //
 // Replaces, for 4 < M <= 32, what the reference runs through LauncherIntKBlock + the VNNI / AMX int8 GemmCores
 // (bestla/bestla/bestla_wrapper.h:214-350, bestla_gemm.h "ICoreRowNAvx512vnniKBlock" etc.): u8 (or s8) activations quantised
@@ -631,7 +631,7 @@ int launch_m(const CUtensorMap* maps, const ImmaParams& P, const Plan& pl, int s
 
 }  // namespace
 
-// Can this (fused) matmul of m activation rows run on the integer tensor cores?
+// Does the weight format of this (fused) matmul of m activation rows belong to the integer tensor cores?
 bool ns_gemm_imma_supported(const ns_weight* const* ws, int nw, int m) {
   static const bool off = getenv("NS_NO_IMMA") != nullptr;
   static const int min_m = getenv("NS_IMMA_MIN_M") ? atoi(getenv("NS_IMMA_MIN_M")) : 3;  // measured: the 4-row GEMV tile is slower already
@@ -647,6 +647,13 @@ bool ns_gemm_imma_supported(const ns_weight* const* ws, int nw, int m) {
   if (w0->k % KS) return false;  // whole 256-k stages only (every model width is): no per-chunk tail checks in the loop
   if (w0->pitch % 16) return false;
   return true;
+}
+
+// Does the shared-memory planner find a plan for this launch (mode: NS_GEMV_*)?  The launcher runs the same make_plan, so a
+// launch the route sends here never fails for want of one.
+bool ns_gemm_imma_planned(const ns_weight* const* ws, int nw, int mode, int m) {
+  Plan pl;
+  return make_plan(ws, nw, mode, m, &pl);
 }
 
 // Workspace = activation image + split-K partial tiles + tickets.  The planner keeps tiles x ksplit <= kMaxPartialTiles when it

@@ -127,8 +127,10 @@ int ns_launch_silu_mul(const float* g, const float* u, float* out, float* aux, s
 int ns_launch_gelu(float* x, size_t total, cudaStream_t st);
 bool ns_launch_silu_mul_bf16(const ns_weight* w2, const float* g, const float* u, int m, void* ws, cudaStream_t st, int eltop, int* rc);
 
-// integer tensor-core path for 5..32 activation rows (gemm_imma.cu); modes and epilogue arguments as ns_launch_gemv
+// integer tensor-core path for 3..32 activation rows (gemm_imma.cu); modes and epilogue arguments as ns_launch_gemv.
+// supported: the weight format and row count; planned: the shared-memory planner fits the launch (mode NS_GEMV_*)
 bool ns_gemm_imma_supported(const ns_weight* const* ws, int nw, int m);
+bool ns_gemm_imma_planned(const ns_weight* const* ws, int nw, int mode, int m);
 size_t ns_gemm_imma_workspace_bound(int m, int kpad);  // enough for any weight shape the launcher accepts
 int ns_launch_gemm_imma(const ns_weight* const* ws, int nw, int mode, const float* act, int lda, float* dst, int ldo, int m,
                         const float* bias, int bias_bcast, const float* residual, int eltop, void* workspace, cudaStream_t st);

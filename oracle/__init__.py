@@ -493,6 +493,55 @@ def gemv_bound_ratio(got, a_eff, w_eff):
     return float((np.abs(np.asarray(got, np.float64) - want) / unit).max())
 
 
+def imma_act(a, comp, g):
+    """The activations of an integer block-sum matmul as the quantisers give them: (codes - zero point) int64 [M,K], scales fp32
+    [M, K/ab] and the activation block ab.  comp: 'q8_0' (quantize_row_q8_0: blocks of 32, fp16 d), 'int8' (u8 with zero points
+    per weight group) or 'int8_s8' (s8 per weight group)."""
+    a = _c(a, np.float32)
+    m, k = a.shape
+    if comp == "q8_0":
+        blk = quantize_q8_0(a).reshape(m, k // 32, 34)
+        codes = blk[:, :, 2:].copy().view(np.int8).reshape(m, k).astype(np.int64)
+        return codes, blk[:, :, :2].copy().view(np.float16).reshape(m, k // 32).astype(np.float32), 32
+    if comp == "int8":
+        q, sc, zp = btla_quantize_act_u8(a, g)
+        return q.astype(np.int64) - np.repeat(zp.astype(np.int64), g, axis=1)[:, :k], sc, g
+    q, sc = btla_quantize_act_s8(a, g)
+    return q.astype(np.int64), sc, g
+
+
+def imma_stated(a_codes, a_scale, ab, q, w_scale, w_zp, g):
+    """fp64 model of the integer block-sum matmul (gemm_imma_kernel, DESIGN.md section 4).  a_codes / a_scale / ab as imma_act;
+    q int [K,N] signed weight codes, w_scale fp32 [K/g, N] as stored, w_zp [K/g, N] or None.  Per activation block b:
+    isum_b = sum (a - za)(q - zp), an exact integer; c_b = fp32(a_scale_b * w_scale_b); t_b = isum_b * c_b (exact in fp64).
+    Returns (sum_b t_b, sum_b |t_b|, number of blocks), [M,N] float64."""
+    a = np.asarray(a_codes, np.float64)
+    w = np.asarray(q, np.float64)
+    k, n = w.shape
+    if w_zp is not None:
+        w = w - np.repeat(np.asarray(w_zp, np.float64), g, axis=0)[:k]
+    asc, wsc = np.asarray(a_scale, np.float32), np.asarray(w_scale, np.float32)
+    tot = np.zeros((a.shape[0], n))
+    mag = np.zeros((a.shape[0], n))
+    nb = k // ab
+    for b in range(nb):
+        isum = a[:, b * ab:(b + 1) * ab] @ w[b * ab:(b + 1) * ab]  # integers below 2^53: exact
+        c = np.multiply(asc[:, b, None], wsc[b * ab // g][None, :], dtype=np.float32)
+        t = isum * c.astype(np.float64)
+        tot += t
+        mag += np.abs(t)
+    return tot, mag, nb
+
+
+def imma_bound_ratio(got, tot, mag, nb, splits=16):
+    """max over outputs of |got - sum t_b| / (gamma_n sum |t_b|), n = nb + splits: one fp32 fma per block and at most `splits`
+    partial sums, each one rounding (gamma_n = n u / (1 - n u), u = 2^-24).  A correct kernel stays at or below 1."""
+    n = nb + splits
+    gam = n * 2.0 ** -24 / (1 - n * 2.0 ** -24)
+    err = np.abs(np.asarray(got, np.float64) - tot)
+    return float((err / np.maximum(gam * mag, np.finfo(np.float64).tiny)).max())
+
+
 def f32_to_bf16_bits(x):
     """RNE fp32 -> bf16 bit pattern (bestla_utils.h:146-153), vectorised."""
     u = _c(x, np.float32).view(np.uint32).astype(np.uint64)

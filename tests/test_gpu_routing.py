@@ -3,6 +3,7 @@
 The path fixes the numerics class of a call, so it must be a function of (format, m, flags) only:
   Q6_K weights (plain nodes)                      Q6_K kernel, tiles of <= 4 rows (2 launches per tile)
   3 <= m <= 32, int4 weights, integer compute     integer tensor cores (IMMA): 2 launches per launch set; FFN: both halves or neither
+                                                  (GEMV tiles when its shared-memory planner cannot fit a launch of the node)
   m > 16 or NS_MM_FORCE_TC                        wgmma GEMM (bf16): activation image + one GEMM per weight
   otherwise, or NS_MM_FORCE_GEMV                  GEMV tiles of <= 4 rows: 1 launch per tile on the ring (int4 weights with an
                                                   integer compute type quantise their own activations), else act_prep + GEMV
