@@ -387,6 +387,48 @@ NS_API int ns_llama_eval_batch(ns_llama* ctx, int n, const int* seq, const int* 
  * segment}; counts [3] = {T, d = number of one-token segments, number of tile entries}. */
 NS_API int ns_llama_batch_plan(int n_seq, int n_ctx, int n, const int* seq, const int* n_tokens, const int* n_past, int* order,
                                int* rows, int* tiles, int* counts);
+/* ---- sampling (the reference's Model.generate(do_sample=True): model_post_sample_top_k_top_p_repeat, model_utils.cpp:2987-3032)
+ * Per row, in this order: the repetition penalty on every candidate whose id occurs in the sequence's window (once per id:
+ * logit <= 0 ? logit * penalty : logit / penalty), the top_k largest logits (ties: lower id first), top-p on their fp32 softmax
+ * (the first i >= 1 whose running sum passes top_p is dropped with everything after it), logits / temperature, an fp32 softmax,
+ * and a draw of std::discrete_distribution on one std::mt19937(seed) for the whole context (GCC libstdc++'s arithmetic; a list
+ * of one candidate takes it without drawing).  Rows of a batch draw in the caller's order.  The exp is the library's own
+ * (ns_sample_expf_host), within 1 ulp of glibc's expf.
+ * Window of a sequence: its last W = min(repeat_last_n, n_ctx) evaluated tokens, preceded by zeros (the reference's history
+ * starts as n_ctx zeros, application/main_pybind.cpp:460-474), including every token of the pass that samples.  Windows are kept
+ * only while sampling is on: tokens evaluated with sampling off are in no window.  A sequence's window restarts as zeros when one
+ * of its segments is evaluated at n_past == 0, and every window does on ns_llama_set_sampling and ns_llama_set_sequences. */
+typedef struct ns_llama_sampling {
+  int top_k;            /* 1 .. 1024 (NS_E_UNSUPPORTED above: the limit of the device selection) */
+  float top_p;          /* (0, 1]; 1 = off */
+  float temperature;    /* finite, > 0 */
+  float repeat_penalty; /* finite, > 0; 1 = off */
+  int repeat_last_n;    /* 0 .. 256 (the reference uses 64) */
+  uint32_t seed;        /* std::mt19937(seed); a time-based seed is the caller's choice */
+} ns_llama_sampling;
+/* s non-null: sample from now on -- reseeds the generator and restarts every window; NULL: greedy (the default).  Either drops
+ * the captured graphs.  Picks returned and fed back by ns_llama_eval, ns_llama_eval_seq, ns_llama_generate (also past n_ctx on
+ * the streaming ring), ns_llama_decode_batch, ns_llama_generate_batch and ns_llama_eval_batch are then sampled; returned
+ * logits stay the raw logits.  The sampler takes the argmax's launch, so every step launches as many kernels as greedy.
+ * NS_E_INVALID (mode unchanged) for a field out of range; NS_E_UNSUPPORTED for top_k > 1024. */
+NS_API int ns_llama_set_sampling(ns_llama* ctx, const ns_llama_sampling* s);
+/* The sampler on its own, for parity tests: one launch over device logits [n][n_vocab] (1 <= n <= 32), device windows
+ * [n][n_window] (0 <= n_window <= 256; every entry counts, repeat_last_n is not read) and a device generator mt_state[625] (as
+ * ns_sample_seed_host writes it; advanced by the call).  picks [n] device; kept [n], ids [n][top_k] (the top_k list in selection
+ * order) and probs [n][top_k] (the final probabilities of the kept entries, 0 after them), device and nullable.  ws: device
+ * workspace of ns_llama_sample_workspace_bytes(n, top_k) bytes, zeroed once by the caller: its tickets lie in the first 144
+ * bytes for every n and top_k and are zero again after every call.  NS_E_INVALID / NS_E_UNSUPPORTED as ns_llama_set_sampling, and for bad sizes or null pointers; a refused call
+ * launches nothing. */
+NS_API size_t ns_llama_sample_workspace_bytes(int n, int top_k);
+NS_API int ns_llama_sample(const float* logits, int n, int n_vocab, const int32_t* windows, int n_window, const ns_llama_sampling* s,
+                           uint32_t* mt_state, int32_t* picks, int* kept, int32_t* ids, float* probs, void* ws, void* queue);
+/* Host restatements (no device needed): std::mt19937(seed) as 625 words; steps 2-7 for one row of n_vocab logits with the window
+ * window[0 .. n_window) -- pick, kept count, ids [top_k] and probs [top_k] as ns_llama_sample writes them -- advancing `state`;
+ * and the sampler's exp. */
+NS_API void ns_sample_seed_host(uint32_t seed, uint32_t* state);
+NS_API int ns_sample_row_host(const float* logits, int n_vocab, const int32_t* window, int n_window, const ns_llama_sampling* s,
+                              uint32_t* state, int32_t* pick, int* kept, int32_t* ids, float* probs);
+NS_API float ns_sample_expf_host(float x);
 NS_API unsigned long long ns_llama_kv_bytes(const ns_llama* ctx); /* all n_seq blocks */
 /* One layer's attention of the eval step on its own, for parity tests: RoPE (mode 0, angle = p * rope_theta^(-2i/hd) / rope_scale)
  * of q [m][n_head * hd] in place and of the m new rows k [m][n_head_kv * hd] at positions n_past .. n_past + m - 1, k and v appended

@@ -63,6 +63,8 @@ EXPORTS = [
     "ns_llama_set_sequences", "ns_llama_eval_seq", "ns_llama_decode_batch", "ns_llama_generate_batch",
     "ns_llama_attention_batch_workspace_bytes", "ns_llama_attention_batch",
     "ns_llama_eval_batch", "ns_llama_batch_plan", "ns_llama_attention_ragged_workspace_bytes", "ns_llama_attention_ragged",
+    "ns_llama_set_sampling", "ns_llama_sample_workspace_bytes", "ns_llama_sample", "ns_sample_seed_host", "ns_sample_row_host",
+    "ns_sample_expf_host",
     "ns_comm_handle_bytes", "ns_comm_create", "ns_comm_get_handle", "ns_comm_open_peers", "ns_comm_link_local", "ns_comm_all_reduce_f32",
     "ns_comm_status", "ns_comm_free",
 ]
@@ -201,6 +203,15 @@ def lib() -> C.CDLL:
     L.ns_llama_attention_ragged_workspace_bytes.restype = sz
     L.ns_llama_attention_ragged_workspace_bytes.argtypes = [i, i]
     L.ns_llama_attention_ragged.argtypes = [vp, vp, vp, vp, vp, i, i, vp, vp, vp, i, i, i, i, C.c_float, C.c_float, vp, vp, vp]
+    L.ns_llama_set_sampling.argtypes = [vp, vp]
+    L.ns_llama_sample_workspace_bytes.restype = sz
+    L.ns_llama_sample_workspace_bytes.argtypes = [i, i]
+    L.ns_llama_sample.argtypes = [vp, i, i, vp, i, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.ns_sample_seed_host.restype = None
+    L.ns_sample_seed_host.argtypes = [C.c_uint32, vp]
+    L.ns_sample_row_host.argtypes = [vp, i, vp, i, vp, vp, vp, vp, vp, vp]
+    L.ns_sample_expf_host.restype = C.c_float
+    L.ns_sample_expf_host.argtypes = [C.c_float]
     L.ns_comm_handle_bytes.restype = sz
     L.ns_comm_create.restype = vp
     L.ns_comm_create.argtypes = [i, i, sz, vp]
@@ -467,8 +478,22 @@ class LlamaHParams(C.Structure):
                 ("n_ff", C.c_int), ("n_ctx", C.c_int), ("norm_eps", C.c_float), ("rope_theta", C.c_float), ("rope_scale", C.c_float)]
 
 
+class Sampling(C.Structure):
+    """ns_llama_sampling (include/ns_b200.h)"""
+    _fields_ = [("top_k", C.c_int), ("top_p", C.c_float), ("temperature", C.c_float), ("repeat_penalty", C.c_float),
+                ("repeat_last_n", C.c_int), ("seed", C.c_uint32)]
+
+
+def sampling(top_k=40, top_p=0.95, temperature=0.8, repeat_penalty=1.1, repeat_last_n=64, seed=0) -> Sampling:
+    """the reference's do_sample defaults (application/main_pybind.cpp, Model.generate)"""
+    return Sampling(top_k, top_p, temperature, repeat_penalty, repeat_last_n, seed & 0xFFFFFFFF)
+
+
 class Llama:
-    """Device-resident Llama-family eval step (ns_llama_*): model_eval + greedy sampling of the reference, on the GPU."""
+    """Device-resident Llama-family eval step (ns_llama_*): model_eval of the reference on the GPU, and its next-token pick --
+    greedy (model_post_greedy_search) by default, or after set_sampling() the repetition-penalty / top-k / top-p / temperature
+    sampler of Model.generate(do_sample=True) (model_post_sample_top_k_top_p_repeat), drawn on the device so generate() and
+    generate_batch() keep feeding picks back without a host round trip."""
 
     TOK_EMBD, OUT_NORM, OUTPUT, ATTN_NORM, WQ, WK, WV, WO, FFN_NORM, W1, W2, W3 = range(12)
 
@@ -512,6 +537,15 @@ class Llama:
         """Generate past n_ctx through the StreamingLLM ring with n_keep attention-sink slots (-1: off); n_past then counts every
         token evaluated so far (include/ns_b200.h, ns_llama_set_streaming)"""
         _check(lib().ns_llama_set_streaming(self.h, n_keep), "ns_llama_set_streaming")
+
+    def set_sampling(self, top_k=40, top_p=0.95, temperature=0.8, repeat_penalty=1.1, repeat_last_n=64, seed=0):
+        """Sample every pick from now on (the reference's defaults; seed seeds the context's std::mt19937 and every window
+        restarts); set_sampling(None) returns to greedy (include/ns_b200.h, ns_llama_set_sampling)"""
+        if top_k is None:
+            _check(lib().ns_llama_set_sampling(self.h, None), "ns_llama_set_sampling")
+            return
+        s = sampling(top_k, top_p, temperature, repeat_penalty, repeat_last_n, seed)
+        _check(lib().ns_llama_set_sampling(self.h, C.byref(s)), "ns_llama_set_sampling")
 
     def set_sequences(self, n_seq: int):
         """n_seq KV blocks for continuous batching; every sequence restarts empty (include/ns_b200.h, ns_llama_set_sequences)"""
@@ -602,3 +636,38 @@ def batch_plan(n_seq: int, n_ctx: int, seqs, n_tokens, n_past):
     if rc != 0:
         return rc, None
     return rc, dict(order=order[:s.size], rows=rows[:counts[0]], d=int(counts[1]), tiles=tiles[:counts[2]])
+
+
+def sample_seed_host(seed: int) -> np.ndarray:
+    """std::mt19937(seed) as the sampler keeps it: 624 state words and the index of the next one"""
+    st = np.zeros(625, np.uint32)
+    lib().ns_sample_seed_host(seed & 0xFFFFFFFF, _np_ptr(st))
+    return st
+
+
+def sample_row_host(logits, window, s: Sampling, state: np.ndarray):
+    """steps 2-7 of the sampler for one row on the host (ns_sample_row_host); advances `state` in place ->
+    (pick, kept, ids [top_k], probs [top_k])"""
+    lg = np.ascontiguousarray(logits, np.float32)
+    w = np.ascontiguousarray(window, np.int32)
+    k = min(s.top_k, lg.size)
+    ids = np.zeros(max(s.top_k, 1), np.int32)
+    probs = np.zeros(max(s.top_k, 1), np.float32)
+    pick, kept = C.c_int32(0), C.c_int(0)
+    assert state.dtype == np.uint32 and state.size == 625 and state.flags.c_contiguous
+    _check(lib().ns_sample_row_host(_np_ptr(lg), lg.size, _np_ptr(w) if w.size else None, w.size, C.byref(s), _np_ptr(state),
+                                    C.byref(pick), C.byref(kept), _np_ptr(ids), _np_ptr(probs)), "ns_sample_row_host")
+    return int(pick.value), int(kept.value), ids[:k], probs[:k]
+
+
+def sample_expf_host(x: float) -> float:
+    return float(lib().ns_sample_expf_host(x))
+
+
+def sample(logits_ptr: int, n: int, n_vocab: int, windows_ptr, n_window: int, s: Sampling, mt_ptr: int, picks_ptr: int, kept_ptr,
+           ids_ptr, probs_ptr, ws_ptr: int, queue=None) -> int:
+    """ns_llama_sample on device pointers (the sampler's one launch on its own); returns the status code"""
+    return lib().ns_llama_sample(C.c_void_p(logits_ptr), n, n_vocab, C.c_void_p(windows_ptr) if windows_ptr else None, n_window,
+                                 C.byref(s), C.c_void_p(mt_ptr), C.c_void_p(picks_ptr), C.c_void_p(kept_ptr) if kept_ptr else None,
+                                 C.c_void_p(ids_ptr) if ids_ptr else None, C.c_void_p(probs_ptr) if probs_ptr else None,
+                                 C.c_void_p(ws_ptr), queue)

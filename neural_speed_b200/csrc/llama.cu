@@ -10,6 +10,8 @@
 //              cur = rms_norm(inpFF) * ffn_norm ; cur = ffn_silu(cur) + inpFF  :601-698
 //   logits = output * (rms_norm(inpL) * out_norm)                              :707-719
 // Greedy sampling = argmax with the lowest index on ties (model_utils.cpp:2963-2985).
+// ns_llama_set_sampling swaps the argmax's launch for sample_kernel (sample.cu): model_post_sample_top_k_top_p_repeat
+// (model_utils.cpp:2987-3032) with its generator and the sequences' repetition windows in device memory.
 //
 // One token (n_tokens == 1) is ONE CUDA graph: the token id and n_past live in device memory (`state`), so the same graph
 // replays for every position; ns_llama_generate chains graph launches with the argmax feeding the next embedding
@@ -24,6 +26,7 @@
 #include <vector>
 
 #include "nsb.cuh"
+#include "sample.h"
 
 namespace {
 
@@ -1426,8 +1429,9 @@ extern "C" int ns_llama_attention_ragged(float* q, const float* k, const float* 
 
 constexpr int kMaxSeq = 32;  // KV blocks of one context (ns_llama_set_sequences)
 constexpr int kPlanTiles = kMaxBatchRows / kAttnMmaRows + kMaxSeq;  // tile entries of one mixed pass, at most
-// device tables of a mixed pass: rows [kMaxBatchRows][2] | tiles [kPlanTiles][kTileInts] | last row of each segment [kMaxSeq]
-constexpr int kPlanInts = 2 * kMaxBatchRows + kPlanTiles * kTileInts + kMaxSeq;
+// device tables of a mixed pass: rows [kMaxBatchRows][2] | tiles [kPlanTiles][kTileInts] | last row of each segment [kMaxSeq] |
+// KV block of each segment [kMaxSeq] | internal segment of each caller index [kMaxSeq] (the sampler's window slots and draw order)
+constexpr int kPlanInts = 2 * kMaxBatchRows + kPlanTiles * kTileInts + 3 * kMaxSeq;
 
 struct ns_llama {
   ns_llama_hparams hp;
@@ -1470,6 +1474,18 @@ struct ns_llama {
   int* h_bstate = nullptr;  // [kMaxSeq * 5]
   int* h_plan = nullptr;      // [kMaxBatchRows] tokens | kPlanInts tables, as `plan` (allocated with it)
   float* h_logits = nullptr;  // [n_seq][n_vocab]
+  // ns_llama_set_sampling: the sampler takes the argmax's launch while `sampling`; its device state is allocated on first use
+  bool sampling = false;
+  ns_llama_sampling smp{};
+  uint32_t* mt = nullptr;             // std::mt19937 [kMtWords]
+  int* win = nullptr;                 // windows [kMaxSeq][kSampleMaxWindow], slot = KV block
+  unsigned long long* s_keys = nullptr;  // [kMaxSeq][kSampleSlices][kSampleMaxK]
+  int* s_pcnt = nullptr;              // [kMaxSeq][kSampleSlices]
+  double* s_cp = nullptr;             // [kMaxSeq][kSampleMaxK]
+  unsigned* s_tickets = nullptr;      // [kMaxSeq + 1]
+  int* s_kept = nullptr;              // [kMaxSeq]
+  int* s_ids = nullptr;               // [kMaxSeq][kSampleMaxK]
+  float* s_probs = nullptr;           // [kMaxSeq][kSampleMaxK]
 };
 
 static void* dev_alloc(ns_llama* c, size_t bytes) {
@@ -1719,14 +1735,18 @@ static int check_complete(const ns_llama* c) {
 // mix: m rows of mix->n segments of distinct sequences (ns_llama_eval_batch), ids in c->tokens; rows 0 .. d - 1 are one-token
 // segments (token, position and block in bstate as a batched step), rows d .. m - 1 the longer ones (mix->rows / mix->tiles);
 // logits and argmax (no advance) of each segment's last row, in internal order.
+// sample (while sampling is on): 2 = store the windows and draw, 1 = store the windows and take each row's first candidate
+// (a prompt piece whose pick is not returned), 0 = neither (the eager pass before a capture, evaluated again by the graph).
 struct MixedPass {
   int n, d, n_tiles;
   const int* rows;   // device [m][2]: {position, KV block}
   const int* tiles;  // device [n_tiles][kTileInts], rows counted from row d
   const int* last;   // device [n]: last row of each segment
+  const int* slot;   // device [n]: KV block of each segment
+  const int* draw;   // device [n]: internal segment of caller index i
 };
 static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int* record, bool ring, int seq = 0, bool batch = false,
-                           const MixedPass* mix = nullptr) {
+                           const MixedPass* mix = nullptr, int sample = 2) {
   const ns_llama_hparams& hp = c->hp;
   cudaStream_t st = c->st;
   const int E = hp.n_embd, hd = E / hp.n_head, kvd = hd * hp.n_head_kv;
@@ -1813,6 +1833,51 @@ static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int
     if (int rc = ns_mul_mat(c->output, c->xn, E, c->logits, hp.n_vocab, rows, nullptr, nullptr, 0, c->ws, (void*)st)) return rc;
   }
   const bool rowwise = batch || mix;  // a pick per row, in bstate
+  if (c->sampling) {
+    SampleLaunch a{};
+    a.logits = c->logits;
+    a.n_vocab = hp.n_vocab;
+    a.rows = rows;
+    a.k = c->smp.top_k;
+    a.top_p = c->smp.top_p;
+    a.temp = c->smp.temperature;
+    a.penalty = c->smp.repeat_penalty;
+    a.W = c->smp.repeat_last_n < hp.n_ctx ? c->smp.repeat_last_n : hp.n_ctx;
+    a.win = c->win;
+    a.win_stride = kSampleMaxWindow;
+    if (mix) {
+      a.toks = c->tokens;
+      a.last = mix->last;
+      a.slot = mix->slot;
+      a.order = mix->draw;
+    } else if (batch) {
+      a.toks = c->bstate;
+      a.tok_stride = 4;
+      a.tok_len = 1;
+      a.slot = c->bstate + 4 * kMaxSeq;
+    } else {
+      a.toks = toks;
+      a.tok_len = m;
+      a.slot_const = seq;
+    }
+    a.store = sample >= 1;
+    a.draw = sample >= 2;
+    a.mt = c->mt;
+    a.pkeys = c->s_keys;
+    a.pcnt = c->s_pcnt;
+    a.cp = c->s_cp;
+    a.tickets = c->s_tickets;
+    a.kept = c->s_kept;
+    a.ids = c->s_ids;
+    a.probs = c->s_probs;
+    a.state = rowwise ? c->bstate : c->state;
+    a.rowwise = rowwise;
+    a.n_tokens = rowwise ? 1 : m;
+    a.advance = advance;
+    a.record = record;
+    a.rec_stride = hp.n_ctx;
+    return ns_launch_sample(a, st);
+  }
   NS_CUDA_TRY(ns_launch_pdl(rowwise ? argmax_kernel<true> : argmax_kernel<false>, dim3((unsigned)kArgmaxBlocks, (unsigned)rows), dim3(256), 0, st, (const float*)c->logits,
                             hp.n_vocab, rowwise ? c->bstate : c->state, rowwise ? 1 : m, advance, record, hp.n_ctx, c->am_val, c->am_idx,
                             c->am_ticket));
@@ -1824,7 +1889,7 @@ static int ensure_batch_graph(ns_llama* c, int n) {
   if (c->batch_exec[n]) return NS_OK;
   // as ensure_decode_graph: one eager pass that does not advance the rows (it writes the K/V rows the captured pass rewrites
   // with the same values), then the capture
-  if (int rc = enqueue_forward(c, n, true, 0, nullptr, false, 0, true)) return rc;
+  if (int rc = enqueue_forward(c, n, true, 0, nullptr, false, 0, true, nullptr, 0)) return rc;
   NS_CUDA_TRY(cudaStreamSynchronize(c->st));
   NS_CUDA_TRY(cudaStreamBeginCapture(c->st, cudaStreamCaptureModeThreadLocal));
   int rc = enqueue_forward(c, n, true, 1, c->brecord, false, 0, true);
@@ -1848,7 +1913,7 @@ static int ensure_decode_graph(ns_llama* c) {
   // one eager pass (no state advance; it writes the same K/V the real pass will) sets kernel attributes and sizes every
   // lazily-grown buffer outside the capture, then capture.  The eager pass runs the plain attention even when streaming: a
   // ring step rotates the cache, which must happen once; the plain kernel writes nothing once the cache is full.
-  if (int rc = enqueue_forward(c, 1, true, 0, nullptr, false)) return rc;
+  if (int rc = enqueue_forward(c, 1, true, 0, nullptr, false, 0, false, nullptr, 0)) return rc;
   NS_CUDA_TRY(cudaStreamSynchronize(c->st));
   NS_CUDA_TRY(cudaStreamBeginCapture(c->st, cudaStreamCaptureModeThreadLocal));
   int rc = enqueue_forward(c, 1, true, 1, c->record, c->streaming);
@@ -1901,6 +1966,43 @@ extern "C" int ns_llama_set_streaming(ns_llama* c, int n_keep) {
   return NS_OK;
 }
 
+// Sampling in place of greedy (model_post_sample_top_k_top_p_repeat): the generator is reseeded and every window restarts;
+// NULL returns to greedy.  Either way the captured graphs, which bake in the pick kernel and its parameters, are dropped.
+extern "C" int ns_llama_set_sampling(ns_llama* c, const ns_llama_sampling* s) {
+  if (!c) return NS_E_INVALID;
+  if (s)
+    if (int rc = ns_sample_check("ns_llama_set_sampling", s)) return rc;
+  if (s && !c->mt) {
+    c->mt = (uint32_t*)dev_alloc(c, kMtWords * sizeof(uint32_t));
+    c->win = (int*)dev_alloc(c, (size_t)kMaxSeq * kSampleMaxWindow * sizeof(int));
+    c->s_keys = (unsigned long long*)dev_alloc(c, (size_t)kMaxSeq * kSampleSlices * kSampleMaxK * sizeof(unsigned long long));
+    c->s_pcnt = (int*)dev_alloc(c, (size_t)kMaxSeq * kSampleSlices * sizeof(int));
+    c->s_cp = (double*)dev_alloc(c, (size_t)kMaxSeq * kSampleMaxK * sizeof(double));
+    c->s_tickets = (unsigned*)dev_alloc(c, (kMaxSeq + 1) * sizeof(unsigned));
+    c->s_kept = (int*)dev_alloc(c, kMaxSeq * sizeof(int));
+    c->s_ids = (int*)dev_alloc(c, (size_t)kMaxSeq * kSampleMaxK * sizeof(int));
+    c->s_probs = (float*)dev_alloc(c, (size_t)kMaxSeq * kSampleMaxK * sizeof(float));
+    if (!c->mt || !c->win || !c->s_keys || !c->s_pcnt || !c->s_cp || !c->s_tickets || !c->s_kept || !c->s_ids || !c->s_probs) {
+      void* got[9] = {c->mt, c->win, c->s_keys, c->s_pcnt, c->s_cp, c->s_tickets, c->s_kept, c->s_ids, c->s_probs};
+      for (void* p : got) dev_free(c, p);
+      c->mt = nullptr;
+      return NS_E_CUDA;
+    }
+    NS_CUDA_TRY(cudaMemsetAsync(c->s_tickets, 0, (kMaxSeq + 1) * sizeof(unsigned), c->st));
+  }
+  NS_CUDA_TRY(cudaStreamSynchronize(c->st));  // nothing in flight replays the graphs dropped below or reads the generator
+  drop_graphs(c);
+  c->sampling = s != nullptr;
+  if (!s) return NS_OK;
+  c->smp = *s;
+  uint32_t mt[kMtWords];
+  ns_mt_seed(s->seed, mt);
+  NS_CUDA_TRY(cudaMemcpy(c->mt, mt, sizeof(mt), cudaMemcpyHostToDevice));
+  NS_CUDA_TRY(cudaMemsetAsync(c->win, 0, (size_t)kMaxSeq * kSampleMaxWindow * sizeof(int), c->st));
+  NS_CUDA_TRY(cudaStreamSynchronize(c->st));
+  return NS_OK;
+}
+
 // Positions of a streaming context: n_past is n_total.  Steps that reach past n_ctx take one token and continue the sequence;
 // once such a step has run, only a continuation or a restart inside the sinks (n_past <= n_keep) is meaningful.
 static int check_streaming(ns_llama* c, const char* who, int n_past, int n) {
@@ -1927,9 +2029,17 @@ static void advance_position(ns_llama* c, int n_past, int n) {
   c->wrapped = c->streaming && ((c->wrapped && n_past > c->ring.n_keep) || n_past + n > c->hp.n_ctx);
 }
 
+// a sequence evaluated at n_past 0 restarts its sampling window as zeros (the reference's fresh history); nothing while greedy
+static int reset_window(ns_llama* c, int slot) {
+  if (!c->sampling) return NS_OK;
+  NS_CUDA_TRY(cudaMemsetAsync(c->win + (size_t)slot * kSampleMaxWindow, 0, kSampleMaxWindow * sizeof(int), c->st));
+  return NS_OK;
+}
+
 // ns_llama_eval on KV block `seq`: block 0 one-token steps replay the decode graph, every other step (prompts, and single
 // tokens of the other blocks, whose graph would bake in the block) runs the same kernels eagerly
-static int eval_block(ns_llama* c, int seq, const int32_t* tokens, int n_tokens, int n_past, float* logits_host, int32_t* next_token) {
+static int eval_block(ns_llama* c, int seq, const int32_t* tokens, int n_tokens, int n_past, float* logits_host, int32_t* next_token,
+                      bool draw = true) {
   if (c->streaming && n_tokens > 1 && n_past + n_tokens > c->hp.n_ctx) {
     // the reference masks a multi-token step in slot order, which means nothing in ring order (llama.cpp:467, a TODO there)
     ns_set_error("ns_llama_eval: %d tokens past n_ctx %d: the ring takes one token per step", n_tokens, c->hp.n_ctx);
@@ -1942,24 +2052,27 @@ static int eval_block(ns_llama* c, int seq, const int32_t* tokens, int n_tokens,
     for (int t0 = 0; t0 < n_tokens; t0 += 32) {
       const int nt = n_tokens - t0 < 32 ? n_tokens - t0 : 32;
       const bool last = t0 + nt == n_tokens;
-      if (int rc = eval_block(c, seq, tokens + t0, nt, n_past + t0, last ? logits_host : nullptr, last ? next_token : nullptr)) return rc;
+      if (int rc = eval_block(c, seq, tokens + t0, nt, n_past + t0, last ? logits_host : nullptr, last ? next_token : nullptr, last && draw))
+        return rc;
     }
     return NS_OK;
   }
   if (int rc = check_complete(c)) return rc;
   if (int rc = ensure_buffers(c, n_tokens)) return rc;
   cudaStream_t st = c->st;
+  if (n_past == 0)
+    if (int rc = reset_window(c, seq)) return rc;
   c->h_state[0] = tokens[0];
   c->h_state[1] = n_past;
   c->h_state[2] = 0;
   c->h_state[3] = 0;
   NS_CUDA_TRY(cudaMemcpyAsync(c->state, c->h_state, 4 * sizeof(int), cudaMemcpyHostToDevice, st));
-  if (n_tokens == 1 && seq == 0) {
+  if (n_tokens == 1 && seq == 0 && draw) {
     if (int rc = ensure_decode_graph(c)) return rc;
     NS_CUDA_TRY(cudaGraphLaunch(c->decode_exec, st));
   } else {
     NS_CUDA_TRY(cudaMemcpyAsync(c->tokens, tokens, (size_t)n_tokens * sizeof(int), cudaMemcpyHostToDevice, st));
-    if (int rc = enqueue_forward(c, n_tokens, false, 1, nullptr, false, seq)) return rc;
+    if (int rc = enqueue_forward(c, n_tokens, false, 1, nullptr, false, seq, false, nullptr, draw ? 2 : 1)) return rc;
   }
   if (logits_host) NS_CUDA_TRY(cudaMemcpyAsync(c->h_logits, c->logits, (size_t)c->hp.n_vocab * 4, cudaMemcpyDeviceToHost, st));
   NS_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->state, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2012,7 +2125,9 @@ extern "C" int ns_llama_set_sequences(ns_llama* c, int n_seq) {
   drop_graphs(c);
   c->n_total = 0;
   c->wrapped = false;
-  return alloc_sequences(c, n_seq);
+  if (int rc = alloc_sequences(c, n_seq)) return rc;
+  if (c->win) NS_CUDA_TRY(cudaMemsetAsync(c->win, 0, (size_t)kMaxSeq * kSampleMaxWindow * sizeof(int), c->st));
+  return NS_OK;
 }
 
 // argument checks and the rows' device state of a batched call (no launch when the call is refused)
@@ -2037,6 +2152,9 @@ static int start_batch(ns_llama* c, const char* who, int n, const int* seq, cons
   }
   if (int rc = check_complete(c)) return rc;
   if (int rc = ensure_buffers(c, n)) return rc;
+  for (int i = 0; i < n; ++i)
+    if (n_past[i] == 0)
+      if (int rc = reset_window(c, seq[i])) return rc;
   for (int i = 0; i < kMaxSeq; ++i) {
     int* r = c->h_bstate + 4 * i;
     r[0] = i < n ? tokens[i] : 0;
@@ -2131,11 +2249,17 @@ extern "C" int ns_llama_eval_batch(ns_llama* c, int n, const int* seq, const int
   int* h_tab = c->h_plan + kMaxBatchRows;
   std::vector<int> off(n, 0);  // first id of segment i in `tokens` (caller's order)
   for (int i = 1; i < n; ++i) off[i] = off[i - 1] + n_tokens[i - 1];
+  int* h_last = h_tab + 2 * kMaxBatchRows + kPlanTiles * kTileInts;
   for (int j = 0; j < n; ++j) {
     const int i = p.order[j];
     memcpy(h_tok + p.first[j], tokens + off[i], (size_t)n_tokens[i] * sizeof(int));
-    h_tab[2 * kMaxBatchRows + kPlanTiles * kTileInts + j] = p.first[j] + n_tokens[i] - 1;
+    h_last[j] = p.first[j] + n_tokens[i] - 1;
+    h_last[kMaxSeq + j] = seq[i];
+    h_last[2 * kMaxSeq + i] = j;
   }
+  for (int i = 0; i < n; ++i)
+    if (n_past[i] == 0)
+      if (int rc = reset_window(c, seq[i])) return rc;
   std::copy(p.rows.begin(), p.rows.end(), h_tab);
   std::copy(p.tiles.begin(), p.tiles.end(), h_tab + 2 * kMaxBatchRows);
   for (int j = 0; j < kMaxSeq; ++j) {
@@ -2149,8 +2273,9 @@ extern "C" int ns_llama_eval_batch(ns_llama* c, int n, const int* seq, const int
   NS_CUDA_TRY(cudaMemcpyAsync(c->tokens, h_tok, (size_t)p.T * sizeof(int), cudaMemcpyHostToDevice, st));
   NS_CUDA_TRY(cudaMemcpyAsync(c->plan, h_tab, (size_t)kPlanInts * sizeof(int), cudaMemcpyHostToDevice, st));
   NS_CUDA_TRY(cudaMemcpyAsync(c->bstate, c->h_bstate, (size_t)kMaxSeq * 5 * sizeof(int), cudaMemcpyHostToDevice, st));
-  const MixedPass mix{n, p.d, (int)p.tiles.size() / kTileInts, c->plan, c->plan + 2 * kMaxBatchRows,
-                      c->plan + 2 * kMaxBatchRows + kPlanTiles * kTileInts};
+  const int* d_last = c->plan + 2 * kMaxBatchRows + kPlanTiles * kTileInts;
+  const MixedPass mix{n, p.d, (int)p.tiles.size() / kTileInts, c->plan, c->plan + 2 * kMaxBatchRows, d_last, d_last + kMaxSeq,
+                      d_last + 2 * kMaxSeq};
   if (int rc = enqueue_forward(c, p.T, false, 0, nullptr, false, 0, false, &mix)) return rc;
   const size_t nv = (size_t)c->hp.n_vocab;
   if (logits_host) NS_CUDA_TRY(cudaMemcpyAsync(c->h_logits, c->logits, n * nv * 4, cudaMemcpyDeviceToHost, st));
@@ -2177,6 +2302,8 @@ extern "C" int ns_llama_generate(ns_llama* c, int32_t first_token, int n_past, i
   if (int rc = ensure_buffers(c, 1)) return rc;
   if (int rc = ensure_decode_graph(c)) return rc;
   cudaStream_t st = c->st;
+  if (n_past == 0)
+    if (int rc = reset_window(c, 0)) return rc;
   c->h_state[0] = first_token;
   c->h_state[1] = n_past;
   c->h_state[2] = 0;

@@ -1,0 +1,386 @@
+// sample.cu -- the reference's sampler (model_post_sample_top_k_top_p_repeat, model_utils.cpp:2987-3032) on the device, in one
+// launch that takes the argmax's place in the eval step; its host restatement; and the parity entry ns_llama_sample.
+//
+// Grid (kSampleSlices, rows), 512 threads.  Each CTA loads one slice of its row's logits into shared memory, applies the
+// repetition penalty to the slice's ids found in the row's window (stored window + this pass's tokens, each id once), and
+// radix-selects the slice's top k keys (logit descending, id ascending: ns_sample_key) into global scratch.  The last CTA of a
+// row (ticket) radix-selects the row's top k over those partials in global memory, bitonic-sorts them in shared memory and runs
+// steps 5-7 in one thread (sample.h: every sum in the reference's order), then stores the row's window.  The last row to finish
+// (a second ticket) walks the rows in caller order, draws from the device-resident std::mt19937, and writes picks and state.
+#include "nsb.cuh"
+#include "sample.h"
+
+#include <algorithm>
+#include <vector>
+
+namespace {
+
+constexpr int kSampleThreads = 512;
+
+// row r's window entry j (0 <= j < W): the last W of (stored window ++ this pass's tl tokens)
+__device__ __forceinline__ int window_at(const int* wv, const int* tp, int tl, int W, int j) {
+  return j + tl < W ? wv[j + tl] : tp[j + tl - W];
+}
+
+// the kth largest (1-based) of a set of distinct 64-bit keys: eight passes of an 8-bit digit histogram over the keys that share
+// the digits chosen so far.  each(fn) calls fn(key) for this thread's share of the keys.  All threads of the CTA call it.
+template <class Each>
+__device__ uint64_t radix_kth(Each each, int kth, unsigned* hist, uint64_t* s_prefix, int* s_rem) {
+  uint64_t prefix = 0, mask = 0;
+  int rem = kth;
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    if (threadIdx.x == 0) {
+      *s_prefix = prefix;
+      *s_rem = rem;
+    }
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    each([&](uint64_t key) {
+      if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255], 1u);
+    });
+    __syncthreads();
+    if (threadIdx.x < 32) {  // lane L: digits 255 - 8 L .. 248 - 8 L, counted from the top
+      const int lane = threadIdx.x;
+      unsigned c = 0;
+      for (int j = 0; j < 8; ++j) c += hist[255 - 8 * lane - j];
+      unsigned incl = c;
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+      }
+      const unsigned excl = incl - c;
+      if (excl < (unsigned)rem && (unsigned)rem <= incl) {
+        unsigned acc = excl;
+        for (int j = 0; j < 8; ++j) {
+          const int b = 255 - 8 * lane - j;
+          if (acc + hist[b] >= (unsigned)rem) {
+            *s_prefix = prefix | ((uint64_t)b << shift);
+            *s_rem = rem - (int)acc;
+            break;
+          }
+          acc += hist[b];
+        }
+      }
+    }
+    __syncthreads();
+    prefix = *s_prefix;
+    rem = *s_rem;
+    mask |= (uint64_t)255 << shift;
+    __syncthreads();
+  }
+  return prefix;
+}
+
+__global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SampleLaunch a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ __align__(16) unsigned char smem[];
+  __shared__ unsigned hist[256];
+  __shared__ uint64_t s_prefix;
+  __shared__ int s_rem, s_cnt, s_total, s_off[kSampleSlices + 1];
+  __shared__ bool last;
+  const int row = blockIdx.y, sl = blockIdx.x, tid = threadIdx.x;
+  const int n = a.n_vocab, per = (n + kSampleSlices - 1) / kSampleSlices;
+  const int lo = min(n, sl * per), hi = min(n, lo + per), len = hi - lo;
+  const float* lg = a.logits + (size_t)row * n;
+  const int* tp;
+  int tl;
+  if (a.last) {
+    const int t0 = row ? a.last[row - 1] + 1 : 0;
+    tp = a.toks + t0;
+    tl = a.last[row] - t0 + 1;
+  } else {
+    tp = a.toks ? a.toks + (size_t)row * a.tok_stride : nullptr;
+    tl = a.toks ? a.tok_len : 0;
+  }
+  int* wv = a.win ? a.win + (size_t)(a.slot ? a.slot[row] : a.slot_const >= 0 ? a.slot_const : row) * a.win_stride : nullptr;
+  const int W = a.W, K = min(a.k, n);
+  const bool pen = W > 0 && a.penalty != 1.f;
+
+  // ---- slice: load, penalise each window id of the slice once, select the slice's top min(K, len) ----
+  float* vals = reinterpret_cast<float*>(smem);
+  unsigned char* flag = smem + (size_t)per * sizeof(float);
+  for (int i = tid; i < len; i += blockDim.x) {
+    vals[i] = lg[lo + i];
+    flag[i] = 0;
+  }
+  if (tid == 0) s_cnt = 0;
+  __syncthreads();
+  if (pen) {
+    for (int j = tid; j < W; j += blockDim.x) {
+      const int id = window_at(wv, tp, tl, W, j);
+      if (id >= lo && id < hi) flag[id - lo] = 1;
+    }
+    __syncthreads();
+    for (int i = tid; i < len; i += blockDim.x)
+      if (flag[i]) vals[i] = ns_sample_penalize(vals[i], a.penalty);
+    __syncthreads();
+  }
+  const int kk = min(K, len);
+  uint64_t thr = 0;
+  if (kk < len)
+    thr = radix_kth([&](auto fn) { for (int i = tid; i < len; i += blockDim.x) fn(ns_sample_key(vals[i], lo + i)); }, kk, hist, &s_prefix,
+                    &s_rem);
+  unsigned long long* pk = a.pkeys + ((size_t)row * kSampleSlices + sl) * a.k;
+  for (int i = tid; i < len; i += blockDim.x) {
+    const uint64_t key = ns_sample_key(vals[i], lo + i);
+    if (key >= thr) {
+      const int pos = atomicAdd(&s_cnt, 1);
+      if (pos < kk) pk[pos] = key;
+    }
+  }
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) {
+    a.pcnt[row * kSampleSlices + sl] = min(s_cnt, kk);
+    __threadfence();
+    last = atomicAdd(&a.tickets[row], 1u) == kSampleSlices - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+
+  // ---- the row's last CTA: top K of the partials, sorted ----
+  if (tid == 0) {
+    int t = 0;
+    for (int s = 0; s < kSampleSlices; ++s) {
+      s_off[s] = t;
+      t += ((volatile int*)a.pcnt)[row * kSampleSlices + s];
+    }
+    s_off[kSampleSlices] = t;
+    s_total = t;
+    s_cnt = 0;
+  }
+  __syncthreads();
+  const volatile unsigned long long* rk = a.pkeys + (size_t)row * kSampleSlices * a.k;
+  auto each_part = [&](auto fn) {
+    for (int s = 0; s < kSampleSlices; ++s) {
+      const int c = s_off[s + 1] - s_off[s];
+      for (int j = tid; j < c; j += blockDim.x) fn((uint64_t)rk[(size_t)s * a.k + j]);
+    }
+  };
+  thr = s_total > K ? radix_kth(each_part, K, hist, &s_prefix, &s_rem) : 0;
+  int P = 1;
+  while (P < K) P <<= 1;
+  uint64_t* sk = reinterpret_cast<uint64_t*>(smem);  // [P] (the slice's values are dead)
+  for (int i = tid; i < P; i += blockDim.x) sk[i] = 0;
+  __syncthreads();
+  each_part([&](uint64_t key) {
+    if (key >= thr) {
+      const int pos = atomicAdd(&s_cnt, 1);
+      if (pos < K) sk[pos] = key;
+    }
+  });
+  __syncthreads();
+  for (int size = 2; size <= P; size <<= 1)  // bitonic sort, descending
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int t = tid; t < P / 2; t += blockDim.x) {
+        const int i = (t / stride) * stride * 2 + t % stride, j = i + stride;
+        const bool desc = (i & size) == 0;
+        const uint64_t x = sk[i], y = sk[j];
+        if ((x < y) == desc) {
+          sk[i] = y;
+          sk[j] = x;
+        }
+      }
+      __syncthreads();
+    }
+  float* l = reinterpret_cast<float*>(sk + P);  // [K]
+  float* p = l + K;                             // [K]
+  int* rid = a.ids + (size_t)row * a.k;
+  for (int i = tid; i < K; i += blockDim.x) {
+    l[i] = ns_sample_key_value(sk[i]);
+    rid[i] = ns_sample_key_id(sk[i]);
+  }
+  __syncthreads();
+  // ---- steps 5-7 in one thread, in the reference's order ----
+  if (tid == 0) {
+    const int kept = ns_sample_tail(l, p, K, a.top_p, a.temp);
+    ns_sample_cumulative(p, kept, a.cp + (size_t)row * a.k);
+    a.kept[row] = kept;
+    s_cnt = kept;
+  }
+  __syncthreads();
+  float* rp = a.probs + (size_t)row * a.k;
+  for (int i = tid; i < K; i += blockDim.x) rp[i] = i < s_cnt ? p[i] : 0.f;
+  // ---- the row's window: the last W of (stored ++ this pass's tokens) ----
+  if (a.store && wv && tl > 0) {
+    const int v = tid < W ? window_at(wv, tp, tl, W, tid) : 0;
+    __syncthreads();
+    if (tid < W) wv[tid] = v;
+  }
+  __threadfence();  // ids, probs, the window: visible to the drawing CTA and the next launch
+  __syncthreads();
+  if (tid != 0) return;
+  a.tickets[row] = 0u;
+  __threadfence();
+  if (atomicAdd(&a.tickets[a.rows], 1u) != (unsigned)a.rows - 1) return;
+  __threadfence();
+  // ---- the last row: draws in caller order ----
+  for (int i = 0; i < a.rows; ++i) {
+    const int r = a.order ? a.order[i] : i;
+    const int kept = ((volatile int*)a.kept)[r];
+    int idx = 0;
+    if (a.draw && kept >= 2 && kept <= a.k) {
+      const double* cpr = a.cp + (size_t)r * a.k;
+      idx = ns_sample_pick(cpr, kept, a.mt);  // cp was written by other CTAs before their ticket: fenced above
+    }
+    const int pick = ((volatile int*)a.ids)[(size_t)r * a.k + idx];
+    if (a.picks) a.picks[r] = pick;
+    if (a.state) {
+      int* st = a.state + (a.rowwise ? 4 * r : 0);
+      st[3] = pick;
+      if (a.advance) {
+        st[0] = pick;
+        st[1] += a.n_tokens;
+        if (a.record) a.record[(size_t)r * a.rec_stride + st[2]++] = pick;
+      }
+    }
+  }
+  a.tickets[a.rows] = 0u;
+}
+
+size_t sample_smem(int n_vocab, int k) {
+  const size_t per = (size_t)(n_vocab + kSampleSlices - 1) / kSampleSlices;
+  const int K = k < n_vocab ? k : n_vocab;
+  size_t P = 1;
+  while (P < (size_t)K) P <<= 1;
+  return std::max(per * 5, P * 8 + (size_t)K * 8);
+}
+
+}  // namespace
+
+int ns_sample_check(const char* who, const ns_llama_sampling* s) {
+  if (!(s->top_k >= 1) || !(s->top_p > 0.f && s->top_p <= 1.f) || !(s->temperature > 0.f && isfinite(s->temperature)) ||
+      !(s->repeat_penalty > 0.f && isfinite(s->repeat_penalty)) || s->repeat_last_n < 0 || s->repeat_last_n > kSampleMaxWindow) {
+    ns_set_error("%s: top_k %d top_p %g temperature %g repeat_penalty %g repeat_last_n %d: need top_k >= 1, 0 < top_p <= 1, finite "
+                 "temperature and repeat_penalty > 0, 0 <= repeat_last_n <= %d",
+                 who, s->top_k, s->top_p, s->temperature, s->repeat_penalty, s->repeat_last_n, kSampleMaxWindow);
+    return NS_E_INVALID;
+  }
+  if (s->top_k > kSampleMaxK) {
+    ns_set_error("%s: top_k %d above %d (the device selection sorts at most %d candidates per row)", who, s->top_k, kSampleMaxK,
+                 kSampleMaxK);
+    return NS_E_UNSUPPORTED;
+  }
+  return NS_OK;
+}
+
+int ns_launch_sample(const SampleLaunch& a, cudaStream_t st) {
+  const size_t smem = sample_smem(a.n_vocab, a.k);
+  if (smem > 48 * 1024) {
+    if (smem > 220 * 1024) {
+      ns_set_error("sampler: n_vocab %d too large (a slice of %d logits must fit in shared memory)", a.n_vocab, a.n_vocab / kSampleSlices);
+      return NS_E_UNSUPPORTED;
+    }
+    NS_CUDA_TRY(cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  }
+  NS_CUDA_TRY(ns_launch_pdl(sample_kernel, dim3((unsigned)kSampleSlices, (unsigned)a.rows), dim3(kSampleThreads), smem, st, a));
+  ns_count_launch();
+  return NS_OK;
+}
+
+// ---- host restatement ------------------------------------------------------------------------------------------------------
+
+extern "C" void ns_sample_seed_host(uint32_t seed, uint32_t* state) {
+  if (state) ns_mt_seed(seed, state);
+}
+
+extern "C" float ns_sample_expf_host(float x) { return ns_sample_expf(x); }
+
+extern "C" int ns_sample_row_host(const float* logits, int n_vocab, const int32_t* window, int n_window, const ns_llama_sampling* s,
+                                  uint32_t* state, int32_t* pick, int* kept, int32_t* ids, float* probs) {
+  if (!logits || !s || !state || !pick || n_vocab < 1 || n_window < 0 || n_window > kSampleMaxWindow || (n_window && !window)) {
+    ns_set_error("ns_sample_row_host: invalid arguments (n_vocab %d n_window %d)", n_vocab, n_window);
+    return NS_E_INVALID;
+  }
+  if (int rc = ns_sample_check("ns_sample_row_host", s)) return rc;
+  // step 2: each candidate whose id is in the window changed once (model_utils.cpp:798-828)
+  std::vector<float> v(logits, logits + n_vocab);
+  if (s->repeat_penalty != 1.f) {
+    std::vector<char> hit(n_vocab, 0);
+    for (int j = 0; j < n_window; ++j)
+      if (window[j] >= 0 && window[j] < n_vocab) hit[window[j]] = 1;
+    for (int i = 0; i < n_vocab; ++i)
+      if (hit[i]) v[i] = ns_sample_penalize(v[i], s->repeat_penalty);
+  }
+  // step 3: the top K in selection order (:549-570)
+  const int K = std::min(s->top_k, n_vocab);
+  std::vector<uint64_t> key(n_vocab);
+  for (int i = 0; i < n_vocab; ++i) key[i] = ns_sample_key(v[i], i);
+  std::partial_sort(key.begin(), key.begin() + K, key.end(), [](uint64_t x, uint64_t y) { return x > y; });
+  std::vector<float> l(K), p(K);
+  std::vector<double> cp(K);
+  for (int i = 0; i < K; ++i) l[i] = ns_sample_key_value(key[i]);
+  // steps 5-7
+  const int n = ns_sample_tail(l.data(), p.data(), K, s->top_p, s->temperature);
+  ns_sample_cumulative(p.data(), n, cp.data());
+  const int idx = ns_sample_pick(cp.data(), n, state);
+  *pick = ns_sample_key_id(key[idx]);
+  if (kept) *kept = n;
+  for (int i = 0; i < K; ++i) {
+    if (ids) ids[i] = ns_sample_key_id(key[i]);
+    if (probs) probs[i] = i < n ? p[i] : 0.f;
+  }
+  return NS_OK;
+}
+
+// ---- parity entry --------------------------------------------------------------------------------------------------------
+// workspace: tickets [kSampleMaxRows + 1] (at the same place for every n and k, so one zeroed workspace serves calls of any
+// shape) | pcnt [n][slices] | kept [n], each padded to 16 bytes | cp [n][k] | ids [n][k] | probs [n][k] | pkeys [n][slices][k]
+constexpr int kSampleMaxRows = 32;
+static size_t pad16(size_t b) { return (b + 15) / 16 * 16; }
+extern "C" size_t ns_llama_sample_workspace_bytes(int n, int top_k) {
+  if (n < 1 || top_k < 1) return 0;
+  const size_t k = (size_t)std::min(top_k, kSampleMaxK);
+  return pad16((size_t)(kSampleMaxRows + 1) * 4) + pad16((size_t)n * kSampleSlices * 4) + pad16((size_t)n * 4) + pad16((size_t)n * k * 8) +
+         pad16((size_t)n * k * 4) * 2 + (size_t)n * kSampleSlices * k * 8;
+}
+
+extern "C" int ns_llama_sample(const float* logits, int n, int n_vocab, const int32_t* windows, int n_window, const ns_llama_sampling* s,
+                               uint32_t* mt_state, int32_t* picks, int* kept, int32_t* ids, float* probs, void* ws, void* queue) {
+  const char* who = "ns_llama_sample";
+  if (int rc = ns_ensure_device()) return rc;
+  if (!logits || !s || !mt_state || !picks || !ws || n < 1 || n > kSampleMaxRows || n_vocab < 1 || n_window < 0 || n_window > kSampleMaxWindow ||
+      (n_window && !windows)) {
+    ns_set_error("%s: invalid arguments (n %d n_vocab %d n_window %d, or a null pointer)", who, n, n_vocab, n_window);
+    return NS_E_INVALID;
+  }
+  if (int rc = ns_sample_check(who, s)) return rc;
+  const int k = s->top_k;
+  char* w = static_cast<char*>(ws);
+  SampleLaunch a{};
+  a.tickets = reinterpret_cast<unsigned*>(w);
+  w += pad16((size_t)(kSampleMaxRows + 1) * 4);
+  a.pcnt = reinterpret_cast<int*>(w);
+  w += pad16((size_t)n * kSampleSlices * 4);
+  a.kept = reinterpret_cast<int*>(w);
+  w += pad16((size_t)n * 4);
+  a.cp = reinterpret_cast<double*>(w);
+  w += pad16((size_t)n * k * 8);
+  a.ids = reinterpret_cast<int*>(w);
+  w += pad16((size_t)n * k * 4);
+  a.probs = reinterpret_cast<float*>(w);
+  w += pad16((size_t)n * k * 4);
+  a.pkeys = reinterpret_cast<unsigned long long*>(w);
+  if (kept) a.kept = kept;
+  if (ids) a.ids = ids;
+  if (probs) a.probs = probs;
+  a.logits = logits;
+  a.n_vocab = n_vocab;
+  a.rows = n;
+  a.k = k;
+  a.top_p = s->top_p;
+  a.temp = s->temperature;
+  a.penalty = s->repeat_penalty;
+  a.W = n_window;
+  a.win = const_cast<int*>(windows);
+  a.win_stride = n_window;
+  a.slot = nullptr;
+  a.slot_const = -1;  // row r reads windows + r * n_window
+  a.store = 0;
+  a.draw = 1;
+  a.mt = mt_state;
+  a.picks = picks;
+  return ns_launch_sample(a, ns_stream_of(queue));
+}
