@@ -387,6 +387,35 @@ NS_API int ns_llama_eval_batch(ns_llama* ctx, int n, const int* seq, const int* 
  * segment}; counts [3] = {T, d = number of one-token segments, number of tile entries}. */
 NS_API int ns_llama_batch_plan(int n_seq, int n_ctx, int n, const int* seq, const int* n_tokens, const int* n_past, int* order,
                                int* rows, int* tiles, int* counts);
+/* model_eval with logits_all (llama.cpp:743-747; Model.__call__(logits_all=True) -> model.evaluate) over the segments of
+ * ns_llama_eval_batch: every input token's row, scored on the device.  Rows are the T = sum n_tokens input tokens in the caller's
+ * order (segments back to back, as `tokens`).  Outputs, each nullable, at least one non-null:
+ *   logprobs [T]              log softmax(logits of row r)[targets[r]] (targets and logprobs both null or both non-null; every
+ *                             target in [0, n_vocab))
+ *   argmax [T]                the greedy pick of row r (lowest id on ties, as ns_llama_eval_batch's picks)
+ *   logits_host [T][n_vocab]  the raw logits of every row
+ * The body is ns_llama_eval_batch's pass on the same segments (run eagerly also when every segment has one token) and appends
+ * the same K/V.  Then the final RMSNorm of all T rows, and per chunk of <= 32 rows the lm_head at the chunk's row count through
+ * ns_route -- GEMV tiles where the route would take the bf16 GEMM, so integer formats keep their exact block sums on every row --
+ * and one log-prob launch (the arithmetic of ns_logprob_row_host).  Device memory for logits is one chunk; logits_host fills
+ * through pinned staging.  Argument rules and codes as ns_llama_eval_batch; also NS_E_INVALID for a target outside
+ * [0, n_vocab), targets / logprobs not paired, or no output; NS_E_UNSUPPORTED while sampling is on (a scoring pass draws nothing).
+ * A refused call launches nothing. */
+NS_API int ns_llama_eval_all(ns_llama* ctx, int n, const int* seq, const int* n_tokens, const int32_t* tokens, const int* n_past,
+                             const int32_t* targets, float* logprobs, int32_t* argmax, float* logits_host);
+/* The log-prob kernel on its own, for parity tests: one launch over device logits [n][n_vocab] (1 <= n <= 32); device targets /
+ * logprobs [n] (both or neither) and argmax [n] (nullable; one output at least).  ws: device workspace of
+ * ns_llama_logprob_workspace_bytes(n, n_vocab) bytes, zeroed once by the caller: its tickets lie in the first 128 bytes for every
+ * n and are zero again after every call.  A target outside [0, n_vocab) gives a NaN log-prob. */
+NS_API size_t ns_llama_logprob_workspace_bytes(int n, int n_vocab);
+NS_API int ns_llama_logprob(const float* logits, int n, int n_vocab, const int32_t* targets, float* logprobs, int32_t* argmax,
+                            void* ws, void* queue);
+/* Host restatement of one row (no device needed), bit for bit what the kernel computes (neural_speed_b200/csrc/logprob.h states
+ * the order of every sum): max M and argmax over 32 slices, S = sum of exp(x - M) with the library's exp (ns_sample_expf_host),
+ * logprob = (x[target] - M) - log(S) with the library's log (within 1 ulp of glibc's logf).  A NaN logit makes the row's log-probs
+ * NaN; a -inf target logit gives -inf when the row has a finite max; a row with nothing above -inf gives NaN.  logprob or argmax
+ * nullable (one at least); target read only with logprob. */
+NS_API int ns_logprob_row_host(const float* logits, int n_vocab, int32_t target, float* logprob, int32_t* argmax);
 /* ---- sampling (the reference's Model.generate(do_sample=True): model_post_sample_top_k_top_p_repeat, model_utils.cpp:2987-3032)
  * Per row, in this order: the repetition penalty on every candidate whose id occurs in the sequence's window (once per id:
  * logit <= 0 ? logit * penalty : logit / penalty), the top_k largest logits (ties: lower id first), top-p on their fp32 softmax

@@ -64,7 +64,7 @@ EXPORTS = [
     "ns_llama_attention_batch_workspace_bytes", "ns_llama_attention_batch",
     "ns_llama_eval_batch", "ns_llama_batch_plan", "ns_llama_attention_ragged_workspace_bytes", "ns_llama_attention_ragged",
     "ns_llama_set_sampling", "ns_llama_sample_workspace_bytes", "ns_llama_sample", "ns_sample_seed_host", "ns_sample_row_host",
-    "ns_sample_expf_host",
+    "ns_sample_expf_host", "ns_llama_eval_all", "ns_llama_logprob_workspace_bytes", "ns_llama_logprob", "ns_logprob_row_host",
     "ns_comm_handle_bytes", "ns_comm_create", "ns_comm_get_handle", "ns_comm_open_peers", "ns_comm_link_local", "ns_comm_all_reduce_f32",
     "ns_comm_status", "ns_comm_free",
 ]
@@ -212,6 +212,11 @@ def lib() -> C.CDLL:
     L.ns_sample_row_host.argtypes = [vp, i, vp, i, vp, vp, vp, vp, vp, vp]
     L.ns_sample_expf_host.restype = C.c_float
     L.ns_sample_expf_host.argtypes = [C.c_float]
+    L.ns_llama_eval_all.argtypes = [vp, i, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.ns_llama_logprob_workspace_bytes.restype = sz
+    L.ns_llama_logprob_workspace_bytes.argtypes = [i, i]
+    L.ns_llama_logprob.argtypes = [vp, i, i, vp, vp, vp, vp, vp]
+    L.ns_logprob_row_host.argtypes = [vp, i, C.c_int32, vp, vp]
     L.ns_comm_handle_bytes.restype = sz
     L.ns_comm_create.restype = vp
     L.ns_comm_create.argtypes = [i, i, sz, vp]
@@ -584,6 +589,30 @@ class Llama:
                                          _np_ptr(logits) if want_logits else None, _np_ptr(nxt)), "ns_llama_eval_batch")
         return logits, nxt
 
+    def eval_all(self, seqs, token_lists, n_past, targets=None, want_logits=False):
+        """model_eval with logits_all (the reference's Model.__call__(input_ids, logits_all=True) -> model.evaluate): one pass over
+        the segments as eval_batch, scoring every input token on the device (include/ns_b200.h, ns_llama_eval_all).  targets: one
+        list per segment, a target id for each token (e.g. the next token), or None.  -> (log-probs of the targets per segment
+        or None, greedy picks per segment, logits [len][n_vocab] per segment or None), in the caller's order"""
+        s, p = (np.ascontiguousarray(a, np.int32) for a in (seqs, n_past))
+        parts = [np.asarray(x, np.int32).ravel() for x in token_lists]
+        lens = np.array([x.size for x in parts], np.int32)
+        t = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0, np.int32))
+        T = t.size
+        tg = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int32).ravel() for x in targets]), np.int32) \
+            if targets is not None else None
+        if tg is not None and tg.size != T:
+            raise ValueError(f"targets: {tg.size} ids for {T} tokens")
+        lp = np.empty(T, np.float32) if targets is not None else None
+        am = np.empty(T, np.int32)
+        logits = np.empty((T, self.hp.n_vocab), np.float32) if want_logits else None
+        _check(lib().ns_llama_eval_all(self.h, s.size, _np_ptr(s), _np_ptr(lens), _np_ptr(t), _np_ptr(p),
+                                       _np_ptr(tg) if tg is not None else None, _np_ptr(lp) if lp is not None else None, _np_ptr(am),
+                                       _np_ptr(logits) if want_logits else None), "ns_llama_eval_all")
+        cuts = np.cumsum(lens)[:-1]
+        split = (lambda a: np.split(a, cuts)) if s.size else (lambda a: [])  # noqa: E731
+        return (split(lp) if lp is not None else None), split(am), (split(logits) if want_logits else None)
+
     def generate_batch(self, seqs, first_tokens, n_past, n_new: int) -> np.ndarray:
         """greedy generation of n_new tokens for each sequence, picks fed back on the device -> [n][n_new]"""
         s, t, p = (np.ascontiguousarray(a, np.int32) for a in (seqs, first_tokens, n_past))
@@ -662,6 +691,22 @@ def sample_row_host(logits, window, s: Sampling, state: np.ndarray):
 
 def sample_expf_host(x: float) -> float:
     return float(lib().ns_sample_expf_host(x))
+
+
+def logprob_row_host(logits, target=None):
+    """one row of the log-prob kernel's arithmetic on the host (ns_logprob_row_host) -> (log-prob of target or None, argmax)"""
+    lg = np.ascontiguousarray(logits, np.float32)
+    lp, am = C.c_float(0.0), C.c_int32(0)
+    _check(lib().ns_logprob_row_host(_np_ptr(lg), lg.size, 0 if target is None else int(target),
+                                     None if target is None else C.byref(lp), C.byref(am)), "ns_logprob_row_host")
+    return (None if target is None else float(lp.value)), int(am.value)
+
+
+def logprob(logits_ptr: int, n: int, n_vocab: int, targets_ptr, logprobs_ptr, argmax_ptr, ws_ptr: int, queue=None) -> int:
+    """ns_llama_logprob on device pointers (the log-prob kernel's one launch on its own); returns the status code"""
+    return lib().ns_llama_logprob(C.c_void_p(logits_ptr), n, n_vocab, C.c_void_p(targets_ptr) if targets_ptr else None,
+                                  C.c_void_p(logprobs_ptr) if logprobs_ptr else None, C.c_void_p(argmax_ptr) if argmax_ptr else None,
+                                  C.c_void_p(ws_ptr), queue)
 
 
 def sample(logits_ptr: int, n: int, n_vocab: int, windows_ptr, n_window: int, s: Sampling, mt_ptr: int, picks_ptr: int, kept_ptr,

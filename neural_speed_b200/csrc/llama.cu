@@ -27,6 +27,7 @@
 
 #include "nsb.cuh"
 #include "sample.h"
+#include "logprob.h"
 
 namespace {
 
@@ -1432,6 +1433,7 @@ constexpr int kPlanTiles = kMaxBatchRows / kAttnMmaRows + kMaxSeq;  // tile entr
 // device tables of a mixed pass: rows [kMaxBatchRows][2] | tiles [kPlanTiles][kTileInts] | last row of each segment [kMaxSeq] |
 // KV block of each segment [kMaxSeq] | internal segment of each caller index [kMaxSeq] (the sampler's window slots and draw order)
 constexpr int kPlanInts = 2 * kMaxBatchRows + kPlanTiles * kTileInts + 3 * kMaxSeq;
+constexpr int kAllChunk = kLogprobMaxRows;  // rows of one lm_head launch of ns_llama_eval_all
 
 struct ns_llama {
   ns_llama_hparams hp;
@@ -1486,6 +1488,13 @@ struct ns_llama {
   int* s_kept = nullptr;              // [kMaxSeq]
   int* s_ids = nullptr;               // [kMaxSeq][kSampleMaxK]
   float* s_probs = nullptr;           // [kMaxSeq][kSampleMaxK]
+  // ns_llama_eval_all (allocated on first use): the lm_head's logits of one chunk of rows, the log-prob kernel's tickets and
+  // partials, the rows' targets / log-probs / picks in internal order, and pinned staging for those and two chunks of logits
+  float* all_logits = nullptr;        // [kAllChunk][n_vocab]
+  unsigned* lp_tickets = nullptr;     // [kAllChunk] | max, id, sum [kAllChunk][kLogprobSlices]
+  int* all_io = nullptr;              // [3][kMaxBatchRows]
+  int* h_all = nullptr;               // [3][kMaxBatchRows] | [2][kAllChunk][n_vocab] floats
+  cudaEvent_t all_ev[2] = {};
 };
 
 static void* dev_alloc(ns_llama* c, size_t bytes) {
@@ -1612,6 +1621,9 @@ extern "C" void ns_llama_free(ns_llama* c) {
   if (c->h_bstate) cudaFreeHost(c->h_bstate);
   if (c->h_plan) cudaFreeHost(c->h_plan);
   if (c->h_logits) cudaFreeHost(c->h_logits);
+  if (c->h_all) cudaFreeHost(c->h_all);
+  for (cudaEvent_t e : c->all_ev)
+    if (e) cudaEventDestroy(e);
   delete c;
 }
 
@@ -1745,8 +1757,8 @@ struct MixedPass {
   const int* slot;   // device [n]: KV block of each segment
   const int* draw;   // device [n]: internal segment of caller index i
 };
-static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int* record, bool ring, int seq = 0, bool batch = false,
-                           const MixedPass* mix = nullptr, int sample = 2) {
+// the embedding and every layer: leaves the last layer's output rows in c->x
+static int enqueue_body(ns_llama* c, int m, bool from_state, bool ring, int seq, bool batch, const MixedPass* mix) {
   const ns_llama_hparams& hp = c->hp;
   cudaStream_t st = c->st;
   const int E = hp.n_embd, hd = E / hp.n_head, kvd = hd * hp.n_head_kv;
@@ -1814,6 +1826,16 @@ static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int
       if (int rc = ns_ffn_silu_residual(L.w1, L.w2, L.w3, c->attn, E, c->tmp, c->x, E, m, c->xn, c->ws, st, nullptr, 0.f, 1)) return rc;
     }
   }
+  return NS_OK;
+}
+
+static int enqueue_forward(ns_llama* c, int m, bool from_state, int advance, int* record, bool ring, int seq = 0, bool batch = false,
+                           const MixedPass* mix = nullptr, int sample = 2) {
+  if (int rc = enqueue_body(c, m, from_state, ring, seq, batch, mix)) return rc;
+  const ns_llama_hparams& hp = c->hp;
+  cudaStream_t st = c->st;
+  const int E = hp.n_embd;
+  const int* toks = batch ? c->bstate : from_state ? c->state : c->tokens;
   // logits of the last token only (model_eval keeps the last row unless logits_all); a batched step: of every row, each being
   // its sequence's last token (llama.cpp:745-758)
   const int rows = batch ? m : mix ? mix->n : 1;
@@ -2199,16 +2221,13 @@ extern "C" int ns_llama_generate_batch(ns_llama* c, int n, const int* seq, const
   return NS_OK;
 }
 
-// model_eval over n inputs (llama.cpp:53-90, 329-460, 745-758): one pass over the token segments of n distinct sequences
-extern "C" int ns_llama_eval_batch(ns_llama* c, int n, const int* seq, const int* n_tokens, const int32_t* tokens, const int* n_past,
-                                   float* logits_host, int32_t* next_tokens) {
-  const char* who = "ns_llama_eval_batch";
-  if (int rc = ns_ensure_device()) return rc;
+// the argument rules of a pass over segments (ns_llama_eval_batch, ns_llama_eval_all); nothing is launched
+static int check_pass(ns_llama* c, const char* who, int n, const int* seq, const int* n_tokens, const int32_t* tokens, const int* n_past,
+                      BatchPlan& p) {
   if (!c || !tokens) {
     ns_set_error("%s: null pointer", who);
     return NS_E_INVALID;
   }
-  BatchPlan p;
   if (int rc = plan_batch(who, c->n_seq, c->hp.n_ctx, n, seq, n_tokens, n_past, p)) return rc;
   const int hd = c->hp.n_embd / c->hp.n_head;
   if (hd != 64 && hd != 128) {
@@ -2223,9 +2242,13 @@ extern "C" int ns_llama_eval_batch(ns_llama* c, int n, const int* seq, const int
     ns_set_error("%s: %d rows in exact-prefill mode (the integer block sums hold up to 32 rows)", who, p.T);
     return NS_E_UNSUPPORTED;
   }
-  if (p.d == n) return ns_llama_decode_batch(c, n, seq, tokens, n_past, logits_host, next_tokens);  // its captured graph
-  if (int rc = check_complete(c)) return rc;
-  if (int rc = ensure_buffers(c, p.T)) return rc;
+  return NS_OK;
+}
+
+// The device tables of a pass over the segments of plan p: ids in internal order, rows, tiles, each segment's last row, block and
+// draw order, and the one-token rows' states as a batched step's.  *mix describes the pass.
+static int stage_segments(ns_llama* c, int n, const int* seq, const int* n_tokens, const int32_t* tokens, const int* n_past,
+                          const BatchPlan& p, MixedPass* mix) {
   cudaStream_t st = c->st;
   if (!c->plan) {
     c->plan = (int*)dev_alloc(c, (size_t)kPlanInts * sizeof(int));
@@ -2274,8 +2297,24 @@ extern "C" int ns_llama_eval_batch(ns_llama* c, int n, const int* seq, const int
   NS_CUDA_TRY(cudaMemcpyAsync(c->plan, h_tab, (size_t)kPlanInts * sizeof(int), cudaMemcpyHostToDevice, st));
   NS_CUDA_TRY(cudaMemcpyAsync(c->bstate, c->h_bstate, (size_t)kMaxSeq * 5 * sizeof(int), cudaMemcpyHostToDevice, st));
   const int* d_last = c->plan + 2 * kMaxBatchRows + kPlanTiles * kTileInts;
-  const MixedPass mix{n, p.d, (int)p.tiles.size() / kTileInts, c->plan, c->plan + 2 * kMaxBatchRows, d_last, d_last + kMaxSeq,
-                      d_last + 2 * kMaxSeq};
+  *mix = MixedPass{n, p.d, (int)p.tiles.size() / kTileInts, c->plan, c->plan + 2 * kMaxBatchRows, d_last, d_last + kMaxSeq,
+                   d_last + 2 * kMaxSeq};
+  return NS_OK;
+}
+
+// model_eval over n inputs (llama.cpp:53-90, 329-460, 745-758): one pass over the token segments of n distinct sequences
+extern "C" int ns_llama_eval_batch(ns_llama* c, int n, const int* seq, const int* n_tokens, const int32_t* tokens, const int* n_past,
+                                   float* logits_host, int32_t* next_tokens) {
+  const char* who = "ns_llama_eval_batch";
+  if (int rc = ns_ensure_device()) return rc;
+  BatchPlan p;
+  if (int rc = check_pass(c, who, n, seq, n_tokens, tokens, n_past, p)) return rc;
+  if (p.d == n) return ns_llama_decode_batch(c, n, seq, tokens, n_past, logits_host, next_tokens);  // its captured graph
+  if (int rc = check_complete(c)) return rc;
+  if (int rc = ensure_buffers(c, p.T)) return rc;
+  cudaStream_t st = c->st;
+  MixedPass mix;
+  if (int rc = stage_segments(c, n, seq, n_tokens, tokens, n_past, p, &mix)) return rc;
   if (int rc = enqueue_forward(c, p.T, false, 0, nullptr, false, 0, false, &mix)) return rc;
   const size_t nv = (size_t)c->hp.n_vocab;
   if (logits_host) NS_CUDA_TRY(cudaMemcpyAsync(c->h_logits, c->logits, n * nv * 4, cudaMemcpyDeviceToHost, st));
@@ -2285,6 +2324,130 @@ extern "C" int ns_llama_eval_batch(ns_llama* c, int n, const int* seq, const int
     const int i = p.order[j];
     if (logits_host) memcpy(logits_host + (size_t)i * nv, c->h_logits + (size_t)j * nv, nv * 4);
     if (next_tokens) next_tokens[i] = c->h_bstate[4 * j + 3];
+  }
+  return NS_OK;
+}
+
+static int ensure_all_rows(ns_llama* c) {
+  if (c->all_logits) return NS_OK;
+  const size_t V = (size_t)c->hp.n_vocab;
+  float* lg = (float*)dev_alloc(c, (size_t)kAllChunk * V * 4);
+  unsigned* tk = (unsigned*)dev_alloc(c, (size_t)kAllChunk * (1 + 3 * kLogprobSlices) * 4);
+  int* io = (int*)dev_alloc(c, (size_t)3 * kMaxBatchRows * 4);
+  int* h = nullptr;
+  cudaEvent_t ev[2] = {};
+  bool ok = lg && tk && io && cudaMallocHost((void**)&h, ((size_t)3 * kMaxBatchRows + 2 * kAllChunk * V) * 4) == cudaSuccess;
+  for (int i = 0; i < 2 && ok; ++i) ok = cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && cudaMemsetAsync(tk, 0, (size_t)kAllChunk * 4, c->st) == cudaSuccess;
+  if (!ok) {
+    ns_set_error("ns_llama_eval_all: allocation failed");
+    for (void* q : {(void*)lg, (void*)tk, (void*)io}) dev_free(c, q);
+    if (h) cudaFreeHost(h);
+    for (cudaEvent_t e : ev)
+      if (e) cudaEventDestroy(e);
+    return NS_E_CUDA;
+  }
+  c->all_logits = lg;
+  c->lp_tickets = tk;
+  c->all_io = io;
+  c->h_all = h;
+  c->all_ev[0] = ev[0];
+  c->all_ev[1] = ev[1];
+  return NS_OK;
+}
+
+// model_eval with logits_all (llama.cpp:743-747) over the segments of ns_llama_eval_batch: the same body, then the final RMSNorm
+// over all T rows (folded into the lm_head where enqueue_forward folds it: one chunk of a row count ns_rmsnorm_fusable takes) and,
+// per chunk of <= kAllChunk rows, the lm_head on its own route -- never the bf16 GEMM -- and one log-prob launch
+extern "C" int ns_llama_eval_all(ns_llama* c, int n, const int* seq, const int* n_tokens, const int32_t* tokens, const int* n_past,
+                                 const int32_t* targets, float* logprobs, int32_t* argmax, float* logits_host) {
+  const char* who = "ns_llama_eval_all";
+  if (int rc = ns_ensure_device()) return rc;
+  BatchPlan p;
+  if (int rc = check_pass(c, who, n, seq, n_tokens, tokens, n_past, p)) return rc;
+  const int V = c->hp.n_vocab, E = c->hp.n_embd, T = p.T;
+  if ((!targets) != (!logprobs) || (!logprobs && !argmax && !logits_host)) {
+    ns_set_error("%s: targets and logprobs must be both null or both non-null, and one output at least non-null", who);
+    return NS_E_INVALID;
+  }
+  if (targets)
+    for (int r = 0; r < T; ++r)
+      if (targets[r] < 0 || targets[r] >= V) {
+        ns_set_error("%s: target %d of row %d outside [0, n_vocab %d)", who, targets[r], r, V);
+        return NS_E_INVALID;
+      }
+  if (c->sampling) {
+    ns_set_error("%s: sampling is on (a scoring pass draws nothing; set greedy first)", who);
+    return NS_E_UNSUPPORTED;
+  }
+  if (int rc = check_complete(c)) return rc;
+  if (int rc = ensure_buffers(c, T)) return rc;
+  if (int rc = ensure_all_rows(c)) return rc;
+  cudaStream_t st = c->st;
+  MixedPass mix;
+  if (int rc = stage_segments(c, n, seq, n_tokens, tokens, n_past, p, &mix)) return rc;
+  // caller row of each internal row; targets up in internal order
+  std::vector<int> off(n, 0), dst(T);
+  for (int i = 1; i < n; ++i) off[i] = off[i - 1] + n_tokens[i - 1];
+  for (int j = 0; j < n; ++j)
+    for (int t = 0; t < n_tokens[p.order[j]]; ++t) dst[p.first[j] + t] = off[p.order[j]] + t;
+  int* h_tgt = c->h_all;
+  float* h_lp = reinterpret_cast<float*>(c->h_all + kMaxBatchRows);
+  int* h_am = c->h_all + 2 * kMaxBatchRows;
+  float* h_stage = reinterpret_cast<float*>(c->h_all + 3 * kMaxBatchRows);
+  if (targets) {
+    for (int r = 0; r < T; ++r) h_tgt[r] = targets[dst[r]];
+    NS_CUDA_TRY(cudaMemcpyAsync(c->all_io, h_tgt, (size_t)T * 4, cudaMemcpyHostToDevice, st));
+  }
+  // one-token segments only: the kernels of ns_llama_decode_batch's graph, eagerly
+  if (int rc = enqueue_body(c, T, false, false, 0, p.d == n, p.d == n ? nullptr : &mix)) return rc;
+  const ns_weight* outw[1] = {c->output};
+  const bool fold = T <= kAllChunk && ns_rmsnorm_fusable(outw, 1, T);
+  if (!fold)
+    if (int rc = launch_rmsnorm(c->x, c->out_norm, c->xn, T, E, c->hp.norm_eps, st)) return rc;
+  LogprobLaunch a{};
+  a.logits = c->all_logits;
+  a.n_vocab = V;
+  a.tickets = c->lp_tickets;
+  a.pmax = reinterpret_cast<float*>(c->lp_tickets + kAllChunk);
+  a.pidx = reinterpret_cast<int*>(a.pmax + kAllChunk * kLogprobSlices);
+  a.psum = reinterpret_cast<float*>(a.pidx + kAllChunk * kLogprobSlices);
+  int* d_lp = c->all_io + kMaxBatchRows;
+  int* d_am = c->all_io + 2 * kMaxBatchRows;
+  const size_t chunk_floats = (size_t)kAllChunk * V;
+  auto scatter = [&](int k) {  // chunk k's logits, staged in buffer k & 1, to the caller's rows
+    const float* src = h_stage + (size_t)(k & 1) * chunk_floats;
+    const int r0 = k * kAllChunk, rows = std::min(kAllChunk, T - r0);
+    for (int r = 0; r < rows; ++r) memcpy(logits_host + (size_t)dst[r0 + r] * V, src + (size_t)r * V, (size_t)V * 4);
+  };
+  for (int k = 0; k * kAllChunk < T; ++k) {
+    const int r0 = k * kAllChunk, rows = std::min(kAllChunk, T - r0);
+    // the lm_head never takes the bf16 GEMM: a chunk ns_route would send there takes GEMV tiles
+    const int flags = ns_route(NS_NODE_PLAIN, outw, rows, 0) == NS_PATH_TC ? NS_MM_FORCE_GEMV : 0;
+    if (int rc = fold ? ns_rmsnorm_mul_mat(c->output, c->x, E, c->out_norm, c->hp.norm_eps, c->all_logits, V, rows, nullptr, c->ws, (void*)st)
+                      : ns_mul_mat(c->output, c->xn + (size_t)r0 * E, E, c->all_logits, V, rows, nullptr, nullptr, flags, c->ws, (void*)st))
+      return rc;
+    a.rows = rows;
+    a.targets = targets ? c->all_io + r0 : nullptr;
+    a.logprobs = targets ? reinterpret_cast<float*>(d_lp + r0) : nullptr;
+    a.argmax = d_am + r0;
+    if (int rc = ns_launch_logprob(a, st)) return rc;
+    if (logits_host) {  // the host copies chunk k - 1 out while the device runs chunk k
+      NS_CUDA_TRY(cudaMemcpyAsync(h_stage + (size_t)(k & 1) * chunk_floats, c->all_logits, (size_t)rows * V * 4, cudaMemcpyDeviceToHost, st));
+      NS_CUDA_TRY(cudaEventRecord(c->all_ev[k & 1], st));
+      if (k > 0) {
+        NS_CUDA_TRY(cudaEventSynchronize(c->all_ev[(k - 1) & 1]));
+        scatter(k - 1);
+      }
+    }
+  }
+  if (logprobs) NS_CUDA_TRY(cudaMemcpyAsync(h_lp, d_lp, (size_t)T * 4, cudaMemcpyDeviceToHost, st));
+  if (argmax) NS_CUDA_TRY(cudaMemcpyAsync(h_am, d_am, (size_t)T * 4, cudaMemcpyDeviceToHost, st));
+  NS_CUDA_TRY(cudaStreamSynchronize(st));
+  if (logits_host) scatter((T - 1) / kAllChunk);
+  for (int r = 0; r < T; ++r) {
+    if (logprobs) logprobs[dst[r]] = h_lp[r];
+    if (argmax) argmax[dst[r]] = h_am[r];
   }
   return NS_OK;
 }
