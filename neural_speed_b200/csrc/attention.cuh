@@ -1,0 +1,62 @@
+// attention.cuh -- what the eval step (llama.cu) calls in attention.cu: the attention launchers of one layer and the plan of a
+// pass over the token segments of several sequences.
+#pragma once
+#include <cuda_fp16.h>
+
+#include <vector>
+
+#include "nsb.cuh"
+
+constexpr int kMaxSeq = 32;  // KV blocks of one context (ns_llama_set_sequences)
+constexpr int kMaxBatchRows = 4096;  // rows of one pass over segments; the caller chunks longer prompts
+constexpr int kAttnMmaRows = 64, kAttnMmaKeys = 64;
+constexpr int kTileInts = 5;  // ints per entry of the ragged tile table
+
+struct AttnAttr {  // dynamic shared memory already granted to each kernel (function attributes are per device)
+  size_t generic = 0, rows = 0;
+  bool decode = false;
+};
+// {cos, sin} of the one-position back shift per rotary pair, fp16 (model_utils.cpp:165-192); passed by value
+struct ShiftTable {
+  __half2 cs[64];
+};
+
+int attn_ranges(int n_ctx);  // 256-position ranges of the split decode attention
+size_t attn_rows_smem(int hd, int n_ctx);  // dynamic shared memory of attn_fast_kernel
+ShiftTable shift_table(int hd, float freq_base);
+
+// part: [n_head][attn_ranges(n_ctx)][hd + 2] floats, tickets: [n_head] zero words (both read by attn_decode_kernel only; the
+// last CTA of a head leaves its ticket at zero again).  ring (nullable): one-token steps run the ring variant of the split decode
+// attention with ring->n_keep sink slots; prompts (m > 1, which never reach past n_ctx) run the plain kernels.
+struct Ring {
+  int n_keep;
+  ShiftTable tab;
+};
+int launch_attention(int kind, float* q, const float* k, const float* v, __half* kc, __half* vc, const int* state, float* out,
+                     float* part, unsigned* tickets, int n_head, int n_head_kv, int hd, int n_ctx, int m, float rope_theta,
+                     float rope_scale, AttnAttr& attr, cudaStream_t st, const Ring* ring);
+
+// Batched decode attention: one new token for each of n sequences, one launch (attn_decode_kernel<HD, false, true>).  rstate:
+// [n][4] row states (n_past in slot 1), seqs [n] KV block per row, caches [n_seq][n_head_kv][n_ctx][hd] fp16, q / out
+// [n][n_head * hd], k / v [n][n_head_kv * hd], part [n][n_head][ranges][hd + 2], tickets [n][n_head].  hd 64 / 128 only.
+int launch_attention_batch(const float* q, const float* k, const float* v, __half* kc, __half* vc, const int* rstate,
+                           const int* seqs, float* out, float* part, unsigned* tickets, int n, int n_head, int n_head_kv, int hd,
+                           int n_ctx, float rope_theta, float rope_scale, AttnAttr& attr, cudaStream_t st);
+
+// Ragged prompt attention: RoPE + KV append of n_rows rows (rows [n_rows][2] = {position, block}), then attn_mma_kernel<RAGGED> over
+// n_tiles tile entries.  q / out [n_rows][n_head * hd], k / v [n_rows][n_head_kv * hd], caches [n_seq][n_head_kv][n_ctx][hd] fp16.
+int launch_attention_ragged(float* q, const float* k, const float* v, __half* kc, __half* vc, const int* rows, const int* tiles,
+                            int n_rows, int n_tiles, float* out, int n_head, int n_head_kv, int hd, int n_ctx, float rope_theta,
+                            float rope_scale, cudaStream_t st);
+
+// Checks the rows of a batched call: 1 <= n <= n_seq, every id in [0, n_seq) and distinct, 0 <= n_past[i], n_past[i] + steps <= n_ctx
+int check_rows(const char* who, int n_seq, int n, const int* seq, const int* n_past, int steps, int n_ctx);
+
+// The plan of ns_llama_eval_batch: internal order = the one-token segments, then the longer ones, each group in the caller's order.
+// Rows 0 .. d - 1 take the batched decode attention, rows d .. T - 1 the ragged prompt attention (tile rows counted from row d).
+struct BatchPlan {
+  int T = 0, d = 0;
+  std::vector<int> order, first, rows, tiles;
+};
+int plan_batch(const char* who, int n_seq, int n_ctx, int n, const int* seq, const int* n_tokens, const int* n_past,
+               BatchPlan& p);

@@ -131,7 +131,7 @@ def soft_max_f16table(s):
     return (e * np.float32(1.0 / np.float64(e.astype(np.float64).sum()))).astype(np.float32)
 
 
-SPLIT_KEYS = 256  # positions per context range of the split decode attention (kSplitKeys in csrc/llama.cu)
+SPLIT_KEYS = 256  # positions per context range of the split decode attention (kSplitKeys in csrc/attention.cu)
 
 
 def attention_scores(q, kc, n_past, n_head_kv=None):
