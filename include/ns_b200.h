@@ -457,8 +457,61 @@ NS_API int ns_llama_sample(const float* logits, int n, int n_vocab, const int32_
 NS_API void ns_sample_seed_host(uint32_t seed, uint32_t* state);
 NS_API int ns_sample_row_host(const float* logits, int n_vocab, const int32_t* window, int n_window, const ns_llama_sampling* s,
                               uint32_t* state, int32_t* pick, int* kept, int32_t* ids, float* probs);
+/* ---- beam search (the reference's Model.generate(num_beams > 1, do_sample=False): beam_search -> beam_search_flow::loop,
+ * model_utils.cpp:2302-2766, 2939-2944) over n requests of B = num_beams beams each.  Request r owns KV blocks r B .. r B + B - 1
+ * (their contents afterwards are unspecified); blocks from n B up are not touched.  Per step:
+ *   candidates  each running beam's top 2B tokens by logit (B of beam 0 on the first step), scored log softmax + the beam's score
+ *               (neural_speed_b200/csrc/beam.h states the arithmetic; on steps after the first, EOS is forbidden while fewer than
+ *               min_new_tokens were generated: the reference's first step reads the inputs' default min_new_tokens, 0)
+ *   selection   per request the top 2B candidates of all its beams; an EOS candidate ranked below B is dropped, one above scores its
+ *               beam into the hypotheses (score / generated length ^ length_penalty, in double); the first B others become the
+ *               next beams.  Ties: candidates by (score descending, beam ascending, id ascending); hypotheses by score, a later one
+ *               above an earlier one.
+ *   end         a request is done with max_new_tokens tokens, or with early_stopping once B hypotheses exist; then every current
+ *               beam is scored into the hypotheses (unless done by early stopping) and the best one is the response.
+ * The first step evaluates the prompts in one ns_llama_eval_batch pass; every later one replays the captured batched decode step
+ * of the running beams, one candidates launch, one device-to-host copy of the candidates and at most one KV copy launch (a beam
+ * that is not its source's first descendant takes a dropped beam's block and its source's generated positions). */
+typedef struct ns_llama_beams {
+  int num_beams;          /* 2 .. 32, with n * num_beams <= n_seq and 2 * num_beams <= n_vocab */
+  int max_new_tokens;     /* >= 1 (the reference's n_predict) */
+  int min_new_tokens;     /* >= 0: EOS forbidden before this many generated tokens, from the second step on */
+  float length_penalty;   /* finite */
+  int early_stopping;     /* 0 / 1 */
+  int32_t eos_token_id;   /* [0, n_vocab) */
+} ns_llama_beams;
+/* prompts: n_tokens[r] >= 1 tokens each, back to back in `tokens`, with n_tokens[r] + max_new_tokens - 1 <= n_ctx (the last pick
+ * is never evaluated).  out_tokens [n][max_new_tokens]: request r's response in out_tokens[r][0 .. out_len[r]); out_score [n]
+ * (nullable): its length-penalised score.  NS_E_UNSUPPORTED while sampling or streaming is on, for a head size other than
+ * 64 / 128, or in exact-prefill mode for prompts of more than 32 tokens in all (the prompt pass is ns_llama_eval_batch's); NS_E_INVALID for a field or length out of range or a null pointer.  A refused call launches nothing. */
+NS_API int ns_llama_beam_search(ns_llama* ctx, int n, const int* n_tokens, const int32_t* tokens, const ns_llama_beams* cfg,
+                                int32_t* out_tokens, int* out_len, float* out_score);
+/* model_kv_cache_seq_cpy (model_utils.cpp:2058-2064) in one launch: positions [p0, p1) of KV block src[i] into block dst[i] for
+ * i < n, every layer, K and V.  NS_E_INVALID (nothing launched) for a block outside [0, n_seq), a destination that is also a
+ * source or appears twice, n outside [1, n_seq], or 0 <= p0 <= p1 <= n_ctx not holding. */
+NS_API int ns_llama_kv_copy(ns_llama* ctx, int n, const int* src, const int* dst, int p0, int p1);
+/* The candidates kernel on its own, for parity tests: one launch over device logits [n][n_vocab] (1 <= n <= 32), k in 1 .. 64;
+ * prev [n] and mask [n] host arrays (mask[r]: row r's EOS logit is -FLT_MAX).  out: device [n][min(k, n_vocab)] {int32 id,
+ * float score}.  ws: device workspace of ns_llama_beam_candidates_workspace_bytes(n, k) bytes, zeroed once by the caller: its
+ * tickets lie in the first 128 bytes and are zero again after every call. */
+NS_API size_t ns_llama_beam_candidates_workspace_bytes(int n, int k);
+NS_API int ns_llama_beam_candidates(const float* logits, int n, int n_vocab, int k, const float* prev, const int* mask, int32_t eos,
+                                    void* out, void* ws, void* queue);
+/* Host restatement of one row (no device needed), bit for bit what the kernel computes: ids [min(k, n_vocab)] and scores. */
+NS_API int ns_beam_candidates_row_host(const float* logits, int n_vocab, int k, float prev, int mask, int32_t eos, int32_t* ids,
+                                       float* scores);
+/* The library's log (ns_logf), for tests. */
+NS_API float ns_logf_host(float x);
+/* The flow of ns_llama_beam_search without a device: logits(user, rows, req, hist, hist_len, out) fills out [rows][n_vocab] with
+ * the logits of each row's last token, row i being request req[i] with the token history hist[i][0 .. hist_len[i]) (prompt then
+ * generated tokens); it returns 0 or an error that ends the search.  The first call holds the n prompts. */
+typedef int (*ns_beam_logits_fn)(void* user, int rows, const int* req, const int32_t* const* hist, const int* hist_len, float* out);
+NS_API int ns_beam_search_host(int n_vocab, int n_ctx, int n, const int* n_tokens, const int32_t* tokens, const ns_llama_beams* cfg,
+                               ns_beam_logits_fn logits, void* user, int32_t* out_tokens, int* out_len, float* out_score);
 NS_API float ns_sample_expf_host(float x);
 NS_API unsigned long long ns_llama_kv_bytes(const ns_llama* ctx); /* all n_seq blocks */
+/* The device pointers of the fp16 KV cache, [n_layer][n_seq][n_head_kv][n_ctx][head size] each for K and V (for tests). */
+NS_API int ns_llama_kv_cache(const ns_llama* ctx, void** k, void** v);
 /* One layer's attention of the eval step on its own, for parity tests: RoPE (mode 0, angle = p * rope_theta^(-2i/hd) / rope_scale)
  * of q [m][n_head * hd] in place and of the m new rows k [m][n_head_kv * hd] at positions n_past .. n_past + m - 1, k and v appended
  * to the fp16 caches kc / vc [n_head_kv][n_ctx][hd], out [m][n_head * hd] = causal softmax(K q / sqrt(hd)) V (llama.cpp:286-302).

@@ -65,6 +65,8 @@ EXPORTS = [
     "ns_llama_eval_batch", "ns_llama_batch_plan", "ns_llama_attention_ragged_workspace_bytes", "ns_llama_attention_ragged",
     "ns_llama_set_sampling", "ns_llama_sample_workspace_bytes", "ns_llama_sample", "ns_sample_seed_host", "ns_sample_row_host",
     "ns_sample_expf_host", "ns_llama_eval_all", "ns_llama_logprob_workspace_bytes", "ns_llama_logprob", "ns_logprob_row_host",
+    "ns_llama_beam_search", "ns_llama_kv_copy", "ns_llama_kv_cache", "ns_llama_beam_candidates_workspace_bytes", "ns_llama_beam_candidates",
+    "ns_beam_candidates_row_host", "ns_logf_host", "ns_beam_search_host",
     "ns_comm_handle_bytes", "ns_comm_create", "ns_comm_get_handle", "ns_comm_open_peers", "ns_comm_link_local", "ns_comm_all_reduce_f32",
     "ns_comm_status", "ns_comm_free",
 ]
@@ -217,6 +219,16 @@ def lib() -> C.CDLL:
     L.ns_llama_logprob_workspace_bytes.argtypes = [i, i]
     L.ns_llama_logprob.argtypes = [vp, i, i, vp, vp, vp, vp, vp]
     L.ns_logprob_row_host.argtypes = [vp, i, C.c_int32, vp, vp]
+    L.ns_llama_beam_search.argtypes = [vp, i, vp, vp, vp, vp, vp, vp]
+    L.ns_llama_kv_copy.argtypes = [vp, i, vp, vp, i, i]
+    L.ns_llama_kv_cache.argtypes = [vp, vp, vp]
+    L.ns_llama_beam_candidates_workspace_bytes.restype = sz
+    L.ns_llama_beam_candidates_workspace_bytes.argtypes = [i, i]
+    L.ns_llama_beam_candidates.argtypes = [vp, i, i, i, vp, vp, C.c_int32, vp, vp, vp]
+    L.ns_beam_candidates_row_host.argtypes = [vp, i, i, C.c_float, i, C.c_int32, vp, vp]
+    L.ns_logf_host.restype = C.c_float
+    L.ns_logf_host.argtypes = [C.c_float]
+    L.ns_beam_search_host.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.ns_comm_handle_bytes.restype = sz
     L.ns_comm_create.restype = vp
     L.ns_comm_create.argtypes = [i, i, sz, vp]
@@ -489,6 +501,22 @@ class Sampling(C.Structure):
                 ("repeat_last_n", C.c_int), ("seed", C.c_uint32)]
 
 
+class Beams(C.Structure):
+    """ns_llama_beams (include/ns_b200.h)"""
+    _fields_ = [("num_beams", C.c_int), ("max_new_tokens", C.c_int), ("min_new_tokens", C.c_int), ("length_penalty", C.c_float),
+                ("early_stopping", C.c_int), ("eos_token_id", C.c_int32)]
+
+
+BEAM_LOGITS_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.POINTER(C.c_int32)), C.POINTER(C.c_int),
+                             C.POINTER(C.c_float))
+
+
+def _prompts(prompts):
+    parts = [np.asarray(p, np.int32).ravel() for p in prompts]
+    lens = np.array([p.size for p in parts], np.int32)
+    return lens, np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0, np.int32))
+
+
 def sampling(top_k=40, top_p=0.95, temperature=0.8, repeat_penalty=1.1, repeat_last_n=64, seed=0) -> Sampling:
     """the reference's do_sample defaults (application/main_pybind.cpp, Model.generate)"""
     return Sampling(top_k, top_p, temperature, repeat_penalty, repeat_last_n, seed & 0xFFFFFFFF)
@@ -621,6 +649,33 @@ class Llama:
                "ns_llama_generate_batch")
         return out
 
+    def beam_search(self, prompts, num_beams=4, max_new_tokens=32, min_new_tokens=0, length_penalty=1.0, early_stopping=False,
+                    eos_token_id=2):
+        """the reference's Model.generate(num_beams > 1, do_sample=False) over the prompts, request r in KV blocks r num_beams ..
+        (include/ns_b200.h, ns_llama_beam_search) -> [(generated tokens, length-penalised score)] per prompt"""
+        lens, t = _prompts(prompts)
+        cfg = Beams(num_beams, max_new_tokens, min_new_tokens, length_penalty, 1 if early_stopping else 0, eos_token_id)
+        n = lens.size
+        out = np.zeros((max(n, 1), max(max_new_tokens, 1)), np.int32)
+        out_len = np.zeros(max(n, 1), np.int32)
+        score = np.zeros(max(n, 1), np.float32)
+        _check(lib().ns_llama_beam_search(self.h, n, _np_ptr(lens), _np_ptr(t), C.byref(cfg), _np_ptr(out), _np_ptr(out_len),
+                                          _np_ptr(score)), "ns_llama_beam_search")
+        return [(out[r, :out_len[r]].copy(), float(score[r])) for r in range(n)]
+
+    def kv_copy(self, src, dst, p0: int, p1: int):
+        """positions [p0, p1) of KV blocks src[i] into blocks dst[i], every layer, K and V, in one launch (ns_llama_kv_copy)"""
+        s, d = np.ascontiguousarray(src, np.int32), np.ascontiguousarray(dst, np.int32)
+        if s.size != d.size:
+            raise ValueError(f"kv_copy: {s.size} sources for {d.size} destinations")
+        _check(lib().ns_llama_kv_copy(self.h, s.size, _np_ptr(s), _np_ptr(d), p0, p1), "ns_llama_kv_copy")
+
+    def kv_cache(self):
+        """(K, V) device pointers of the fp16 cache, [n_layer][n_seq][n_head_kv][n_ctx][head size] each"""
+        k, v = C.c_void_p(), C.c_void_p()
+        _check(lib().ns_llama_kv_cache(self.h, C.byref(k), C.byref(v)), "ns_llama_kv_cache")
+        return k.value, v.value
+
     def close(self):
         if self.h:
             lib().ns_llama_free(self.h)
@@ -716,3 +771,56 @@ def sample(logits_ptr: int, n: int, n_vocab: int, windows_ptr, n_window: int, s:
                                  C.byref(s), C.c_void_p(mt_ptr), C.c_void_p(picks_ptr), C.c_void_p(kept_ptr) if kept_ptr else None,
                                  C.c_void_p(ids_ptr) if ids_ptr else None, C.c_void_p(probs_ptr) if probs_ptr else None,
                                  C.c_void_p(ws_ptr), queue)
+
+
+def beam_candidates_row_host(logits, k: int, prev=0.0, mask=False, eos=2):
+    """one row of the beam candidates kernel's arithmetic on the host (ns_beam_candidates_row_host) -> (ids, scores)"""
+    lg = np.ascontiguousarray(logits, np.float32)
+    K = min(k, lg.size)
+    ids, sc = np.zeros(K, np.int32), np.zeros(K, np.float32)
+    _check(lib().ns_beam_candidates_row_host(_np_ptr(lg), lg.size, k, prev, 1 if mask else 0, eos, _np_ptr(ids), _np_ptr(sc)),
+           "ns_beam_candidates_row_host")
+    return ids, sc
+
+
+def beam_candidates(logits_ptr: int, n: int, n_vocab: int, k: int, prev, mask, eos: int, out_ptr: int, ws_ptr: int, queue=None) -> int:
+    """ns_llama_beam_candidates on device pointers (the candidates kernel's one launch on its own); returns the status code"""
+    p = np.ascontiguousarray(prev, np.float32)
+    m = np.ascontiguousarray(mask, np.int32)
+    return lib().ns_llama_beam_candidates(C.c_void_p(logits_ptr), n, n_vocab, k, _np_ptr(p), _np_ptr(m), eos, C.c_void_p(out_ptr),
+                                          C.c_void_p(ws_ptr), queue)
+
+
+def logf_host(x: float) -> float:
+    return float(lib().ns_logf_host(x))
+
+
+def beam_search_host(n_vocab: int, n_ctx: int, prompts, logits_fn, num_beams=4, max_new_tokens=32, min_new_tokens=0, length_penalty=1.0,
+                     early_stopping=False, eos_token_id=2):
+    """the flow of Llama.beam_search without a device (ns_beam_search_host): logits_fn(req [rows], histories [rows] of token arrays)
+    returns the logits [rows][n_vocab] of each row's last token -> [(tokens, score)] per prompt"""
+    lens, t = _prompts(prompts)
+    cfg = Beams(num_beams, max_new_tokens, min_new_tokens, length_penalty, 1 if early_stopping else 0, eos_token_id)
+    n = lens.size
+    err = []
+
+    def cb(_user, rows, req, hist, hist_len, out):
+        try:
+            hs = [np.ctypeslib.as_array(hist[i], (hist_len[i],)).copy() for i in range(rows)]
+            lg = np.ascontiguousarray(logits_fn([req[i] for i in range(rows)], hs), np.float32)
+            C.memmove(out, lg.ctypes.data, lg.nbytes)
+            return 0
+        except Exception as e:  # noqa: BLE001 -- reported after the call
+            err.append(e)
+            return -1
+
+    fn = BEAM_LOGITS_FN(cb)
+    out = np.zeros((max(n, 1), max(max_new_tokens, 1)), np.int32)
+    out_len = np.zeros(max(n, 1), np.int32)
+    score = np.zeros(max(n, 1), np.float32)
+    rc = lib().ns_beam_search_host(n_vocab, n_ctx, n, _np_ptr(lens), _np_ptr(t), C.byref(cfg), fn, None, _np_ptr(out), _np_ptr(out_len),
+                                   _np_ptr(score))
+    if err:
+        raise err[0]
+    _check(rc, "ns_beam_search_host")
+    return [(out[r, :out_len[r]].copy(), float(score[r])) for r in range(n)]

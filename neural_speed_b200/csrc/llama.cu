@@ -29,6 +29,7 @@
 #include "nsb.cuh"
 #include "sample.h"
 #include "logprob.h"
+#include "beam.h"
 #include "attention.cuh"
 
 namespace {
@@ -251,6 +252,10 @@ struct ns_llama {
   int* all_io = nullptr;              // [3][kMaxBatchRows]
   int* h_all = nullptr;               // [3][kMaxBatchRows] | [2][kAllChunk][n_vocab] floats
   cudaEvent_t all_ev[2] = {};
+  // ns_llama_beam_search (allocated on first use): the candidates kernel's tickets and scratch, its output and pinned staging
+  unsigned* beam_ws = nullptr;        // tickets [kBeamMaxRows] | ns_beam_scratch(kBeamMaxRows, kBeamMaxK)
+  BeamCand* beam_out = nullptr;       // [kBeamMaxRows][kBeamMaxK]
+  BeamCand* h_beam = nullptr;
 };
 
 static void* dev_alloc(ns_llama* c, size_t bytes) {
@@ -370,6 +375,7 @@ extern "C" void ns_llama_free(ns_llama* c) {
   if (c->h_plan) cudaFreeHost(c->h_plan);
   if (c->h_logits) cudaFreeHost(c->h_logits);
   if (c->h_all) cudaFreeHost(c->h_all);
+  if (c->h_beam) cudaFreeHost(c->h_beam);
   for (cudaEvent_t e : c->all_ev)
     if (e) cudaEventDestroy(e);
   delete c;
@@ -1253,6 +1259,144 @@ extern "C" int ns_llama_generate(ns_llama* c, int32_t first_token, int n_past, i
   }
   NS_CUDA_TRY(cudaStreamSynchronize(st));
   advance_position(c, n_past, n_new);
+  return NS_OK;
+}
+
+// ---- beam search ------------------------------------------------------------------------------------------------------
+// The engine of the flow in beam.cu: the prompt pass is ns_llama_eval_batch's, a step is ns_llama_decode_batch's captured step
+// without its readback; each is followed by one candidates launch over the logits and one copy of the candidates to the host.
+namespace {
+struct DeviceBeams : BeamEngine {
+  ns_llama* c;
+  int n;
+  const int* n_tokens;
+  const int32_t* tokens;
+  int eos;
+  const BatchPlan* plan;
+  // K candidates of the rows of the pass just enqueued: logits row j is caller row order[j] (the identity if null)
+  int candidates(const BeamRows& rows, const int* order, int K, BeamCand* out) {
+    BeamLaunch a{};
+    a.logits = c->logits;
+    a.n_vocab = c->hp.n_vocab;
+    a.rows = rows.n;
+    a.k = K;
+    a.eos = eos;
+    for (int j = 0; j < rows.n; ++j) {
+      const int i = order ? order[j] : j;
+      a.prev[j] = rows.prev[i];
+      if (rows.mask[i]) a.mask |= 1u << j;
+    }
+    a.out = c->beam_out;
+    a.tickets = c->beam_ws;
+    ns_beam_scratch(a, c->beam_ws + kBeamMaxRows, rows.n, K);
+    if (int rc = ns_launch_beam_candidates(a, c->st)) return rc;
+    NS_CUDA_TRY(cudaMemcpyAsync(c->h_beam, c->beam_out, (size_t)rows.n * K * sizeof(BeamCand), cudaMemcpyDeviceToHost, c->st));
+    NS_CUDA_TRY(cudaStreamSynchronize(c->st));
+    for (int j = 0; j < rows.n; ++j) memcpy(out + (size_t)(order ? order[j] : j) * K, c->h_beam + (size_t)j * K, (size_t)K * sizeof(BeamCand));
+    return NS_OK;
+  }
+  int prompts(const BeamRows& rows, int K, BeamCand* out) override {
+    std::vector<int> seq(rows.block, rows.block + n), n_past(n, 0);
+    if (plan->d == n) {  // one-token prompts: the captured batched step, as ns_llama_eval_batch takes it
+      if (int rc = stage_batch(c, n, seq.data(), tokens, n_past.data())) return rc;
+      NS_CUDA_TRY(cudaGraphLaunch(c->graph[n].exec, c->st));
+      return candidates(rows, nullptr, K, out);
+    }
+    Pass s;
+    if (int rc = stage_segments(c, n, seq.data(), n_tokens, tokens, n_past.data(), *plan, &s)) return rc;
+    if (int rc = enqueue_forward(c, s)) return rc;
+    return candidates(rows, plan->order.data(), K, out);
+  }
+  int step(const BeamRows& rows, int K, BeamCand* out) override {
+    if (int rc = stage_batch(c, rows.n, rows.block, rows.tok, rows.n_past)) return rc;
+    NS_CUDA_TRY(cudaGraphLaunch(c->graph[rows.n].exec, c->st));
+    return candidates(rows, nullptr, K, out);
+  }
+  int copy(const KvCopyPairs& p) override {
+    const ns_llama_hparams& hp = c->hp;
+    return ns_launch_kv_copy(p, c->kc, c->vc, hp.n_layer, c->n_seq, hp.n_head_kv, hp.n_ctx, hp.n_embd / hp.n_head, c->st);
+  }
+};
+}  // namespace
+
+static int ensure_beams(ns_llama* c) {
+  if (c->beam_ws) return NS_OK;
+  const size_t wsb = (size_t)kBeamMaxRows * 4 + ns_beam_scratch_bytes(kBeamMaxRows, kBeamMaxK);
+  unsigned* ws = (unsigned*)dev_alloc(c, wsb);
+  BeamCand* out = (BeamCand*)dev_alloc(c, (size_t)kBeamMaxRows * kBeamMaxK * sizeof(BeamCand));
+  BeamCand* h = nullptr;
+  bool ok = ws && out && cudaMallocHost((void**)&h, (size_t)kBeamMaxRows * kBeamMaxK * sizeof(BeamCand)) == cudaSuccess;
+  ok = ok && cudaMemsetAsync(ws, 0, (size_t)kBeamMaxRows * 4, c->st) == cudaSuccess;
+  if (!ok) {
+    ns_set_error("ns_llama_beam_search: allocation failed");
+    dev_free(c, ws);
+    dev_free(c, out);
+    if (h) cudaFreeHost(h);
+    return NS_E_CUDA;
+  }
+  c->beam_ws = ws;
+  c->beam_out = out;
+  c->h_beam = h;
+  return NS_OK;
+}
+
+extern "C" int ns_llama_beam_search(ns_llama* c, int n, const int* n_tokens, const int32_t* tokens, const ns_llama_beams* cfg,
+                                    int32_t* out_tokens, int* out_len, float* out_score) {
+  const char* who = "ns_llama_beam_search";
+  if (int rc = ns_ensure_device()) return rc;
+  if (!c || !n_tokens || !tokens || !cfg || !out_tokens || !out_len) {
+    ns_set_error("%s: null pointer", who);
+    return NS_E_INVALID;
+  }
+  const int hd = c->hp.n_embd / c->hp.n_head;
+  if (c->sampling || c->streaming || (hd != 64 && hd != 128)) {
+    ns_set_error("%s: %s", who, c->sampling ? "sampling is on (the reference searches beams only with do_sample off)"
+                                : c->streaming ? "streaming is on (the reference's beam search has no shifted cache, model_utils.cpp:2245)"
+                                               : "head size other than 64 / 128 (the batched decode attention)");
+    return NS_E_UNSUPPORTED;
+  }
+  if (int rc = ns_beam_check(who, cfg, n, n_tokens, c->hp.n_ctx, c->hp.n_vocab, c->n_seq)) return rc;
+  const int B = cfg->num_beams;
+  std::vector<int> seq(n), n_past(n, 0);
+  for (int r = 0; r < n; ++r) seq[r] = r * B;
+  BatchPlan p;
+  if (int rc = plan_batch(who, c->n_seq, c->hp.n_ctx, n, seq.data(), n_tokens, n_past.data(), p)) return rc;
+  if (int rc = check_context(c, who, std::max(p.T, n * B), true)) return rc;
+  if (int rc = ensure_beams(c)) return rc;
+  DeviceBeams e;
+  e.c = c;
+  e.n = n;
+  e.n_tokens = n_tokens;
+  e.tokens = tokens;
+  e.eos = cfg->eos_token_id;
+  e.plan = &p;
+  return ns_beam_flow(*cfg, n, n_tokens, tokens, e, out_tokens, out_len, out_score);
+}
+
+extern "C" int ns_llama_kv_copy(ns_llama* c, int n, const int* src, const int* dst, int p0, int p1) {
+  if (int rc = ns_ensure_device()) return rc;
+  if (!c || !src || !dst || n < 1 || n > std::min(c->n_seq, kBeamMaxRows)) {
+    ns_set_error("ns_llama_kv_copy: null pointer or %d pairs (1 .. %d)", n, c ? std::min(c->n_seq, kBeamMaxRows) : 0);
+    return NS_E_INVALID;
+  }
+  KvCopyPairs a;
+  a.n = n;
+  for (int i = 0; i < n; ++i) {
+    a.src[i] = src[i];
+    a.dst[i] = dst[i];
+    a.p0[i] = p0;
+    a.p1[i] = p1;
+  }
+  const ns_llama_hparams& hp = c->hp;
+  if (int rc = ns_launch_kv_copy(a, c->kc, c->vc, hp.n_layer, c->n_seq, hp.n_head_kv, hp.n_ctx, hp.n_embd / hp.n_head, c->st)) return rc;
+  NS_CUDA_TRY(cudaStreamSynchronize(c->st));
+  return NS_OK;
+}
+
+extern "C" int ns_llama_kv_cache(const ns_llama* c, void** k, void** v) {
+  if (!c || !k || !v) return NS_E_INVALID;
+  *k = c->kc;
+  *v = c->vc;
   return NS_OK;
 }
 
