@@ -259,6 +259,20 @@ NS_API int ns_prepare_activation(const ns_weight* w, const float* act, int lda, 
 NS_API int ns_matmul_prepared(const ns_weight* const* weights, int nw, int mode, const void* workspace, float* dst, int ldo,
                               int m, const float* bias, int bias_bcast, const float* residual, float* aux, void* queue);
 
+/* The decode GEMV's launch plan on its own, for parity tests (no device needed): how ns_mul_mat & co. run one launch of m <= 4
+ * activation rows of int4 weights with an integer compute type (k, group, stype, asym, comp as ns_weight_from_unpacked; Q4_0:
+ * group 32, NS_S_F16, asym 0, NS_COMP_Q8_0) in mode 0 / 1 / 2 of ns_matmul_prepared.  fused: the kernel quantises fp32
+ * activations itself (the ns_mul_mat path for groups of 32..256 dividing k), else it reads an ns_prepare_activation image;
+ * norm: a folded RMSNorm (fused, m <= 2).  out[5] = {wide (1: one CTA per SM with 14 consumer warps, 0: the 7-warp kernel),
+ * weight rows per ring stage (2 or 1), ring stages, stage-owning consumer warps, CTAs per SM}.  Returns 1 when the launch has
+ * a plan, 0 when none fits shared memory (the matmul calls then refuse the node with NS_E_UNSUPPORTED before launching
+ * anything), NS_E_INVALID for a launch the ring does not run. */
+NS_API int ns_gemv_ring_plan(int k, int group, int stype, int asym, int comp, int mode, int m, int fused, int norm, int* out);
+/* ns_mul_mat as the eval step runs its GEMV nodes, for parity tests: on the kernel image that can fold an RMSNorm, without one
+ * (one image for every node of a token); no bias, optional residual */
+NS_API int ns_mul_mat_engine_image(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* residual,
+                                   void* workspace, void* queue);
+
 /* CUDA-graph capture of a sequence of calls on one queue (replaces the reference's per-token graph rebuild +
  * ne_graph_compute, models/llama/llama.cpp:136-143 / core/ne_layers.c:11915): begin, issue ns_* device calls with
  * caller-provided workspaces (no allocation may happen while capturing), end -> executable graph handle. */

@@ -628,10 +628,14 @@ int ns_route(int kind, const ns_weight* const* w, int m, int flags) {
   if (kind == NS_NODE_FFN)  // shuffles are checked on gate/up only
     tc = tc && ns_gemm_tc_supported(w[2]) && (!w[1] || ns_gemm_tc_supported(w[1])) && !w[0]->shuffle && !(w[1] && w[1]->shuffle);
   if (tc) return NS_PATH_TC;
-  // the weights of the first launch must fit one GEMV launch, and an FFN's down projection one of its own
-  if (int rc = ns_gemv_check(w, nw, kind == NS_NODE_QKV ? NS_GEMV_CONCAT : nw == 2 ? NS_GEMV_GATE_UP_SILU : NS_GEMV_PLAIN)) return rc;
-  if (kind == NS_NODE_FFN)
+  // the weights of the first launch must fit one GEMV launch, and an FFN's down projection one of its own; every tile of both
+  // must have a kernel plan, so that a node the ring cannot run is refused before any of its launches is issued
+  if (int rc = ns_gemv_check(w, nw, mode)) return rc;
+  if (int rc = ns_gemv_planned(w, nw, mode, m, (flags & NS_ROUTE_NORM) != 0)) return rc;
+  if (kind == NS_NODE_FFN) {
     if (int rc = ns_gemv_check(&w[2], 1, NS_GEMV_PLAIN)) return rc;
+    if (int rc = ns_gemv_planned(&w[2], 1, NS_GEMV_PLAIN, m, false)) return rc;
+  }
   return NS_PATH_GEMV;
 }
 
@@ -718,7 +722,7 @@ static int mul_mat_impl(const ns_weight* w, const float* act, int lda, float* ds
     return NS_E_INVALID;
   }
   if (norm_w && !norm_foldable(&w, 1, m)) return norm_unsupported("ns_rmsnorm_mul_mat");
-  const int path = ns_route(NS_NODE_PLAIN, &w, m, flags);
+  const int path = ns_route(NS_NODE_PLAIN, &w, m, (flags & ~NS_ROUTE_NORM) | (norm_w ? NS_ROUTE_NORM : 0));
   if (path < 0) return path;
   cudaStream_t st = stream_of(queue);
   void* ws = pick_ws(workspace, st, path_workspace_bytes(path, m, w->kpad));
@@ -734,6 +738,10 @@ int ns_mul_mat_engine(const ns_weight* w, const float* act, int lda, float* dst,
                       cudaStream_t st, const float* norm_w, float norm_eps) {
   return mul_mat_impl(w, act, lda, dst, ldo, m, nullptr, residual, 0, workspace, (void*)st, norm_w, norm_eps, 1);
 }
+extern "C" int ns_mul_mat_engine_image(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* residual,
+                                       void* workspace, void* queue) {
+  return mul_mat_impl(w, act, lda, dst, ldo, m, nullptr, residual, 0, workspace, queue, nullptr, 0.f, 1);
+}
 // dst = W * (rms_norm(act) * norm_w) [+ residual]: ne_rms_norm + ne_mul + ne_mul_mat (llama.cpp:205-215, :703-712) as ONE launch
 extern "C" int ns_rmsnorm_mul_mat(const ns_weight* w, const float* act, int lda, const float* norm_w, float norm_eps, float* dst,
                                   int ldo, int m, const float* residual, void* workspace, void* queue) {
@@ -747,7 +755,7 @@ int ns_mul_qkv_norm(const ns_weight* wq, const ns_weight* wk, const ns_weight* w
   if (!wq || !wk || !wv || !act || !dst || m <= 0) return NS_E_INVALID;
   const ns_weight* wl[3] = {wq, wk, wv};
   if (norm_w && !norm_foldable(wl, 3, m)) return norm_unsupported("ns_rmsnorm_mul_qkv");
-  const int path = ns_route(NS_NODE_QKV, wl, m, 0);
+  const int path = ns_route(NS_NODE_QKV, wl, m, norm_w ? NS_ROUTE_NORM : 0);
   if (path < 0) return path;
   cudaStream_t st = stream_of(queue);
   void* ws = pick_ws(workspace, st, path_workspace_bytes(path, m, wq->kpad));
@@ -779,7 +787,7 @@ static int ffn_impl(const ns_weight* w1, const ns_weight* w2, const ns_weight* w
   const ns_weight* wn[3] = {w1, w3, w2};
   const int ngu = w3 ? 2 : 1, fmid = w1->n;
   if (norm_w && !norm_foldable(wn, ngu, m)) return norm_unsupported("fused FFN");
-  const int path = ns_route(NS_NODE_FFN, wn, m, 0);
+  const int path = ns_route(NS_NODE_FFN, wn, m, norm_w ? NS_ROUTE_NORM : 0);
   if (path < 0) return path;
   cudaStream_t st = stream_of(queue);
   void* ws = pick_ws(workspace, st, path_workspace_bytes(path, m, w1->kpad > w2->kpad ? w1->kpad : w2->kpad));
@@ -815,6 +823,30 @@ extern "C" int ns_rmsnorm_ffn_silu(const ns_weight* w1, const ns_weight* w2, con
   if (!w3 || !norm_w) return NS_E_INVALID;
   return ffn_impl(w1, w2, w3, NS_ELT_DEFAULT, nullptr, nullptr, 0, act, lda, tmp, dst, ldo, m, workspace, queue, residual, norm_w,
                   norm_eps);
+}
+extern "C" int ns_gemv_ring_plan(int k, int group, int stype, int asym, int comp, int mode, int m, int fused, int norm, int* out) {
+  ns_weight w;
+  memset(&w, 0, sizeof(w));
+  w.n = 2, w.k = k, w.group = group, w.wfmt = NS_W_S4, w.stype = stype, w.comp = comp, w.asym = asym ? 1 : 0;
+  if (k < 1 || stype < NS_S_F32 || stype > NS_S_F16 || !(comp == NS_COMP_INT8 || comp == NS_COMP_INT8_S8 || comp == NS_COMP_Q8_0) ||
+      mode < NS_GEMV_PLAIN || mode > NS_GEMV_GATE_UP_SILU || !out) {
+    ns_set_error("ns_gemv_ring_plan: not a ring GEMV launch (k=%d stype=%d comp=%d mode=%d)", k, stype, comp, mode);
+    return NS_E_INVALID;
+  }
+  ns_weight_layout(&w);
+  if (w.group % 32 && w.group != w.k) {
+    ns_set_error("ns_gemv_ring_plan: group size %d is not a multiple of 32", w.group);
+    return NS_E_INVALID;
+  }
+  if (m < 1 || m > ns_gemv_tile_rows(&w) || (fused && !ns_gemv_fused_quant_ok(&w)) || (norm && (!fused || m > 2))) {
+    ns_set_error("ns_gemv_ring_plan: no such launch (m=%d of at most %d, fused=%d, norm=%d)", m, ns_gemv_tile_rows(&w), fused, norm);
+    return NS_E_INVALID;
+  }
+  RingChoice c;
+  const bool ok = ns_gemv_ring_choose(w.kpad, w.pitch, mode, m >= 3 ? 4 : m, fused != 0, norm != 0, &c);
+  out[0] = ok && c.wide, out[1] = ok ? c.plan.rows : 0, out[2] = ok ? c.plan.stages : 0, out[3] = ok ? c.plan.active : 0;
+  out[4] = ok ? c.plan.ctas : 0;
+  return ok ? 1 : 0;
 }
 extern "C" int ns_rmsnorm_fusable(const ns_weight* const* weights, int nw, int m) {
   return (weights && nw >= 1 && nw <= 3 && norm_foldable(weights, nw, m)) ? 1 : 0;

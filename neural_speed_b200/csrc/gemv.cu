@@ -421,6 +421,25 @@ int ns_gemv_check(const ns_weight* const* ws_, int nw, int mode) {
   return NS_OK;
 }
 
+int ns_gemv_planned(const ns_weight* const* ws, int nw, int mode, int m, bool norm) {
+  const ns_weight* w0 = ws[0];
+  (void)nw;
+  if (!(w0->wfmt == NS_W_S4 && !float_mode(w0))) return NS_OK;  // the register GEMV: ns_gemv_check has sized its launch
+  const int tile = ns_gemv_tile_rows(w0);
+  const bool fused = ns_gemv_fused_quant_ok(w0);
+  const int rows[2] = {m < tile ? m : tile, m % tile};  // the full tiles and the last one
+  for (int t : rows) {
+    if (t < 1) continue;
+    RingChoice c;
+    if (!ns_gemv_ring_choose(w0->kpad, w0->pitch, mode, t >= 3 ? 4 : t, fused, norm && fused, &c)) {
+      ns_set_error("ring GEMV: no shared-memory plan for a %d-row tile of k=%d (row pitch %d B%s)", t, w0->k, w0->pitch,
+                   mode == NS_GEMV_GATE_UP_SILU ? ", gate/up row pairs" : "");
+      return NS_E_UNSUPPORTED;
+    }
+  }
+  return NS_OK;
+}
+
 int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* act_ws, float* dst, int ldo, int m,
                    int m_total, const float* bias, int bias_bcast, const float* residual, float* aux, cudaStream_t st,
                    const float* act_f32, int lda, int eltop, const float* norm_w, float norm_eps, int one_image) {

@@ -1,4 +1,4 @@
-// gemv_ring_impl.cuh -- the ring GEMV kernel template, its activation prologue, its shared-memory planner and launcher.  Included by gemv_ring.cu (two CTAs
+// gemv_ring_impl.cuh -- the ring GEMV kernel template, its activation prologue and launcher (the plan: ns_gemv_ring_choose).  Included by gemv_ring.cu (two CTAs
 // per SM, 7 consumer warps) and gemv_ring_wide.cu (one CTA per SM, 14 consumer warps): two translation units so that the ~170
 // instantiations compile in parallel.  See gemv_ring.cu for the design notes.
 #pragma once
@@ -519,42 +519,6 @@ __global__ void __launch_bounds__((NC + (NC > kConsumers ? 2 : 1)) * 32, NC > kC
       }
     }
   }
-}
-
-struct RingPlan {
-  int rows, stages, active, ctas;
-  size_t budget;
-  double score;
-};
-
-// Shared-memory plan.  Candidates: row pairs or single rows per stage, half an SM (two CTAs per SM) or a whole SM.  The score
-// is the number of consumer warps per SM that own a stage; pairs share the activation loads between two rows (measured:
-// K = 11008 with 7 pair stages beats 14 single-row stages, 950 vs 937 tok/s), so single rows are only taken when pairs would
-// leave consumer warps without a stage (K >= ~14000).  Ties go to the deeper ring.
-static RingPlan plan_ring(const GemvParams& P, size_t act_region, bool wide) {
-  static const int env_budget = getenv("NS_RING_BUDGET_KB") ? atoi(getenv("NS_RING_BUDGET_KB")) : 0;  // tuning aids
-  static const int env_rows = getenv("NS_RING_ROWS") ? atoi(getenv("NS_RING_ROWS")) : 0;
-  const size_t budgets[2] = {(size_t)(env_budget > 0 ? env_budget : 113) * 1024, 200 * 1024};
-  RingPlan best = {0, 0, 0, 0, 0, -1.0};
-  for (int rows = 2; rows >= 1; --rows) {
-    if (rows == 1 && P.mode == NS_GEMV_GATE_UP_SILU) continue;  // the gate/up epilogue needs both rows in one warp
-    if (env_rows && rows != env_rows && !(env_rows == 1 && P.mode == NS_GEMV_GATE_UP_SILU)) continue;
-    const int stage_bytes = rows * P.pitch;
-    for (int i = 0; i < 2; ++i) {
-      if (wide && i == 0) continue;  // the 14-consumer-warp kernel owns the SM
-      const int kc = (wide && i == 1) ? 2 * kConsumers : kConsumers;
-      int raw = 0;
-      if (budgets[i] > act_region + 64) raw = (int)((budgets[i] - act_region - 64) / (stage_bytes + 16));
-      if (raw > (wide ? 56 : 32)) raw = wide ? 56 : 32;
-      const int ac = raw < kc ? raw : kc;
-      if (ac < 1) continue;
-      const int st = raw - raw % ac;  // one consumer warp per stage residue class (see kernel)
-      const int ctas = i == 0 ? 2 : 1;
-      const double score = ctas * ac * (rows == 2 ? 1.1 : 1.0) + 0.001 * st;
-      if (score > best.score) best = RingPlan{rows, st, ac, ctas, budgets[i], score};
-    }
-  }
-  return best;
 }
 
 template <int AMODE, int M, bool ASYM, int STYPE, int ROWS, bool NORM, int NC = kConsumers>

@@ -10,11 +10,10 @@
 namespace {
 
 template <int AMODE, bool ASYM, int STYPE>
-int wide_launch(const GemvParams& P, size_t act_region, int act_row, int red_off, cudaStream_t st, bool* taken) {
-  const RingPlan wp = plan_ring(P, act_region, true);
-  // two producer warps on alternate stages need an even ring; a ring too short for two consumer warps is not worth the SM
-  if (!(wp.stages >= 2 && wp.stages % 2 == 0 && wp.active >= 2)) return NS_OK;
-  *taken = true;
+int wide_launch(const GemvParams& P, const RingChoice& c, cudaStream_t st) {
+  const RingPlan& wp = c.plan;
+  const size_t act_region = c.act_region;
+  const int act_row = c.act_row, red_off = c.red_off;
   if (P.norm_w && !P.act_f32) {
     ns_set_error("gemv_ring: fused RMSNorm needs fp32 activations");
     return NS_E_INVALID;
@@ -29,20 +28,18 @@ int wide_launch(const GemvParams& P, size_t act_region, int act_row, int red_off
 }
 
 template <int AMODE, bool ASYM>
-int wide_s(const GemvParams& P, size_t act_region, int act_row, int red_off, cudaStream_t st, bool* taken) {
+int wide_s(const GemvParams& P, const RingChoice& c, cudaStream_t st) {
   switch (P.stype) {
-    case NS_S_F32: return wide_launch<AMODE, ASYM, NS_S_F32>(P, act_region, act_row, red_off, st, taken);
-    case NS_S_F16: return wide_launch<AMODE, ASYM, NS_S_F16>(P, act_region, act_row, red_off, st, taken);
-    default: return wide_launch<AMODE, ASYM, NS_S_BF16>(P, act_region, act_row, red_off, st, taken);
+    case NS_S_F32: return wide_launch<AMODE, ASYM, NS_S_F32>(P, c, st);
+    case NS_S_F16: return wide_launch<AMODE, ASYM, NS_S_F16>(P, c, st);
+    default: return wide_launch<AMODE, ASYM, NS_S_BF16>(P, c, st);
   }
 }
 
 }  // namespace
 
-// *taken = false: no plan for this shape on the wide kernel, the caller launches the two-CTA kernel
-int ns_launch_gemv_ring_wide(const GemvParams& P, int amode, bool asym, size_t act_region, int act_row, int red_off, cudaStream_t st,
-                             bool* taken) {
-  *taken = false;
-  if (amode == A_U8) return asym ? wide_s<A_U8, true>(P, act_region, act_row, red_off, st, taken) : wide_s<A_U8, false>(P, act_region, act_row, red_off, st, taken);
-  return asym ? wide_s<A_S8, true>(P, act_region, act_row, red_off, st, taken) : wide_s<A_S8, false>(P, act_region, act_row, red_off, st, taken);
+// c: a wide choice of ns_gemv_ring_choose
+int ns_launch_gemv_ring_wide(const GemvParams& P, int amode, bool asym, const RingChoice& c, cudaStream_t st) {
+  if (amode == A_U8) return asym ? wide_s<A_U8, true>(P, c, st) : wide_s<A_U8, false>(P, c, st);
+  return asym ? wide_s<A_S8, true>(P, c, st) : wide_s<A_S8, false>(P, c, st);
 }

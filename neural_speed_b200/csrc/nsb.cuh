@@ -101,6 +101,7 @@ int ns_launch_mul_mat_q6k(const ns_weight* w, const float* act, int lda, float* 
 // w: {w} (plain), {wq, wk, wv} (QKV concat) or {w1, w3, w2} (FFN gate, up (NULL: two-weight FFN), down); flags: NS_MM_*
 enum { NS_PATH_GEMV, NS_PATH_IMMA, NS_PATH_TC, NS_PATH_Q6K };
 enum { NS_NODE_PLAIN, NS_NODE_QKV, NS_NODE_FFN };
+enum { NS_ROUTE_NORM = 1 << 16 };  // flags bit of ns_route: an RMSNorm folds into the node's first launch (it takes shared memory)
 int ns_route(int kind, const ns_weight* const* w, int m, int flags);
 // abi.cu: fused FFN with the residual add folded into the down projection (used by the decode engine, llama.cu)
 int ns_ffn_silu_residual(const ns_weight* w1, const ns_weight* w2, const ns_weight* w3, const float* act, int lda, float* tmp,
@@ -169,9 +170,29 @@ struct GemvParams {
   int one_image;  // decode engine: run this node on the norm-capable kernel image even without a norm, so that ALL the GEMV nodes of
                   // a token share ONE code image (two alternating images cost ~70 us per token in instruction fetch, measured: 736 -> 776 tok/s)
 };
-int ns_launch_gemv_ring(const GemvParams& P, int amode, bool asym, int mt, cudaStream_t st);  // gemv_ring.cu
-int ns_launch_gemv_ring_wide(const GemvParams& P, int amode, bool asym, size_t act_region, int act_row, int red_off, cudaStream_t st,
-                             bool* taken);  // gemv_ring_wide.cu
+// How one ring GEMV launch runs: which kernel shape, how its shared memory is split.  ns_gemv_ring_choose is the only place
+// that decides it; the launchers run what it returns and ns_route refuses a node when any of its launches has no plan.
+struct RingPlan {
+  int rows;    // weight rows per ring stage: 2 (a row pair) or 1
+  int stages;  // ring depth, a multiple of `active`
+  int active;  // consumer warps that own ring stages
+  int ctas;    // CTAs per SM: 2 (two-CTA kernel, 7 consumer warps each) or 1
+  size_t budget;
+  double score;
+};
+struct RingChoice {
+  bool wide;          // the one-CTA-per-SM kernel with 14 consumer warps (else the two-CTA kernel, 7 consumer warps)
+  RingPlan plan;
+  size_t act_region;  // bytes of shared memory ahead of the ring: activation image, meta, RMSNorm scratch
+  int act_row, red_off;
+};
+// kpad / pitch: the weight's; mt: the kernel template's activation rows (1, 2 or 4); fused: the kernel quantises fp32 activations
+// itself (else it copies a prepared image); norm: a fused RMSNorm.  false: no shared-memory plan fits.
+bool ns_gemv_ring_choose(int kpad, int pitch, int mode, int mt, bool fused, bool norm, RingChoice* c);  // gemv_ring.cu
+int ns_launch_gemv_ring(const GemvParams& P, int amode, bool asym, int mt, cudaStream_t st);                       // gemv_ring.cu
+int ns_launch_gemv_ring_wide(const GemvParams& P, int amode, bool asym, const RingChoice& c, cudaStream_t st);  // gemv_ring_wide.cu
+// NS_OK when every GEMV tile of an m-row launch of these weights has a kernel plan, else NS_E_UNSUPPORTED naming the ring (gemv.cu)
+int ns_gemv_planned(const ns_weight* const* ws, int nw, int mode, int m, bool norm);
 
 template <typename... Args>
 static inline cudaError_t ns_launch_pdl(void (*kern)(Args...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,

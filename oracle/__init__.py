@@ -542,6 +542,109 @@ def imma_bound_ratio(got, tot, mag, nb, splits=16):
     return float((err / np.maximum(gam * mag, np.finfo(np.float64).tiny)).max())
 
 
+_F32_NORMAL = 2.0 ** -126
+
+
+def _assert_normal(*arrs):
+    for a in arrs:
+        a = np.abs(np.asarray(a, np.float64))
+        assert np.isfinite(a).all() and not ((a > 0) & (a < _F32_NORMAL)).any(), "subnormal or non-finite fp32 value"
+
+
+def fma32(x, y, z):
+    """fmaf(x, y, z) for arrays: the exact x * y + z rounded once to fp32 (nearest, ties to even).  x: fp32 values or integers
+    below 2^29, y and z fp32, so x * y is exact in fp64; the fp64 sum is split into s + e exactly (TwoSum), and s rounds to the
+    right fp32 unless it is an fp32 midpoint, where the sign of e decides.  Operands and results must be normal fp32 (asserted)."""
+    x = np.asarray(x)
+    if np.issubdtype(x.dtype, np.integer):
+        assert np.abs(x).max(initial=0) < 2 ** 29
+    else:
+        assert x.dtype == np.float32, x.dtype
+    y, z = np.asarray(y, np.float32), np.asarray(z, np.float32)
+    _assert_normal(x, y, z)
+    p, zd = x.astype(np.float64) * y.astype(np.float64), z.astype(np.float64)
+    s = p + zd
+    bb = s - zd
+    e = (zd - (s - bb)) + (p - bb)  # s + e == p + z exactly
+    r = s.astype(np.float32)
+    d = s - r.astype(np.float64)   # exact
+    nb = np.nextafter(r, np.where(d > 0, np.float32(np.inf), np.float32(-np.inf)))
+    mid = (d != 0) & (2 * d == nb.astype(np.float64) - r.astype(np.float64))
+    out = np.where(mid & (np.sign(e) == np.sign(d)), nb, r)
+    _assert_normal(out)
+    return out
+
+
+def warp_butterfly(v):
+    """lane 0 of warp_sum (nsb.cuh): v [32, ...] fp32 per lane, v_L += v_{L xor o} for o = 16, 8, 4, 2, 1, in fp32"""
+    v = np.asarray(v, np.float32)
+    assert v.shape[0] == 32
+    lanes = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        v = v + v[lanes ^ o]
+    return v[0]
+
+
+def ring_stated(a_codes, a_scale, ab, q, w_scale, w_zp, g, lanes=False):
+    """The ring GEMV's exact fp32 result before its epilogue (gemv_ring_kernel, DESIGN.md section 4).  a_codes / a_scale / ab as
+    imma_act (codes minus zero point [M, K], one scale per activation block of ab); q int [K, N] signed weight codes, w_scale
+    [ceil(K/g), N] as stored, w_zp the same shape or None.  Per 32-element chunk c: isum_c = sum (a - za)(q - zp), an exact
+    integer (the chunk's elements past K are zero), t_c = fp32(a_scale_c * w_scale_gi), gi = c // ceil(g / 32).  Lane L runs
+    acc = fmaf(isum_c, t_c, acc) over c = L, L + 32, ... from +0; lane 0 of the xor butterfly is the output.
+    Returns fp32 [M, N] (and with lanes=True the per-lane accumulators [32, M, N] too)."""
+    a = np.asarray(a_codes, np.int64)
+    m, k = a.shape
+    w = np.asarray(q, np.int64)
+    n = w.shape[1]
+    cpg = -(-g // 32)
+    nch = -(-k // 32)
+    gi = np.arange(nch) // cpg
+    if w_zp is not None:
+        w = w - np.asarray(w_zp, np.int64)[gi].repeat(32, axis=0)[:k]
+    ap = np.zeros((m, nch * 32), np.float64)
+    ap[:, :k] = a
+    wp = np.zeros((nch * 32, n), np.float64)
+    wp[:k] = w
+    # integers below 2^17 per chunk: exact in fp64 whatever the summation order
+    isum = np.matmul(ap.reshape(m, nch, 32).transpose(1, 0, 2), wp.reshape(nch, 32, n))  # [nch, M, N]
+    assert np.abs(isum).max(initial=0) < 2 ** 17
+    asc = np.asarray(a_scale, np.float32)[:, (np.arange(nch) * 32) // ab]                 # [M, nch]
+    wsc = np.asarray(w_scale, np.float32)[gi]                                             # [nch, N]
+    t = asc.T[:, :, None] * wsc[:, None, :]                                                # fp32 products [nch, M, N]
+    nst = -(-nch // 32)
+    acc = np.zeros((32, m, n), np.float32)
+    for j in range(nst):
+        c0, c1 = 32 * j, min(32 * j + 32, nch)
+        live = c1 - c0
+        acc[:live] = fma32(isum[c0:c1].astype(np.int64), t[c0:c1], acc[:live])
+    out = warp_butterfly(acc)
+    return (out, acc) if lanes else out
+
+
+def ring_norm_row(x, w, eps, nt):
+    """The fp32 row the ring GEMV's fused RMSNorm prologue hands to its quantiser (quantise_to_smem, csrc/gemv_ring_impl.cuh) for a
+    CTA of nt consumer threads (224: the two-CTA kernel, 448: the wide one).  Thread i owns the 8-groups i, i + nt, ... and runs
+    ss = fmaf(v, v, ss) over them in that order (single-pass and multi-pass rows visit them alike); each warp's lane 0 of the
+    xor butterfly, summed in warp order from 0; inv = 1 / sqrtf(tot / k + eps); row = (x * inv) * w, all fp32."""
+    x = np.asarray(x, np.float32).ravel()
+    wn = np.asarray(w, np.float32).ravel()
+    k = x.size
+    ng8 = -(-k // 32) * 4
+    npass = -(-ng8 // nt)
+    v = np.zeros(npass * nt * 8, np.float32)
+    v[:k] = x
+    v = v.reshape(npass, nt, 8)
+    ss = np.zeros(nt, np.float32)
+    for j in range(npass):
+        for i in range(8):
+            ss = fma32(v[j, :, i], v[j, :, i], ss)
+    tot = np.float32(0)
+    for wp in range(nt // 32):
+        tot = np.float32(tot + warp_butterfly(ss[32 * wp:32 * wp + 32]))
+    inv = np.float32(1) / np.sqrt(np.float32(tot / np.float32(k)) + np.float32(eps))
+    return (x * np.float32(inv)) * wn
+
+
 def f32_to_bf16_bits(x):
     """RNE fp32 -> bf16 bit pattern (bestla_utils.h:146-153), vectorised."""
     u = _c(x, np.float32).view(np.uint32).astype(np.uint64)
