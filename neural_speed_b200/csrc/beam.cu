@@ -2,17 +2,17 @@
 // restatement, the KV block copy, and the flow itself in host C++ over an engine (the device one is in llama.cu, a host one with a
 // caller's logits here).
 //
-// beam_candidates_kernel: grid (kBeamSlices, rows), kBeamThreads threads, in the style of logprob_kernel.  Each CTA takes its
-// slice's max and sum of exp(x - max) exactly as logprob_kernel does, radix-selects the slice's top K keys (masked logit
-// descending, id ascending: ns_sample_key) into global scratch, and takes a ticket; the row's last CTA merges the slices' max and
-// sums in slice order, radix-selects the row's top K over the partials, sorts them and writes {id, score}.  beam.h states the
-// arithmetic.
+// beam_candidates_kernel: grid (kVocabSlices, rows), kLogprobThreads threads, on the slice reductions of vocab_slices.cuh.  Each
+// CTA takes its slice's max and sum of exp(x - max) as logprob_kernel does (slice_argmax, slice_expsum) and its top K keys of the
+// masked logits (masked logit descending, id ascending: ns_sample_key; slice_top_keys); the row's last CTA merges the slices' max
+// and sums in slice order, takes the row's top K over the partials, sorted (row_top_keys), and writes {id, score}.  beam.h states
+// the arithmetic.
 //
 // kv_copy_kernel: grid (chunks, layer x KV head x {K, V}, pairs); a (layer, head) range of positions is contiguous in the
 // [layer][seq][kv head][n_ctx][hd] fp16 cache, copied in 16-byte vectors.
 #include "nsb.cuh"
 #include "beam.h"
-#include "select.cuh"
+#include "vocab_slices.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -21,132 +21,46 @@
 
 namespace {
 
-__global__ void __launch_bounds__(kBeamThreads) beam_candidates_kernel(const BeamLaunch a) {
+__global__ void __launch_bounds__(kLogprobThreads) beam_candidates_kernel(const BeamLaunch a) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ unsigned hist[256];
-  __shared__ uint64_t s_prefix;
-  __shared__ int s_rem, s_cnt, s_off[kBeamSlices + 1];
-  __shared__ float sv[kBeamThreads / 32];
-  __shared__ float s_max;
-  __shared__ bool last;
+  __shared__ float s_max, s_norm;
   __shared__ uint64_t sk[kBeamMaxK];
-  const int row = blockIdx.y, sl = blockIdx.x, tid = threadIdx.x;
-  const int n = a.n_vocab, per = (n + kBeamSlices - 1) / kBeamSlices;
-  const int lo = min(n, sl * per), hi = min(n, lo + per), len = hi - lo;
+  const int row = blockIdx.y, tid = threadIdx.x, n = a.n_vocab, slot = row * kVocabSlices + blockIdx.x;
+  const VocabSlice sl = vocab_slice(n, blockIdx.x);
   const float* x = a.logits + (size_t)row * n;
   const int mask = (a.mask >> row) & 1, K = min(a.k, n);
-  // the slice's max and sum of the raw logits (logprob_kernel's passes 1 and 2)
-  float best = -INFINITY;
-  for (int i = lo + tid; i < hi; i += kBeamThreads) best = x[i] > best ? x[i] : best;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float v = __shfl_xor_sync(0xffffffffu, best, o);
-    best = v > best ? v : best;
-  }
-  if ((tid & 31) == 0) sv[tid >> 5] = best;
-  __syncthreads();
+  // the slice's max and sum of the raw logits (logprob_kernel's)
+  float best;
+  int bi;
+  slice_argmax<kLogprobThreads>(x, sl.lo, sl.hi, best, bi);
+  const float sum = slice_expsum<kLogprobThreads>(x, sl.lo, sl.hi, best);
   if (tid == 0) {
-    for (int w = 1; w < kBeamThreads / 32; ++w) best = sv[w] > best ? sv[w] : best;
-    s_max = best;
-    s_cnt = 0;
+    a.pmax[slot] = best;
+    a.psum[slot] = sum;
   }
-  __syncthreads();
-  const float m = s_max;
-  float acc = 0.f;
-  for (int i = lo + tid; i < hi; i += kBeamThreads) acc = __fadd_rn(acc, ns_logprob_term(x[i], m));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc = __fadd_rn(acc, __shfl_xor_sync(0xffffffffu, acc, o));
-  __syncthreads();  // sv is reused
-  if ((tid & 31) == 0) sv[tid >> 5] = acc;
-  __syncthreads();
-  const int slot = row * kBeamSlices + sl;
-  if (tid == 0) {
-    for (int w = 1; w < kBeamThreads / 32; ++w) acc = __fadd_rn(acc, sv[w]);
-    a.pmax[slot] = m;
-    a.psum[slot] = acc;
-  }
-  // the slice's top min(K, len) keys of the masked logits
-  auto key_at = [&](int i) { return ns_sample_key(ns_beam_masked(x[i], i, a.eos, mask), i); };
-  const int kk = min(K, len);
-  uint64_t thr = 0;
-  if (kk < len)
-    thr = radix_kth([&](auto fn) { for (int i = lo + tid; i < hi; i += kBeamThreads) fn(key_at(i)); }, kk, hist, &s_prefix, &s_rem);
-  unsigned long long* pk = a.pkeys + (size_t)slot * a.k;
-  for (int i = lo + tid; i < hi; i += kBeamThreads) {
-    const uint64_t key = key_at(i);
-    if (key >= thr) {
-      const int pos = atomicAdd(&s_cnt, 1);
-      if (pos < kk) pk[pos] = key;
-    }
-  }
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) {
-    a.pcnt[slot] = max(kk, 0);
-    __threadfence();
-    last = atomicAdd(&a.tickets[row], 1u) == kBeamSlices - 1;
-  }
-  __syncthreads();
-  if (!last) return;
-  __threadfence();
+  // the slice's top keys of the masked logits
+  slice_top_keys<kLogprobThreads>(
+      [&](int j) {
+        const int i = sl.lo + j;
+        return ns_sample_key(ns_beam_masked(x[i], i, a.eos, mask), i);
+      },
+      sl.hi - sl.lo, K, a.pkeys + (size_t)slot * a.k, a.pcnt + slot);
+  if (!last_of_row(a.tickets, row)) return;
 
   // ---- the row's last CTA: M, S in slice order; the top K of the partials, sorted ----
+  row_top_keys<kLogprobThreads>(a.pkeys + (size_t)row * kVocabSlices * a.k, a.pcnt + row * kVocabSlices, a.k, K, sk);
   if (tid == 0) {
-    int t = 0;
-    for (int s = 0; s < kBeamSlices; ++s) {
-      s_off[s] = t;
-      t += ((volatile int*)a.pcnt)[row * kBeamSlices + s];
-    }
-    s_off[kBeamSlices] = t;
-    s_cnt = 0;
-  }
-  for (int i = tid; i < kBeamMaxK; i += kBeamThreads) sk[i] = 0;
-  __syncthreads();
-  const volatile unsigned long long* rk = a.pkeys + (size_t)row * kBeamSlices * a.k;
-  auto each_part = [&](auto fn) {
-    for (int s = 0; s < kBeamSlices; ++s) {
-      const int c = s_off[s + 1] - s_off[s];
-      for (int j = tid; j < c; j += kBeamThreads) fn((uint64_t)rk[(size_t)s * a.k + j]);
-    }
-  };
-  thr = s_off[kBeamSlices] > K ? radix_kth(each_part, K, hist, &s_prefix, &s_rem) : 0;
-  each_part([&](uint64_t key) {
-    if (key >= thr) {
-      const int pos = atomicAdd(&s_cnt, 1);
-      if (pos < K) sk[pos] = key;
-    }
-  });
-  __syncthreads();
-  int P = 1;
-  while (P < K) P <<= 1;
-  for (int size = 2; size <= P; size <<= 1)  // bitonic sort, descending
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int t = tid; t < P / 2; t += kBeamThreads) {
-        const int i = (t / stride) * stride * 2 + t % stride, j = i + stride;
-        const bool desc = (i & size) == 0;
-        const uint64_t u = sk[i], v = sk[j];
-        if ((u < v) == desc) {
-          sk[i] = v;
-          sk[j] = u;
-        }
-      }
-      __syncthreads();
-    }
-  if (tid == 0) {
-    const volatile float* pm = a.pmax + row * kBeamSlices;
-    const volatile float* ps = a.psum + row * kBeamSlices;
+    const volatile float* pm = a.pmax + row * kVocabSlices;
     float M = -INFINITY;
-    for (int s = 0; s < kBeamSlices; ++s) M = pm[s] > M ? pm[s] : M;
-    float S = 0.f;
-    for (int s = 0; s < kBeamSlices; ++s) S = __fadd_rn(S, ns_logprob_merge_term(ps[s], pm[s], M));
+    for (int s = 0; s < kVocabSlices; ++s) M = pm[s] > M ? pm[s] : M;
     s_max = M;
-    sv[0] = __fdiv_rn(1.f, S);
+    s_norm = __fdiv_rn(1.f, merge_slice_sums((const volatile float*)a.psum + row * kVocabSlices, pm, M));
     a.tickets[row] = 0u;  // ready for the next launch
   }
   __syncthreads();
-  const float M = s_max, norm = sv[0], prev = a.prev[row];
-  for (int i = tid; i < K; i += kBeamThreads) {
+  const float M = s_max, norm = s_norm, prev = a.prev[row];
+  for (int i = tid; i < K; i += kLogprobThreads) {
     BeamCand c;
     c.id = ns_sample_key_id(sk[i]);
     c.score = ns_beam_score(ns_sample_key_value(sk[i]), M, norm, prev);
@@ -170,20 +84,20 @@ __global__ void __launch_bounds__(256) kv_copy_kernel(const KvCopyPairs a, __hal
 }  // namespace
 
 size_t ns_beam_scratch_bytes(int rows, int k) {
-  return (size_t)rows * kBeamSlices * 12 + (size_t)rows * kBeamSlices * k * 8;
+  return (size_t)rows * kVocabSlices * 12 + (size_t)rows * kVocabSlices * k * 8;
 }
 
 void ns_beam_scratch(BeamLaunch& a, void* scratch, int rows, int k) {
   char* w = static_cast<char*>(scratch);
   a.pkeys = reinterpret_cast<unsigned long long*>(w);  // 8-byte aligned first
-  w += (size_t)rows * kBeamSlices * k * 8;
+  w += (size_t)rows * kVocabSlices * k * 8;
   a.pmax = reinterpret_cast<float*>(w);
-  a.psum = a.pmax + (size_t)rows * kBeamSlices;
-  a.pcnt = reinterpret_cast<int*>(a.psum + (size_t)rows * kBeamSlices);
+  a.psum = a.pmax + (size_t)rows * kVocabSlices;
+  a.pcnt = reinterpret_cast<int*>(a.psum + (size_t)rows * kVocabSlices);
 }
 
 int ns_launch_beam_candidates(const BeamLaunch& a, cudaStream_t st) {
-  NS_CUDA_TRY(ns_launch_pdl(beam_candidates_kernel, dim3((unsigned)kBeamSlices, (unsigned)a.rows), dim3(kBeamThreads), 0, st, a));
+  NS_CUDA_TRY(ns_launch_pdl(beam_candidates_kernel, dim3((unsigned)kVocabSlices, (unsigned)a.rows), dim3(kLogprobThreads), 0, st, a));
   ns_count_launch();
   return NS_OK;
 }
@@ -219,42 +133,10 @@ int ns_launch_kv_copy(const KvCopyPairs& a, __half* kc, __half* vc, int n_layer,
 }
 
 // ---- host restatement ------------------------------------------------------------------------------------------------------
-// M and S of one row in logprob.h's order: thread j of a slice adds its entries in ascending order, warps combine by xor butterfly,
-// warps in order, slices in order
-static void row_stats_host(const float* x, int n, float* M_out, float* S_out) {
-  const int per = (n + kBeamSlices - 1) / kBeamSlices;
-  float m[kBeamSlices], S_s[kBeamSlices];
-  float M = -INFINITY;
-  for (int s = 0; s < kBeamSlices; ++s) {
-    const int lo = std::min(n, s * per), hi = std::min(n, lo + per);
-    m[s] = -INFINITY;
-    for (int i = lo; i < hi; ++i) m[s] = x[i] > m[s] ? x[i] : m[s];
-    float lane[kBeamThreads];
-    for (int j = 0; j < kBeamThreads; ++j) {
-      lane[j] = 0.f;
-      for (int i = lo + j; i < hi; i += kBeamThreads) lane[j] = NS_FADD(lane[j], ns_logprob_term(x[i], m[s]));
-    }
-    for (int w = 0; w < kBeamThreads / 32; ++w) {
-      float* v = lane + 32 * w;
-      for (int o = 16; o > 0; o >>= 1) {
-        float t[32];
-        for (int L = 0; L < 32; ++L) t[L] = NS_FADD(v[L], v[L ^ o]);
-        for (int L = 0; L < 32; ++L) v[L] = t[L];
-      }
-    }
-    S_s[s] = lane[0];
-    for (int w = 1; w < kBeamThreads / 32; ++w) S_s[s] = NS_FADD(S_s[s], lane[32 * w]);
-    M = m[s] > M ? m[s] : M;
-  }
-  float S = 0.f;
-  for (int s = 0; s < kBeamSlices; ++s) S = NS_FADD(S, ns_logprob_merge_term(S_s[s], m[s], M));
-  *M_out = M;
-  *S_out = S;
-}
-
 static void candidates_row_host(const float* x, int n, int k, float prev, int mask, int eos, BeamCand* out) {
   float M, S;
-  row_stats_host(x, n, &M, &S);
+  int I;
+  ns_logprob_stats_host(x, n, &M, &I, &S);
   const float norm = NS_FDIV(1.f, S);
   const int K = std::min(k, n);
   std::vector<uint64_t> key(n);

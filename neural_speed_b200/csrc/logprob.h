@@ -3,13 +3,13 @@
 // so ns_logprob_row_host and logprob_kernel (logprob.cu) run the same operations in the same order.
 //
 // One row x[0 .. n) with a target t:
-//   slices     s = 0 .. kLogprobSlices - 1 cover [s per, min(n, (s + 1) per)), per = ceil(n / kLogprobSlices)
+//   slices     s = 0 .. kVocabSlices - 1, the slices of vocab_slices.cuh (vocab_slice)
 //   max        m_s, i_s = the largest value of slice s and its lowest id (NaN never wins; -inf, id i_s, when it holds no
 //              number above -inf; an empty slice or one of NaN only gives -inf and no id); M, I the same over the slices in
 //              order; I = 0 when no slice has an id (argmax_kernel's rule, model_utils.cpp:2963-2985)
 //   sum        S_s = sum of ns_logprob_term(x_i, m_s) over slice s: thread j of kLogprobThreads adds x_{lo + j}, x_{lo + j + 256},
 //              ... in ascending order into 0, the 32 lanes of a warp then combine by xor butterfly (v_L += v_{L ^ o}, o = 16, 8,
-//              4, 2, 1), and the 8 warps' values are added in warp order;
+//              4, 2, 1), and the 8 warps' values are added in warp order (slice_expsum);
 //              S = sum over s = 0 .. 31 in order of ns_logprob_merge_term(S_s, m_s, M)
 //   logprob    (x_t - M) - ns_logf(S)
 // Every term is exp(x - m) <= 1 with one term equal to 1 in the slice (or row) of the max, so S_s and S lie in [1, n] whenever
@@ -20,8 +20,7 @@
 #pragma once
 #include "sample.h"
 
-constexpr int kLogprobSlices = 32;    // CTAs per row
-constexpr int kLogprobThreads = 256;  // threads per CTA
+constexpr int kLogprobThreads = 256;  // threads per CTA, which fixes the order of S_s
 constexpr int kLogprobMaxRows = 32;   // rows of one launch (the eval step's lm_head chunk)
 
 // log(x) in IEEE fp32 operations (fdlibm's e_logf.c scheme): x = 2^k (1 + f) with 1 + f in [sqrt(2)/2, sqrt(2)), s = f / (2 + f),
@@ -80,19 +79,29 @@ NS_HD void ns_logprob_argmax_merge(float& best, int& bi, float v, int i) {
 }
 NS_HD float ns_logprob_final(float xt, float M, float S) { return NS_FSUB(NS_FSUB(xt, M), ns_logf(S)); }
 
+// the host restatement (logprob.cu) of one row's M, I and S
+void ns_logprob_stats_host(const float* x, int n, float* M, int* I, float* S);
+
 #ifdef __CUDACC__
-// ---- the device kernel (logprob.cu): grid (kLogprobSlices, rows), one launch per lm_head chunk -------------------------------
+// ---- the device kernels (logprob.cu), grid (kVocabSlices, rows) -------------------------------------------------------------
+// logprob_kernel: one launch per lm_head chunk
 struct LogprobLaunch {
   const float* logits;  // [rows][n_vocab]
   int n_vocab, rows;    // 1 <= rows <= kLogprobMaxRows
   const int* targets;   // [rows], nullable (then no sums and no log-probs)
   float* logprobs;      // [rows], non-null with targets
   int* argmax;          // [rows], nullable
-  // scratch: per-slice max / id / sum [rows][kLogprobSlices], tickets [rows] (zero, and zero again after the launch)
+  // scratch: per-slice max / id / sum [rows][kVocabSlices], tickets [rows] (zero, and zero again after the launch)
   float* pmax;
   int* pidx;
   float* psum;
   unsigned* tickets;
 };
 int ns_launch_logprob(const LogprobLaunch& a, cudaStream_t st);  // counts its launch
+// argmax_kernel: the eval step's greedy pick, I of each row, with state[3] = I and, when `advance`, state[0] = I,
+// state[1] += n_tokens, record[state[2]++] = I.  rowwise: row r uses state + 4 r and record + r rec_stride (a pass over several
+// sequences); otherwise the single row uses state and record.  Scratch: max / id [rows][kVocabSlices], tickets [rows] (zero, and
+// zero again after the launch).  Counts its launch.
+int ns_launch_argmax(const float* logits, int n_vocab, int rows, bool rowwise, int* state, int n_tokens, int advance, int* record,
+                     int rec_stride, float* pmax, int* pidx, unsigned* tickets, cudaStream_t st);
 #endif

@@ -1,15 +1,15 @@
 // sample.cu -- the reference's sampler (model_post_sample_top_k_top_p_repeat, model_utils.cpp:2987-3032) on the device, in one
 // launch that takes the argmax's place in the eval step; its host restatement; and the parity entry ns_llama_sample.
 //
-// Grid (kSampleSlices, rows), 512 threads.  Each CTA loads one slice of its row's logits into shared memory, applies the
-// repetition penalty to the slice's ids found in the row's window (stored window + this pass's tokens, each id once), and
-// radix-selects the slice's top k keys (logit descending, id ascending: ns_sample_key) into global scratch.  The last CTA of a
-// row (ticket) radix-selects the row's top k over those partials in global memory, bitonic-sorts them in shared memory and runs
-// steps 5-7 in one thread (sample.h: every sum in the reference's order), then stores the row's window.  The last row to finish
-// (a second ticket) walks the rows in caller order, draws from the device-resident std::mt19937, and writes picks and state.
+// Grid (kVocabSlices, rows), 512 threads, on the slice reductions of vocab_slices.cuh.  Each CTA loads one slice of its row's
+// logits into shared memory, applies the repetition penalty to the slice's ids found in the row's window (stored window + this
+// pass's tokens, each id once), and selects the slice's top k keys (logit descending, id ascending: ns_sample_key) into global
+// scratch (slice_top_keys).  The last CTA of a row takes the row's top k over those partials, sorted (row_top_keys), runs steps
+// 5-7 in one thread (sample.h: every sum in the reference's order), then stores the row's window.  The last row to finish (a
+// second ticket) walks the rows in caller order, draws from the device-resident std::mt19937, and writes picks and state.
 #include "nsb.cuh"
 #include "sample.h"
-#include "select.cuh"
+#include "vocab_slices.cuh"
 
 #include <algorithm>
 #include <vector>
@@ -27,13 +27,10 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SampleLaun
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ __align__(16) unsigned char smem[];
-  __shared__ unsigned hist[256];
-  __shared__ uint64_t s_prefix;
-  __shared__ int s_rem, s_cnt, s_total, s_off[kSampleSlices + 1];
-  __shared__ bool last;
-  const int row = blockIdx.y, sl = blockIdx.x, tid = threadIdx.x;
-  const int n = a.n_vocab, per = (n + kSampleSlices - 1) / kSampleSlices;
-  const int lo = min(n, sl * per), hi = min(n, lo + per), len = hi - lo;
+  __shared__ int s_kept;
+  const int row = blockIdx.y, tid = threadIdx.x, n = a.n_vocab, slot = row * kVocabSlices + blockIdx.x;
+  const VocabSlice sl = vocab_slice(n, blockIdx.x);
+  const int lo = sl.lo, hi = sl.hi, len = hi - lo;
   const float* lg = a.logits + (size_t)row * n;
   const int* tp;
   int tl;
@@ -51,12 +48,11 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SampleLaun
 
   // ---- slice: load, penalise each window id of the slice once, select the slice's top min(K, len) ----
   float* vals = reinterpret_cast<float*>(smem);
-  unsigned char* flag = smem + (size_t)per * sizeof(float);
+  unsigned char* flag = smem + (size_t)vocab_slice_width(n) * sizeof(float);
   for (int i = tid; i < len; i += blockDim.x) {
     vals[i] = lg[lo + i];
     flag[i] = 0;
   }
-  if (tid == 0) s_cnt = 0;
   __syncthreads();
   if (pen) {
     for (int j = tid; j < W; j += blockDim.x) {
@@ -68,75 +64,13 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SampleLaun
       if (flag[i]) vals[i] = ns_sample_penalize(vals[i], a.penalty);
     __syncthreads();
   }
-  const int kk = min(K, len);
-  uint64_t thr = 0;
-  if (kk < len)
-    thr = radix_kth([&](auto fn) { for (int i = tid; i < len; i += blockDim.x) fn(ns_sample_key(vals[i], lo + i)); }, kk, hist, &s_prefix,
-                    &s_rem);
-  unsigned long long* pk = a.pkeys + ((size_t)row * kSampleSlices + sl) * a.k;
-  for (int i = tid; i < len; i += blockDim.x) {
-    const uint64_t key = ns_sample_key(vals[i], lo + i);
-    if (key >= thr) {
-      const int pos = atomicAdd(&s_cnt, 1);
-      if (pos < kk) pk[pos] = key;
-    }
-  }
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) {
-    a.pcnt[row * kSampleSlices + sl] = min(s_cnt, kk);
-    __threadfence();
-    last = atomicAdd(&a.tickets[row], 1u) == kSampleSlices - 1;
-  }
-  __syncthreads();
-  if (!last) return;
-  __threadfence();
+  slice_top_keys<kSampleThreads>([&](int i) { return ns_sample_key(vals[i], lo + i); }, len, K, a.pkeys + (size_t)slot * a.k,
+                                 a.pcnt + slot);
+  if (!last_of_row(a.tickets, row)) return;
 
-  // ---- the row's last CTA: top K of the partials, sorted ----
-  if (tid == 0) {
-    int t = 0;
-    for (int s = 0; s < kSampleSlices; ++s) {
-      s_off[s] = t;
-      t += ((volatile int*)a.pcnt)[row * kSampleSlices + s];
-    }
-    s_off[kSampleSlices] = t;
-    s_total = t;
-    s_cnt = 0;
-  }
-  __syncthreads();
-  const volatile unsigned long long* rk = a.pkeys + (size_t)row * kSampleSlices * a.k;
-  auto each_part = [&](auto fn) {
-    for (int s = 0; s < kSampleSlices; ++s) {
-      const int c = s_off[s + 1] - s_off[s];
-      for (int j = tid; j < c; j += blockDim.x) fn((uint64_t)rk[(size_t)s * a.k + j]);
-    }
-  };
-  thr = s_total > K ? radix_kth(each_part, K, hist, &s_prefix, &s_rem) : 0;
-  int P = 1;
-  while (P < K) P <<= 1;
-  uint64_t* sk = reinterpret_cast<uint64_t*>(smem);  // [P] (the slice's values are dead)
-  for (int i = tid; i < P; i += blockDim.x) sk[i] = 0;
-  __syncthreads();
-  each_part([&](uint64_t key) {
-    if (key >= thr) {
-      const int pos = atomicAdd(&s_cnt, 1);
-      if (pos < K) sk[pos] = key;
-    }
-  });
-  __syncthreads();
-  for (int size = 2; size <= P; size <<= 1)  // bitonic sort, descending
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int t = tid; t < P / 2; t += blockDim.x) {
-        const int i = (t / stride) * stride * 2 + t % stride, j = i + stride;
-        const bool desc = (i & size) == 0;
-        const uint64_t x = sk[i], y = sk[j];
-        if ((x < y) == desc) {
-          sk[i] = y;
-          sk[j] = x;
-        }
-      }
-      __syncthreads();
-    }
+  // ---- the row's last CTA: top K of the partials, sorted (the slice's values are dead) ----
+  uint64_t* sk = reinterpret_cast<uint64_t*>(smem);
+  const int P = row_top_keys<kSampleThreads>(a.pkeys + (size_t)row * kVocabSlices * a.k, a.pcnt + row * kVocabSlices, a.k, K, sk);
   float* l = reinterpret_cast<float*>(sk + P);  // [K]
   float* p = l + K;                             // [K]
   int* rid = a.ids + (size_t)row * a.k;
@@ -150,24 +84,20 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SampleLaun
     const int kept = ns_sample_tail(l, p, K, a.top_p, a.temp);
     ns_sample_cumulative(p, kept, a.cp + (size_t)row * a.k);
     a.kept[row] = kept;
-    s_cnt = kept;
+    s_kept = kept;
   }
   __syncthreads();
   float* rp = a.probs + (size_t)row * a.k;
-  for (int i = tid; i < K; i += blockDim.x) rp[i] = i < s_cnt ? p[i] : 0.f;
+  for (int i = tid; i < K; i += blockDim.x) rp[i] = i < s_kept ? p[i] : 0.f;
   // ---- the row's window: the last W of (stored ++ this pass's tokens) ----
   if (a.store && wv && tl > 0) {
     const int v = tid < W ? window_at(wv, tp, tl, W, tid) : 0;
     __syncthreads();
     if (tid < W) wv[tid] = v;
   }
-  __threadfence();  // ids, probs, the window: visible to the drawing CTA and the next launch
-  __syncthreads();
-  if (tid != 0) return;
-  a.tickets[row] = 0u;
-  __threadfence();
-  if (atomicAdd(&a.tickets[a.rows], 1u) != (unsigned)a.rows - 1) return;
-  __threadfence();
+  if (tid == 0) a.tickets[row] = 0u;
+  // ids, probs, the window: visible to the drawing CTA and the next launch
+  if (!last_of_row(a.tickets, a.rows, a.rows) || tid != 0) return;
   // ---- the last row: draws in caller order ----
   for (int i = 0; i < a.rows; ++i) {
     const int r = a.order ? a.order[i] : i;
@@ -193,7 +123,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SampleLaun
 }
 
 size_t sample_smem(int n_vocab, int k) {
-  const size_t per = (size_t)(n_vocab + kSampleSlices - 1) / kSampleSlices;
+  const size_t per = (size_t)vocab_slice_width(n_vocab);
   const int K = k < n_vocab ? k : n_vocab;
   size_t P = 1;
   while (P < (size_t)K) P <<= 1;
@@ -222,12 +152,12 @@ int ns_launch_sample(const SampleLaunch& a, cudaStream_t st) {
   const size_t smem = sample_smem(a.n_vocab, a.k);
   if (smem > 48 * 1024) {
     if (smem > 220 * 1024) {
-      ns_set_error("sampler: n_vocab %d too large (a slice of %d logits must fit in shared memory)", a.n_vocab, a.n_vocab / kSampleSlices);
+      ns_set_error("sampler: n_vocab %d too large (a slice of %d logits must fit in shared memory)", a.n_vocab, a.n_vocab / kVocabSlices);
       return NS_E_UNSUPPORTED;
     }
     NS_CUDA_TRY(cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
-  NS_CUDA_TRY(ns_launch_pdl(sample_kernel, dim3((unsigned)kSampleSlices, (unsigned)a.rows), dim3(kSampleThreads), smem, st, a));
+  NS_CUDA_TRY(ns_launch_pdl(sample_kernel, dim3((unsigned)kVocabSlices, (unsigned)a.rows), dim3(kSampleThreads), smem, st, a));
   ns_count_launch();
   return NS_OK;
 }
@@ -285,8 +215,8 @@ static size_t pad16(size_t b) { return (b + 15) / 16 * 16; }
 extern "C" size_t ns_llama_sample_workspace_bytes(int n, int top_k) {
   if (n < 1 || top_k < 1) return 0;
   const size_t k = (size_t)std::min(top_k, kSampleMaxK);
-  return pad16((size_t)(kSampleMaxRows + 1) * 4) + pad16((size_t)n * kSampleSlices * 4) + pad16((size_t)n * 4) + pad16((size_t)n * k * 8) +
-         pad16((size_t)n * k * 4) * 2 + (size_t)n * kSampleSlices * k * 8;
+  return pad16((size_t)(kSampleMaxRows + 1) * 4) + pad16((size_t)n * kVocabSlices * 4) + pad16((size_t)n * 4) + pad16((size_t)n * k * 8) +
+         pad16((size_t)n * k * 4) * 2 + (size_t)n * kVocabSlices * k * 8;
 }
 
 extern "C" int ns_llama_sample(const float* logits, int n, int n_vocab, const int32_t* windows, int n_window, const ns_llama_sampling* s,
@@ -305,7 +235,7 @@ extern "C" int ns_llama_sample(const float* logits, int n, int n_vocab, const in
   a.tickets = reinterpret_cast<unsigned*>(w);
   w += pad16((size_t)(kSampleMaxRows + 1) * 4);
   a.pcnt = reinterpret_cast<int*>(w);
-  w += pad16((size_t)n * kSampleSlices * 4);
+  w += pad16((size_t)n * kVocabSlices * 4);
   a.kept = reinterpret_cast<int*>(w);
   w += pad16((size_t)n * 4);
   a.cp = reinterpret_cast<double*>(w);

@@ -186,8 +186,7 @@ NS_HD int ns_sample_pick(const double* cp, int n, uint32_t* mt) {
 
 #ifdef __CUDACC__
 // ---- the device sampler (sample.cu), one launch in place of the eval step's argmax ------------------------------------------
-constexpr int kSampleSlices = 32;  // CTAs per row, each selecting the top k of one slice of the vocabulary
-struct SampleLaunch {
+struct SampleLaunch {  // grid (kVocabSlices, rows): each CTA selects the top k of one slice of the vocabulary
   const float* logits;  // [rows][n_vocab]
   int n_vocab, rows;
   int k;                // top_k, 1 .. kSampleMaxK
@@ -204,7 +203,7 @@ struct SampleLaunch {
   int store;            // write the windows back (0: a pass that will be evaluated again)
   int draw;             // draw from the generator (0: take the first entry and leave the generator alone)
   uint32_t* mt;         // [kMtWords]
-  // scratch: slice candidates [rows][kSampleSlices][k] and their counts, cumulative tables [rows][k], tickets [rows + 1] (zero)
+  // scratch: slice candidates [rows][kVocabSlices][k] and their counts, cumulative tables [rows][k], tickets [rows + 1] (zero)
   unsigned long long* pkeys;
   int* pcnt;
   double* cp;
