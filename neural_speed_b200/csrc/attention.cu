@@ -2,6 +2,7 @@
 // numerics), the plan of a pass over token segments, and the standalone ns_llama_attention* entries.
 #include <algorithm>
 
+#include "async_copy.cuh"
 #include "attention.cuh"
 
 namespace {
@@ -320,7 +321,6 @@ __global__ void __launch_bounds__(kAW * 32) attn_fast_kernel(const float* __rest
 // Everything after those offsets is the RING = false kernel's code, so each row's arithmetic is the single-sequence step's.
 constexpr int kSplitKeys = 256;
 constexpr int kDW = 16;  // warps per CTA
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 template <int HD>
 static constexpr size_t attn_decode_smem() {
   return (size_t)2 * kSplitKeys * HD * 2 + (size_t)(3 + kDW) * HD * 4 + (size_t)(kSplitKeys + 8) * 4 + 16;
@@ -380,23 +380,19 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   __half* kh = kc + (size_t)hk * n_ctx * HD;
   __half* vh = vc + (size_t)hk * n_ctx * HD;
-  const uint32_t bar_a = smem_addr(bar);
+  const uint32_t bar_a = smem_u32(bar);
   if (threadIdx.x == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar_a), "r"(1) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init(bar_a, 1);
+    fence_mbar_init();
     // the cached rows of this range were written by earlier tokens' launches: their copies start before the wait as well and
     // overlap the tail of the Q/K/V launch.  In the ring, the rows this token rewrites (shifted K, the new K / V slot) were
     // likewise last written by this layer's launch of the previous token -- the launch whose appended row the plain step
     // already reads here -- so the same ordering covers them.
     if (ncache > 0) {
       const uint32_t bytes = (uint32_t)ncache * HD * 2;
-      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(2 * bytes) : "memory");
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_addr(Kt)),
-                   "l"(kh + (size_t)i0 * HD), "r"(bytes), "r"(bar_a)
-                   : "memory");
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_addr(Vt)),
-                   "l"(vh + (size_t)i0 * HD), "r"(bytes), "r"(bar_a)
-                   : "memory");
+      mbar_expect_tx(bar_a, 2 * bytes);
+      bulk_g2s(smem_u32(Kt), kh + (size_t)i0 * HD, bytes, bar_a);
+      bulk_g2s(smem_u32(Vt), vh + (size_t)i0 * HD, bytes, bar_a);
     }
   }
   __syncthreads();
@@ -406,20 +402,6 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
     for (int j = 0; j < i; ++j) theta *= theta_scale;  // ne_layers.c:9385: same sequence of roundings
     theta *= freq_scale;
     sincosf(theta, sn, cs);
-  };
-  auto wait_tiles = [&]() {
-    uint32_t ok;
-    do {
-      asm volatile(
-          "{\n"
-          ".reg .pred p;\n"
-          "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-          "selp.u32 %0, 1, 0, p;\n"
-          "}\n"
-          : "=r"(ok)
-          : "r"(bar_a), "r"(0)
-          : "memory");
-    } while (!ok);
   };
   // RoPE of the new k row; KV append by one CTA per kv head -- while the copies fly
   float qsn = 0.f, qcs = 0.f;  // the queries' angle (thread i < HD / 2: pair i)
@@ -449,7 +431,7 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   }
   const int shift0 = wrapped ? min(max(n_keep - i0, 0), ncache) : ncache;  // staged rows [shift0, ncache) are shifted
   if (wrapped) {
-    wait_tiles();
+    mbar_wait(bar_a, 0);
     if (has_new && threadIdx.x < HD / 2) {  // the new row goes over its slot (write before shift: llama.cpp:408-409, :443)
       reinterpret_cast<__half2*>(Kt + (size_t)(slot - i0) * HD)[threadIdx.x] = knew_h;
       reinterpret_cast<__half2*>(Vt + (size_t)(slot - i0) * HD)[threadIdx.x] = vnew_h;
@@ -465,13 +447,11 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
       // form rounds once per output, as every contraction of the reference's expressions does
       kt2[e] = __floats2half2_rn(fmaf(x.x, t.x, -(x.y * t.y)), fmaf(x.y, t.x, x.x * t.y));
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the shifted rows, visible to the bulk store
+    fence_proxy_async();  // the shifted rows, visible to the bulk store
     __syncthreads();
     if (threadIdx.x == 0 && shift0 < ncache) {
-      asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(kh + (size_t)(i0 + shift0) * HD),
-                   "r"(smem_addr(Kt + (size_t)shift0 * HD)), "r"((uint32_t)(ncache - shift0) * HD * 2)
-                   : "memory");
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      bulk_s2g(kh + (size_t)(i0 + shift0) * HD, smem_u32(Kt + (size_t)shift0 * HD), (uint32_t)(ncache - shift0) * HD * 2);
+      bulk_commit();
     }
   }
   for (int hi = 0; hi < nh; ++hi) {
@@ -488,7 +468,7 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   float ql[EPL];
 #pragma unroll
   for (int e = 0; e < EPL; ++e) ql[e] = sq[lane * EPL + e];
-  if (ncache > 0) wait_tiles();
+  if (ncache > 0) mbar_wait(bar_a, 0);
   auto row = [&](const __half* base, int r, float* dst) {
     if (EPL == 4) {
       const uint2 u = *reinterpret_cast<const uint2*>(base + (size_t)r * HD + lane * 4);
@@ -609,7 +589,7 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   if (RING) __syncthreads();  // sq, sc, part and the reduction slots serve the next query head
   }
   // the bulk store reads the shifted rows out of shared memory: it must be complete before the CTA exits
-  if (wrapped && threadIdx.x == 0 && shift0 < ncache) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  if (wrapped && threadIdx.x == 0 && shift0 < ncache) bulk_wait_all();
 }
 
 // ---- prompt attention on the tensor cores ------------------------------------------------------------------------------------
@@ -784,7 +764,7 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
 #pragma unroll
       for (int n2 = 0; n2 < NT / 2; ++n2) {
         uint32_t b0, b1, b2, b3;
-        const uint32_t addr = (uint32_t)__cvta_generic_to_shared(vrow + n2 * 16);
+        const uint32_t addr = smem_u32(vrow + n2 * 16);
         asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(b0), "=r"(b1), "=r"(b2), "=r"(b3) : "r"(addr));
         mma_f16_16816(o[2 * n2], pa, b0, b1);
         mma_f16_16816(o[2 * n2 + 1], pa, b2, b3);

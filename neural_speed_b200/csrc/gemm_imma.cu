@@ -22,10 +22,9 @@
 // Scales and zero points of the CTA's rows / K range are staged once, before griddepcontrol.wait (weights are constant).
 // Split-K: partial tiles go to a workspace; the last CTA of a tile (ticket) sums them in split order -- deterministic --
 // and runs the epilogue (bias, GELU, residual, QKV layout, SiLU(gate) * up).
-#include <cuda.h>
-
 #include "nsb.cuh"
 #include "act_quant.cuh"
+#include "async_copy.cuh"
 
 namespace {
 
@@ -59,50 +58,6 @@ struct ImmaParams {
   int stages;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
-               "r"(bytes), "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void tma_2d(uint32_t dst, const CUtensorMap* map, int x, int y, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
-               "l"(map), "r"(x), "r"(y), "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ uint2 lds64(uint32_t a) {
-  uint2 r;
-  asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "r"(a));
-  return r;
-}
-__device__ __forceinline__ uint4 lds128(uint32_t a) {
-  uint4 r;
-  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(a));
-  return r;
-}
 __device__ __forceinline__ void ldmatrix_x4(uint32_t a, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(a));
 }
@@ -256,7 +211,7 @@ __global__ void __launch_bounds__(kThr, 2)
       mbar_init(full0 + 8 * s, 1);
       mbar_init(empty0 + 8 * s, kCons);
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbar_init();
   }
   __syncthreads();
 
@@ -511,21 +466,6 @@ __global__ void __launch_bounds__(kThr, 2)
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
 constexpr int kMaxPartialTiles = 640;  // tiles x ksplit when K is split
 constexpr int kMaxTiles = 16384;
 
@@ -675,11 +615,7 @@ int ns_launch_gemm_imma(const ns_weight* const* ws, int nw, int mode, const floa
     ns_set_error("gate/up fusion needs two weights with equal n");
     return NS_E_INVALID;
   }
-  EncodeTiledFn enc = get_encode();
-  if (!enc) {
-    ns_set_error("cuTensorMapEncodeTiled not available from the driver");
-    return NS_E_CUDA;
-  }
+  if (!ns_tensor_map_encoder()) return NS_E_CUDA;  // before anything launches
   const ns_weight* w0 = ws[0];
   Plan pl;
   if (!make_plan(ws, nw, mode, m, &pl)) {
@@ -713,16 +649,9 @@ int ns_launch_gemm_imma(const ns_weight* const* ws, int nw, int mode, const floa
   const bool gate_up = mode == NS_GEMV_GATE_UP_SILU;
   for (int i = 0; i < 3; ++i) {
     const ns_weight* w = ws[i < nw ? i : 0];
-    cuuint64_t dims[2] = {(cuuint64_t)w->q_bytes, (cuuint64_t)w->n};
-    cuuint64_t strides[1] = {(cuuint64_t)w->pitch};
-    cuuint32_t box[2] = {(cuuint32_t)(KS / 2), (cuuint32_t)(gate_up ? BN / 2 : BN)};
-    cuuint32_t es[2] = {1, 1};
-    CUresult r = enc(&maps[i], CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, (void*)w->rows, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      ns_set_error("cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
-      return NS_E_CUDA;
-    }
+    const int rc = ns_tensor_map_2d(&maps[i], CU_TENSOR_MAP_DATA_TYPE_UINT8, w->rows, w->q_bytes, w->n, w->pitch, KS / 2,
+                                    gate_up ? BN / 2 : BN, CU_TENSOR_MAP_SWIZZLE_128B, "weights");
+    if (rc != NS_OK) return rc;
   }
 
   ImmaParams P = {};

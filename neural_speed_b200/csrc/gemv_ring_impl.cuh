@@ -3,52 +3,13 @@
 // instantiations compile in parallel.  See gemv_ring.cu for the design notes.
 #pragma once
 #include "act_quant.cuh"
+#include "async_copy.cuh"
 
 namespace {
 
 constexpr int kConsumers = 7;
 constexpr int kThreads = (kConsumers + 1) * 32;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-// TMA 1-D bulk copy global -> shared, completion on an mbarrier (SASS: UBLKCP)
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
-               "r"(bytes), "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ uint4 lds128(uint32_t a) {
-  uint4 r;
-  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(a));
-  return r;
-}
-__device__ __forceinline__ uint2 lds64(uint32_t a) {
-  uint2 r;
-  asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "r"(a));
-  return r;
-}
 __device__ __forceinline__ uint32_t lds32(uint32_t a) {
   uint32_t r;
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(a));
@@ -325,7 +286,7 @@ __global__ void __launch_bounds__((NC + (NC > kConsumers ? 2 : 1)) * 32, NC > kC
       mbar_init(full0 + 8 * s, 1);
       mbar_init(empty0 + 8 * s, 1);
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbar_init();
   }
   __syncthreads();
 
@@ -387,8 +348,7 @@ __global__ void __launch_bounds__((NC + (NC > kConsumers ? 2 : 1)) * 32, NC > kC
   const int nchunks = P.kpad >> 5;
 
   // This warp visits units warp, warp+active, ... .  `stages` is a multiple of `active` (launcher), so stage s is only ever
-  // consumed by warp s % active: every mbarrier is waited on by ONE warp that observes all of its phases in order.
-  // (A parity wait issued a whole phase early returns true immediately -- waiters must never run ahead of a barrier.)
+  // consumed by warp s % active: every mbarrier is waited on by ONE warp that observes all of its phases in order (mbar_wait).
   int s = warp;
   uint32_t phase = 0;
 
