@@ -5,11 +5,11 @@ candidates scored on the device.
    .. 64, 1 .. 32 rows, ties, -inf entries and EOS-masked rows, a poisoned workspace whose tickets are zero again afterwards.
 2. ns_llama_kv_copy: the copied bytes equal their source and every other block and position is unchanged; a sequence forked by the
    copy decodes bit-identically to the original; pair lists that overlap are refused without a launch.
-3. Engine identity: on the toy models of tests/test_gpu_eval_all.py (Q4_0 and Q6_K lm_head), ns_llama_beam_search equals
+3. Engine identity: on the toy models of tests/llama_models.py (GQA 4 on 2, Q4_0 and Q6_K lm_head), ns_llama_beam_search equals
    oracle/beam_search.cpp with the library's row arithmetic, driven by a second engine's own eval_batch / decode_batch logits for
    the same running rows (its KV blocks kept by the same rule: a beam continues in its source's block or a copy of it), bit for bit
    in tokens and scores -- num_beams 2 / 4 / 8, 1-4 requests, passes of 2 and of 3 or more rows.
-4. (Not here: the oracle flow on the toy models' CPU-graph logits.  Their floor_of bar is 2.5e-2 of max |logit|, wider than the
+4. (Not here: the oracle flow on the toy models' CPU-graph logits.  Their running bar is 2.5e-2 of max |logit|, wider than the
    gap between a request's B-th and (B+1)-th candidate in nearly every search, so such a comparison would cover almost no step;
    DESIGN.md section 4 says so.)
 5. Llama-2-7B shapes (head size 128, vocab 32000): the first step's candidates against the reference engine's prompt logits
@@ -24,11 +24,8 @@ import pytest
 import torch
 
 import neural_speed_b200 as ns
-import oracle
-from oracle.llama_model import OracleLlama
+from llama_models import bar, bits, close, distance, llama2_7b_shaped, rows, scale, toy
 from test_beam_cpu import oracle_search, orc  # noqa: F401 -- the oracle fixture
-from test_gpu_eval_all import Toy
-from test_gpu_eval_all import _rows as _token_rows
 from torch.profiler import ProfilerActivity, profile
 
 pytestmark = pytest.mark.gpu
@@ -42,10 +39,6 @@ def _need_gpu():
         pytest.skip("no CUDA device")
     ns.lib().bestla_init()
     yield
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
 # ------------------------------------------------------------------------------------------------------------- 1. kernel
@@ -86,7 +79,7 @@ def test_kernel_equals_the_host_restatement(V):
         for r in range(n):
             ids, sc = ns.beam_candidates_row_host(x[r], k, float(prev[r]), bool(mask[r]), eos)
             assert np.array_equal(got[r, :, 0], ids), (n, k, r)
-            assert np.array_equal(got[r, :, 1].view(np.uint32), _bits(sc)), (n, k, r)
+            assert np.array_equal(got[r, :, 1].view(np.uint32), bits(sc)), (n, k, r)
 
 
 # ------------------------------------------------------------------------------------------------------------- 2. kv_copy
@@ -106,8 +99,7 @@ def _kv(eng):
 
 
 def test_kv_copy_bytes_and_forks():
-    toy = Toy()
-    eng = toy.engine(n_seq=6)
+    eng = toy(4, 2, n_ctx=96).engine(n_seq=6)
     rng = np.random.default_rng(3)
     prompts = [rng.integers(0, 320, 9 + 3 * s).tolist() for s in range(4)]
     eng.eval_batch([0, 1, 2, 3], prompts, [0, 0, 0, 0])
@@ -122,7 +114,7 @@ def test_kv_copy_bytes_and_forks():
     # a fork decodes as the original: block 2's 15 positions into block 4, then the same token on both
     eng.kv_copy([2], [4], 0, 15)
     lg, _ = eng.decode_batch([2, 4], [7, 7], [15, 15])
-    assert np.array_equal(_bits(lg[0]), _bits(lg[1]))
+    assert np.array_equal(bits(lg[0]), bits(lg[1]))
     before = eng.kv_bytes()
     n0 = ns.lib().ns_launch_count()
     for src, dst, p0, p1 in [([1, 4], [4, 5], 0, 4), ([1, 2], [3, 3], 0, 4), ([1], [1], 0, 4), ([1], [6], 0, 4), ([1], [2], 3, 2),
@@ -169,8 +161,8 @@ class EngineModel:
 
 @pytest.mark.parametrize("out_fmt", ["q4_0", "q6_K"])
 def test_engine_equals_the_oracle_on_its_own_logits(orc, out_fmt):  # noqa: F811
-    toy = Toy(out_fmt=out_fmt)
-    eng, ref = toy.engine(n_seq=32), toy.engine(n_seq=32)
+    m = toy(4, 2, out_fmt, n_ctx=96)
+    eng, ref = m.engine(n_seq=32), m.engine(n_seq=32)
     rng = np.random.default_rng(11)
     V, eos = 320, 5
     row_counts = set()
@@ -184,7 +176,7 @@ def test_engine_equals_the_oracle_on_its_own_logits(orc, out_fmt):  # noqa: F811
         row_counts.update(model.rows)
         for (gt, gs), (wt, ws) in zip(got, want):
             assert np.array_equal(gt, wt), (B, n, got, want)
-            assert _bits(gs) == _bits(ws), (B, n, got, want)
+            assert bits(np.float32(gs)) == bits(np.float32(ws)), (B, n, got, want)
     assert {2, 4} <= row_counts and max(row_counts) == 32  # GEMV-tile and tensor-core passes
     eng.close()
     ref.close()
@@ -192,52 +184,19 @@ def test_engine_equals_the_oracle_on_its_own_logits(orc, out_fmt):  # noqa: F811
 
 # ------------------------------------------------------------------------------------------------------------- 5. 7B shapes
 def test_llama2_7b_shaped_candidates_and_identity(orc):  # noqa: F811
-    """synthetic Llama-2-7B weights as tests/test_gpu_eval_all.py's 7B-shape test (Q4_0, two layers, the full output head)"""
+    """synthetic Llama-2-7B weights (tests/llama_models.py: Q4_0, two layers, the full output head); the first step's candidates
+    under the per-step bar of the reference against its +-64 ulp jig"""
     rng = np.random.default_rng(2025)
-    hp = dict(n_vocab=32000, n_embd=4096, n_head=32, n_head_kv=32, n_layer=2, n_ff=11008, n_ctx=64, norm_eps=1e-5, rope_theta=10000.0,
-              rope_scale=1.0)
-    E, FF, V = hp["n_embd"], hp["n_ff"], hp["n_vocab"]
-    tok = rng.standard_normal((V, E), dtype=np.float32)
-    out_norm = rng.uniform(0.5, 1.5, E).astype(np.float32)
-
-    def qw(n, k):
-        return oracle.quantize_q4_0((rng.standard_normal((n, k), dtype=np.float32) * np.float32(1.0 / np.sqrt(k))))
-
-    shapes = dict(wq=(E, E), wk=(E, E), wv=(E, E), wo=(E, E), w1=(FF, E), w2=(E, FF), w3=(FF, E))
-    layers = []
-    for _ in range(hp["n_layer"]):
-        lay = dict(attn_norm=rng.uniform(0.5, 1.5, E).astype(np.float32), ffn_norm=rng.uniform(0.5, 1.5, E).astype(np.float32))
-        for name, (n, k) in shapes.items():
-            lay[name] = qw(n, k)
-        layers.append(lay)
-    out_rows = qw(V, E)
-    mk = (lambda t_: oracle.RefNeLlama(hp, t_, out_norm, out_rows, layers)) if oracle.ref_ne() is not None else (
-        lambda t_: OracleLlama(hp, t_, out_norm, out_rows, layers))
+    m = llama2_7b_shaped(rng, n_ctx=64)
+    V = m.hp["n_vocab"]
     prompts = [[1] + [int(t) for t in rng.integers(3, V, 9)], [1] + [int(t) for t in rng.integers(3, V, 6)]]
-    jig = (rng.integers(0, 2, tok.shape, dtype=np.int8).astype(np.int32) * 2 - 1) * 64
+    m.draw_jig(rng)
     last = {}
-    for which, t_ in (("ref", tok), ("jig", (tok.view(np.int32) + jig).view(np.float32))):
-        r = mk(t_)
-        last[which] = [_token_rows(r, p, 0)[-1] for p in prompts]  # the prompt evaluated token by token, as the 7B logits_all test
-        if hasattr(r, "close"):
-            r.close()
-    del jig
-
-    def engine():
-        eng = ns.Llama(**hp)
-        eng.set_f32(ns.Llama.TOK_EMBD, 0, tok)
-        eng.set_f32(ns.Llama.OUT_NORM, 0, out_norm)
-        eng.set_weight(ns.Llama.OUTPUT, 0, ns.Weight.from_q4_0_host(out_rows, V, E))
-        ids = dict(wq=ns.Llama.WQ, wk=ns.Llama.WK, wv=ns.Llama.WV, wo=ns.Llama.WO, w1=ns.Llama.W1, w2=ns.Llama.W2, w3=ns.Llama.W3)
-        for il, lay in enumerate(layers):
-            eng.set_f32(ns.Llama.ATTN_NORM, il, lay["attn_norm"])
-            eng.set_f32(ns.Llama.FFN_NORM, il, lay["ffn_norm"])
-            for name, (nn, k) in shapes.items():
-                eng.set_weight(ids[name], il, ns.Weight.from_q4_0_host(lay[name], nn, k))
-        eng.set_sequences(8)
-        return eng
-
-    eng, ref = engine(), engine()
+    for which in ("ref", "jig"):
+        r = m.reference(jig=which == "jig")
+        last[which] = [rows(r, p, 0)[-1] for p in prompts]  # the prompt evaluated token by token, as the 7B logits_all test
+        close(r)
+    eng, ref = m.engine(8), m.engine(8)
     B = 4
     # the first step's candidates: the candidates kernel on the engine's prompt logits against float64 log_softmax of the
     # reference's, where the reference's own margins clear the bar
@@ -252,14 +211,13 @@ def test_llama2_7b_shaped_candidates_and_identity(orc):  # noqa: F811
     checked = 0
     for r in range(2):
         want, self_w = last["ref"][r].astype(np.float64), last["jig"][r]
-        scale = max(1.0, float(np.abs(want).max()))
-        bound = min(max(1e-2, 1.5 * float(np.abs(self_w - want).max()) / scale), 2.5e-2)
+        sc, bound = scale(want), bar(distance(self_w, want))
         order = np.lexsort((np.arange(V), -want))
         lsm = want - (want.max() + np.log(np.exp(want - want.max()).sum()))
         scores = cand[r, :, 1].view(np.float32)
         for j in range(B):
-            assert abs(float(scores[j]) - lsm[cand[r, j, 0]]) <= 2 * bound * scale, (r, j, scores[j], lsm[cand[r, j, 0]])
-            if want[order[j]] - want[order[j + 1]] > 2 * bound * scale and (j == 0 or want[order[j - 1]] - want[order[j]] > 2 * bound * scale):
+            assert abs(float(scores[j]) - lsm[cand[r, j, 0]]) <= 2 * bound * sc, (r, j, scores[j], lsm[cand[r, j, 0]])
+            if want[order[j]] - want[order[j + 1]] > 2 * bound * sc and (j == 0 or want[order[j - 1]] - want[order[j]] > 2 * bound * sc):
                 assert cand[r, j, 0] == order[j], (r, j)
                 checked += 1
     print(f"7B-shape first-step candidates: {checked} of {2 * B} ranks clear of the bar and equal")
@@ -268,15 +226,15 @@ def test_llama2_7b_shaped_candidates_and_identity(orc):  # noqa: F811
         got = eng.beam_search(ps, Bq, 4, 0, 1.0, False, 2)
         want = oracle_search(orc, V, ps, EngineModel(ref, Bq), Bq, 4, 0, 1.0, False, 2)
         for (gt, gs), (wt, wsc) in zip(got, want):
-            assert np.array_equal(gt, wt) and _bits(gs) == _bits(wsc), (Bq, got, want)
+            assert np.array_equal(gt, wt) and bits(np.float32(gs)) == bits(np.float32(wsc)), (Bq, got, want)
     eng.close()
     ref.close()
 
 
 # ------------------------------------------------------------------------------------------------------------- 6. structure
 def test_launches_refusals_and_untouched_blocks():
-    toy = Toy()
-    eng = toy.engine(n_seq=12)
+    m = toy(4, 2, n_ctx=96)
+    eng = m.engine(n_seq=12)
     rng = np.random.default_rng(5)
     # a greedy generate before and after, on block 0
     eng.eval([1, 2, 3], 0)
@@ -318,7 +276,7 @@ def test_launches_refusals_and_untouched_blocks():
     eng.set_sampling(None)
     assert L.ns_launch_count() == n0
     eng.close()
-    one = toy.engine()
+    one = m.engine()
     one.set_streaming(4)
     with pytest.raises(RuntimeError, match="streaming"):
         one.beam_search([[1, 2]], 2, 3)

@@ -14,8 +14,8 @@ import numpy as np
 import pytest
 import torch
 
+import llama_models
 import neural_speed_b200 as ns
-import oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -155,45 +155,10 @@ def test_entry_refusals_launch_nothing():
 
 
 # --------------------------------------------------------------------------------------------------------------- engine
-class Toy:
-    """a small Llama with Q4_0 weights (vocab 320, n_embd 256, n_ff 512, head size 64)"""
-
-    def __init__(self, n_ctx=160, seed=0, n_layer=2):
-        rng = np.random.default_rng(seed)
-        self.hp = dict(n_vocab=320, n_embd=256, n_head=4, n_head_kv=2, n_layer=n_layer, n_ff=512, n_ctx=n_ctx, norm_eps=1e-5,
-                       rope_theta=10000.0, rope_scale=1.0)
-        E, FF, V, kvd = 256, 512, 320, 128
-
-        def w(n, k):
-            return oracle.quantize_q4_0(rng.normal(0, 1.0 / np.sqrt(k), (n, k)).astype(np.float32))
-
-        self.tok = rng.normal(0, 1, (V, E)).astype(np.float32)
-        self.out_norm = rng.uniform(0.5, 1.5, E).astype(np.float32)
-        self.shapes = dict(wq=(E, E), wk=(kvd, E), wv=(kvd, E), wo=(E, E), w1=(FF, E), w2=(E, FF), w3=(FF, E))
-        self.layers = [dict(attn_norm=rng.uniform(0.5, 1.5, E).astype(np.float32), ffn_norm=rng.uniform(0.5, 1.5, E).astype(np.float32),
-                            **{name: w(n, k) for name, (n, k) in self.shapes.items()}) for _ in range(n_layer)]
-        self.out_rows = w(V, E)
-
-    def engine(self, n_seq=1):
-        hp = self.hp
-        eng = ns.Llama(**hp)
-        eng.set_f32(ns.Llama.TOK_EMBD, 0, self.tok)
-        eng.set_f32(ns.Llama.OUT_NORM, 0, self.out_norm)
-        eng.set_weight(ns.Llama.OUTPUT, 0, ns.Weight.from_q4_0_host(self.out_rows, hp["n_vocab"], hp["n_embd"]))
-        ids = dict(wq=ns.Llama.WQ, wk=ns.Llama.WK, wv=ns.Llama.WV, wo=ns.Llama.WO, w1=ns.Llama.W1, w2=ns.Llama.W2, w3=ns.Llama.W3)
-        for il, L in enumerate(self.layers):
-            eng.set_f32(ns.Llama.ATTN_NORM, il, L["attn_norm"])
-            eng.set_f32(ns.Llama.FFN_NORM, il, L["ffn_norm"])
-            for name, (n, k) in self.shapes.items():
-                eng.set_weight(ids[name], il, ns.Weight.from_q4_0_host(L[name], n, k))
-        if n_seq != 1:
-            eng.set_sequences(n_seq)
-        return eng
-
-
 @pytest.fixture(scope="module")
 def toy():
-    return Toy()
+    """the toy Llama with GQA (4 heads on 2, head size 64)"""
+    return llama_models.toy(4, 2, n_ctx=160)
 
 
 SAMPLE = dict(top_k=40, top_p=0.95, temperature=0.8, repeat_penalty=1.1, repeat_last_n=64)
@@ -243,8 +208,7 @@ def test_generate_matches_host_sampled_eval_loop(toy):
 
 
 def test_generate_on_the_streaming_ring_matches_host_sampled_eval_loop():
-    t = Toy(n_ctx=48, seed=1)
-    eng = t.engine()
+    eng = llama_models.toy(4, 2, seed=1, n_ctx=48).engine()
     eng.set_streaming(4)
     _generate_vs_eval_loop(eng, 48, [5, 6, 7, 8, 9, 10], 110, seed=99)
 

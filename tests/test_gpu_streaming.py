@@ -6,10 +6,10 @@ import pytest
 import torch
 
 import neural_speed_b200 as ns
-import oracle
+from llama_models import RunningBar, close, llama2_7b_shaped, scale, toy, unambiguous
 from oracle import llama_model as lm
 from oracle import streaming as sm
-from oracle.llama_model import OracleLlama, greedy
+from oracle.llama_model import greedy
 
 pytestmark = pytest.mark.gpu
 
@@ -127,46 +127,15 @@ def test_ring_entry_argument_checks():
 
 
 # ------------------------------------------------------------------------------------------------------------- the engine
-def _build(n_head=4, n_head_kv=4, seed=0, n_ctx=48, n_keep=None, jig=0):
-    """the toy Llama of tests/test_gpu_llama.py: the engine and the CPU graph (ring mode with n_keep)"""
-    rng = np.random.default_rng(seed)
-    hp = dict(n_vocab=320, n_embd=256, n_head=n_head, n_head_kv=n_head_kv, n_layer=2, n_ff=512, n_ctx=n_ctx, norm_eps=1e-5,
-              rope_theta=10000.0, rope_scale=1.0)
-    E, FF, V = hp["n_embd"], hp["n_ff"], hp["n_vocab"]
-    kvd = E // n_head * n_head_kv
-    tok = rng.normal(0, 1, (V, E)).astype(np.float32)
-    out_norm = rng.uniform(0.5, 1.5, E).astype(np.float32)
-    shapes = dict(wq=(E, E), wk=(kvd, E), wv=(kvd, E), wo=(E, E), w1=(FF, E), w2=(E, FF), w3=(FF, E))
-    layers = []
-    for _ in range(2):
-        L = dict(attn_norm=rng.uniform(0.5, 1.5, E).astype(np.float32), ffn_norm=rng.uniform(0.5, 1.5, E).astype(np.float32))
-        for name, (n, k) in shapes.items():
-            L[name] = oracle.quantize_q4_0(rng.normal(0, 1.0 / np.sqrt(k), (n, k)).astype(np.float32))
-        layers.append(L)
-    out_rows = oracle.quantize_q4_0(rng.normal(0, 1.0 / np.sqrt(E), (V, E)).astype(np.float32))
-    cpu = (lambda t_: OracleLlama(hp, t_, out_norm, out_rows, layers)) if n_keep is None else (
-        lambda t_: sm.OracleLlamaRing(hp, t_, out_norm, out_rows, layers, n_keep))
-    orc = cpu(tok)
-    if jig:  # the same CPU graph with every embedding value moved by +-jig ulp: the conditioning floor of the graph itself
-        sgn = (np.random.default_rng(99).integers(0, 2, tok.shape) * 2 - 1).astype(np.int32)
-        orc.jig = cpu((tok.view(np.int32) + sgn * jig).view(np.float32))
-    eng = ns.Llama(**hp)
-    eng.set_f32(ns.Llama.TOK_EMBD, 0, tok)
-    eng.set_f32(ns.Llama.OUT_NORM, 0, out_norm)
-    eng.set_weight(ns.Llama.OUTPUT, 0, ns.Weight.from_q4_0_host(out_rows, V, E))
-    ids = dict(wq=ns.Llama.WQ, wk=ns.Llama.WK, wv=ns.Llama.WV, wo=ns.Llama.WO, w1=ns.Llama.W1, w2=ns.Llama.W2, w3=ns.Llama.W3)
-    for il, L in enumerate(layers):
-        eng.set_f32(ns.Llama.ATTN_NORM, il, L["attn_norm"])
-        eng.set_f32(ns.Llama.FFN_NORM, il, L["ffn_norm"])
-        for name, (n, k) in shapes.items():
-            eng.set_weight(ids[name], il, ns.Weight.from_q4_0_host(L[name], n, k))
-    if n_keep is not None:
-        eng.set_streaming(n_keep)
-    return hp, orc, eng
+def _ring_graph(m, n_keep, jig=False):
+    """the CPU graph of a toy model in ring mode"""
+    return sm.OracleLlamaRing(m.hp, m.tok_jig if jig else m.tok, m.out_norm, m.out_rows, m.layers, n_keep)
 
 
-def _bound(want, floor):
-    return min(max(1e-2, 1.5 * floor), 2.5e-2) * max(1.0, float(np.abs(want).max()))
+def _ring_engine(m, n_keep):
+    eng = m.engine()
+    eng.set_streaming(n_keep)
+    return eng
 
 
 @pytest.mark.parametrize("n_head,n_head_kv,n_keep", [(4, 4, 4), (4, 2, 1), (2, 1, 0), (2, 2, 4)])
@@ -174,30 +143,29 @@ def test_ring_decode_matches_the_cpu_graph(n_head, n_head_kv, n_keep):
     """a 4-token prompt, then single tokens to 2.5 n_ctx (n_ctx 48), teacher-forced: logits at every step within the north star
     of OracleLlamaRing (or 1.5 x the CPU graph's own floor, measured with +-64 ulp inputs, where that is larger), ids
     equal wherever the top-2 margin exceeds the bound; head sizes 64 and 128, MHA and GQA"""
-    hp, orc, eng = _build(n_head, n_head_kv, seed=40 + n_keep, n_keep=n_keep, jig=64)
-    n_ctx = hp["n_ctx"]
-    seq = [int(t) for t in np.random.default_rng(n_head).integers(3, hp["n_vocab"], int(2.5 * n_ctx))]
+    m = toy(n_head, n_head_kv, seed=40 + n_keep)
+    orc, jig, eng = _ring_graph(m, n_keep), _ring_graph(m, n_keep, jig=True), _ring_engine(m, n_keep)
+    n_ctx = m.hp["n_ctx"]
+    seq = [int(t) for t in np.random.default_rng(n_head).integers(3, m.hp["n_vocab"], int(2.5 * n_ctx))]
     steps = [(seq[:4], 0)] + [([seq[t]], t) for t in range(4, len(seq))]
-    worst, floor = 0.0, 0.0
+    worst, running = 0.0, RunningBar()
     for toks, pos in steps:
         want = orc.eval(toks, pos)
-        floor = max(floor, float(np.abs(orc.jig.eval(toks, pos) - want).max()) / max(1.0, float(np.abs(want).max())))
+        tol = running(want, jig.eval(toks, pos))
         got, nxt = eng.eval(toks, pos)
-        err = float(np.abs(got - want).max())
-        bound = _bound(want, floor)
-        assert err <= bound, (pos, err, floor)
-        worst = max(worst, err / max(1.0, float(np.abs(want).max())))
-        top = np.sort(want)[-2:]
-        if top[1] - top[0] > 2 * bound:
+        s, err = scale(want), float(np.abs(got - want).max())
+        assert err <= tol * s, (pos, err, running.floor)
+        worst = max(worst, err / s)
+        if unambiguous(want, 2 * tol):
             assert nxt == greedy(want), pos
-    print(f"ring decode H{n_head}/{n_head_kv} keep{n_keep}: worst |dlogit|/max|logit| {worst:.2e}, CPU graph floor {floor:.2e}")
+    print(f"ring decode H{n_head}/{n_head_kv} keep{n_keep}: worst |dlogit|/max|logit| {worst:.2e}, CPU graph floor {running.floor:.2e}")
     eng.close()
 
 
 def test_before_the_wrap_streaming_is_bit_identical_to_plain():
     for n_head_kv in (4, 2):
-        _, _, plain = _build(4, n_head_kv, seed=50)
-        _, _, ring = _build(4, n_head_kv, seed=50, n_keep=4)
+        m = toy(4, n_head_kv, seed=50)
+        plain, ring = m.engine(), _ring_engine(m, 4)
         seq = [int(t) for t in np.random.default_rng(2).integers(3, 320, 48)]
         steps = [(seq[:20], 0)] + [([seq[t]], t) for t in range(20, 48)]
         for toks, pos in steps:
@@ -211,7 +179,9 @@ def test_a_ring_step_launches_as_many_kernels_as_a_plain_step():
     L = ns.lib()
     counts = []
     for n_keep in (None, 4):
-        _, _, eng = _build(4, 2, seed=51, n_keep=n_keep)
+        eng = toy(4, 2, seed=51).engine()
+        if n_keep is not None:
+            eng.set_streaming(n_keep)
         eng.eval([1, 2, 3], 0)
         before = L.ns_launch_count()
         eng.eval([5], 3)  # builds the decode graph: one eager pass and the captured one
@@ -221,8 +191,8 @@ def test_a_ring_step_launches_as_many_kernels_as_a_plain_step():
 
 
 def test_generate_across_two_wraps_matches_the_eval_loop():
-    _, _, a = _build(4, 2, seed=52, n_keep=4)
-    _, _, b = _build(4, 2, seed=52, n_keep=4)
+    m = toy(4, 2, seed=52)
+    a, b = _ring_engine(m, 4), _ring_engine(m, 4)
     prompt = [3, 14, 15, 92, 65]
     n_new = 2 * 48 + 30  # the record buffer (n_ctx picks) drains three times
     a.eval(prompt, 0)
@@ -242,7 +212,8 @@ def test_generate_across_two_wraps_matches_the_eval_loop():
 
 def test_streaming_argument_checks():
     L = ns.lib()
-    hp, _, eng = _build(4, 2, seed=53, n_ctx=16)
+    m = toy(4, 2, seed=53, n_ctx=16)
+    hp, eng = dict(m.hp), m.engine()
     toks = np.arange(16, dtype=np.int32)
     ev = lambda n, past: L.ns_llama_eval(eng.h, toks.ctypes.data, n, past, None, None)
     assert ev(1, 16) == -1 and "n_ctx" in ns.last_error()          # streaming off: past n_ctx stays invalid
@@ -259,7 +230,7 @@ def test_streaming_argument_checks():
     eng.set_streaming(-1)
     assert ev(1, 16) == -1
     eng.close()
-    _, _, e2 = _build(2, 2, seed=54)
+    e2 = toy(2, 2, seed=54).engine()
     assert L.ns_llama_set_streaming(e2.h, 4) == 0
     e2.close()
     hp["rope_scale"] = 2.0
@@ -275,64 +246,35 @@ def test_streaming_argument_checks():
 def test_llama2_7b_shaped_ring_against_the_reference_engine():
     """n_embd 4096, 32 heads of 128, two layers, vocab 32000, Q4_0, n_ctx 256, n_keep 4: a 240-token prompt (exact prefill), then
     single teacher-forced tokens to position 300, against the reference's engine running the shift-RoPE-K graph
-    (oracle.streaming.RefNeLlamaRing) where oracle/_ref was built, else against OracleLlamaRing.  Bound: max(1e-2, 1.5 x the reference's own floor with +-64 ulp inputs,
-    running maximum), at most 2.5e-2 (cf. tests/test_gpu_llama.py's 7B-shaped test)."""
+    (oracle.streaming.RefNeLlamaRing) where oracle/_ref was built, else against OracleLlamaRing.  Bound: max(1e-2, 1.5 x the
+    reference's own floor with +-64 ulp inputs, running maximum), at most 2.5e-2 (tests/llama_models.py)."""
     rng = np.random.default_rng(2025)
     n_keep = 4
-    hp = dict(n_vocab=32000, n_embd=4096, n_head=32, n_head_kv=32, n_layer=2, n_ff=11008, n_ctx=256, norm_eps=1e-5, rope_theta=10000.0,
-              rope_scale=1.0)
-    E, FF, V = hp["n_embd"], hp["n_ff"], hp["n_vocab"]
-    tok = rng.standard_normal((V, E), dtype=np.float32)
-    out_norm = rng.uniform(0.5, 1.5, E).astype(np.float32)
-    qw = lambda n, k: oracle.quantize_q4_0(rng.standard_normal((n, k), dtype=np.float32) * np.float32(1.0 / np.sqrt(k)))
-    shapes = dict(wq=(E, E), wk=(E, E), wv=(E, E), wo=(E, E), w1=(FF, E), w2=(E, FF), w3=(FF, E))
-    layers = []
-    for _ in range(2):
-        lay = dict(attn_norm=rng.uniform(0.5, 1.5, E).astype(np.float32), ffn_norm=rng.uniform(0.5, 1.5, E).astype(np.float32))
-        for name, (n, k) in shapes.items():
-            lay[name] = qw(n, k)
-        layers.append(lay)
-    out_rows = qw(V, E)
-    table = sm.shift_table(128)
+    m = llama2_7b_shaped(rng, n_ctx=256)
+    m.draw_jig(rng)
     if sm.ref_ne_ring() is not None:
-        mk = lambda t_: sm.RefNeLlamaRing(hp, t_, out_norm, out_rows, layers, n_keep, table)
+        table = sm.shift_table(128)
+        ref, ref_jig = (sm.RefNeLlamaRing(m.hp, t_, m.out_norm, m.out_rows, m.layers, n_keep, table) for t_ in (m.tok, m.tok_jig))
     else:
-        mk = lambda t_: sm.OracleLlamaRing(hp, t_, out_norm, out_rows, layers, n_keep)
-    ref = mk(tok)
-    jig = (rng.integers(0, 2, tok.shape, dtype=np.int8).astype(np.int32) * 2 - 1) * 64
-    ref_jig = mk((tok.view(np.int32) + jig).view(np.float32))
-    del jig
-    eng = ns.Llama(**hp)
-    eng.set_f32(ns.Llama.TOK_EMBD, 0, tok)
-    eng.set_f32(ns.Llama.OUT_NORM, 0, out_norm)
-    eng.set_weight(ns.Llama.OUTPUT, 0, ns.Weight.from_q4_0_host(out_rows, V, E))
-    ids = dict(wq=ns.Llama.WQ, wk=ns.Llama.WK, wv=ns.Llama.WV, wo=ns.Llama.WO, w1=ns.Llama.W1, w2=ns.Llama.W2, w3=ns.Llama.W3)
-    for il, lay in enumerate(layers):
-        eng.set_f32(ns.Llama.ATTN_NORM, il, lay["attn_norm"])
-        eng.set_f32(ns.Llama.FFN_NORM, il, lay["ffn_norm"])
-        for name, (n, k) in shapes.items():
-            eng.set_weight(ids[name], il, ns.Weight.from_q4_0_host(lay[name], n, k))
+        ref, ref_jig = _ring_graph(m, n_keep), _ring_graph(m, n_keep, jig=True)
+    eng = m.engine()
     eng.set_exact_prefill(True)
     eng.set_streaming(n_keep)
-    seq = [1] + [int(t) for t in rng.integers(3, V, 299)]
+    seq = [1] + [int(t) for t in rng.integers(3, m.hp["n_vocab"], 299)]
     steps = [(seq[:240], 0)] + [([seq[t]], t) for t in range(240, 300)]
-    worst, worst_self, checked, agree = 0.0, 0.0, 0, 0
+    worst, running, checked, agree = 0.0, RunningBar(), 0, 0
     for toks, pos in steps:
         want = ref.eval(toks, pos)
-        worst_self = max(worst_self, float(np.abs(ref_jig.eval(toks, pos) - want).max()) / max(1.0, float(np.abs(want).max())))
+        tol = running(want, ref_jig.eval(toks, pos))
         got, nxt = eng.eval(toks, pos)
-        err = float(np.abs(got - want).max())
-        bound = _bound(want, worst_self)
-        assert err <= bound, (pos, err, worst_self)
-        worst = max(worst, err / max(1.0, float(np.abs(want).max())))
-        top = np.sort(want)[-2:]
-        if top[1] - top[0] > 2 * bound:
+        s, err = scale(want), float(np.abs(got - want).max())
+        assert err <= tol * s, (pos, err, running.floor)
+        worst = max(worst, err / s)
+        if unambiguous(want, 2 * tol):
             checked += 1
             agree += int(nxt == greedy(want))
-    print(f"7B-shape ring: worst |dlogit|/max|logit| {worst:.2e}; the reference against itself (+-64 ulp) {worst_self:.2e}; ids "
+    print(f"7B-shape ring: worst |dlogit|/max|logit| {worst:.2e}; the reference against itself (+-64 ulp) {running.floor:.2e}; ids "
           f"{agree}/{checked}")
     assert agree == checked
     eng.close()
-    for m in (ref, ref_jig):
-        if hasattr(m, "close"):
-            m.close()
+    close(ref, ref_jig)
