@@ -523,9 +523,31 @@ typedef int (*ns_beam_logits_fn)(void* user, int rows, const int* req, const int
 NS_API int ns_beam_search_host(int n_vocab, int n_ctx, int n, const int* n_tokens, const int32_t* tokens, const ns_llama_beams* cfg,
                                ns_beam_logits_fn logits, void* user, int32_t* out_tokens, int* out_len, float* out_score);
 NS_API float ns_sample_expf_host(float x);
-NS_API unsigned long long ns_llama_kv_bytes(const ns_llama* ctx); /* all n_seq blocks */
-/* The device pointers of the fp16 KV cache, [n_layer][n_seq][n_head_kv][n_ctx][head size] each for K and V (for tests). */
+NS_API unsigned long long ns_llama_kv_bytes(const ns_llama* ctx); /* all n_seq blocks, every plane: the device allocation */
+/* The device pointers of the fp16 KV cache, [n_layer][n_seq][n_head_kv][n_ctx][head size] each for K and V (for tests).
+ * NS_E_UNSUPPORTED while the cache is Q8_0 (ns_llama_kv_planes). */
 NS_API int ns_llama_kv_cache(const ns_llama* ctx, void** k, void** v);
+/* ---- KV cache element format ------------------------------------------------------------------------------------------------
+ *   NS_KV_F16   (default) fp16 K / V, the reference's ggml cache
+ *   NS_KV_Q8_0  K / V rows stored as ggml Q8_0 blocks of 32: K after RoPE and V as projected are quantised in fp32 by the
+ *               activation quantiser of the NS_COMP_Q8_0 matmuls (d = fp16(amax / 127), codes round-half-even of x * 127 / amax);
+ *               each unit (layer, block, kv head) has a code plane [n_ctx][hd] int8 and a scale plane of hd / 32 fp16 per row,
+ *               n_ctx * hd / 32 halves padded to a multiple of 8.  Attention reads fp16(q * d) wherever it read an fp16 cache value,
+ *               and the decode step's own new row likewise, so a Q8_0 cache C attends exactly as an fp16 cache holding those values.
+ *               About 0.53x the bytes of fp16 at head size 128 (136 B against 256 B per row).
+ * ns_llama_set_kv_type reallocates and zeroes every block (every sequence restarts at n_past 0) and drops the captured graphs, like
+ * ns_llama_set_sequences.  NS_E_INVALID for another type; NS_E_UNSUPPORTED (nothing changed) for Q8_0 with streaming on (either
+ * order: ns_llama_set_streaming refuses n_keep >= 0 on a Q8_0 cache) or a head size other than 64 / 128.  Under Q8_0 one-row steps
+ * take the split decode attention and every longer step the tensor-core prompt attention (also 2 .. 7 rows of ns_llama_eval_seq);
+ * NS_ATTN_ROWS / NS_ATTN_GENERIC (and the NS_ATTN_OLD_DECODE / NS_ATTN_SCALAR switches) have no Q8_0 form: NS_E_UNSUPPORTED. */
+#define NS_KV_F16 0
+#define NS_KV_Q8_0 1
+NS_API int ns_llama_set_kv_type(ns_llama* ctx, int type);
+NS_API int ns_llama_kv_type(const ns_llama* ctx);
+/* The device planes of the KV cache (for tests): fp16 -- k / v as ns_llama_kv_cache, kd / vd null; Q8_0 -- k / v the codes
+ * [n_layer][n_seq][n_head_kv][n_ctx][hd] int8, kd / vd the scales [n_layer][n_seq][n_head_kv][stride] fp16, stride = n_ctx * hd / 32
+ * rounded up to a multiple of 8, row p of a unit at p * hd / 32. */
+NS_API int ns_llama_kv_planes(const ns_llama* ctx, void** k, void** kd, void** v, void** vd);
 /* One layer's attention of the eval step on its own, for parity tests: RoPE (mode 0, angle = p * rope_theta^(-2i/hd) / rope_scale)
  * of q [m][n_head * hd] in place and of the m new rows k [m][n_head_kv * hd] at positions n_past .. n_past + m - 1, k and v appended
  * to the fp16 caches kc / vc [n_head_kv][n_ctx][hd], out [m][n_head * hd] = causal softmax(K q / sqrt(hd)) V (llama.cpp:286-302).
@@ -575,6 +597,19 @@ NS_API size_t ns_llama_attention_ragged_workspace_bytes(int n, int n_rows);
 NS_API int ns_llama_attention_ragged(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n, const int* seq,
                                      const int* n_tokens, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
                                      float rope_theta, float rope_scale, float* out, void* ws, void* queue);
+/* The three entries above on a Q8_0 cache (NS_KV_Q8_0): kq / vq the code planes, kd / vd the scale planes of the same units
+ * (ns_llama_kv_planes' layout with n_layer = 1).  Same workspaces and argument rules; NS_E_UNSUPPORTED (nothing launched) for head
+ * sizes other than 64 / 128 and for NS_ATTN_ROWS / NS_ATTN_GENERIC; NS_ATTN_AUTO takes NS_ATTN_SPLIT_DECODE for m = 1, NS_ATTN_MMA
+ * otherwise. */
+NS_API int ns_llama_attention_q8_0(int kernel, float* q, const float* k, const float* v, void* kq, void* kd, void* vq, void* vd,
+                                   int n_head, int n_head_kv, int hd, int n_ctx, int n_past, int m, float rope_theta, float rope_scale,
+                                   float* out, void* ws, void* queue);
+NS_API int ns_llama_attention_batch_q8_0(float* q, const float* k, const float* v, void* kq, void* kd, void* vq, void* vd, int n_seq,
+                                         int n, const int* seq, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
+                                         float rope_theta, float rope_scale, float* out, void* ws, void* queue);
+NS_API int ns_llama_attention_ragged_q8_0(float* q, const float* k, const float* v, void* kq, void* kd, void* vq, void* vd, int n_seq,
+                                          int n, const int* seq, const int* n_tokens, const int* n_past, int n_head, int n_head_kv,
+                                          int hd, int n_ctx, float rope_theta, float rope_scale, float* out, void* ws, void* queue);
 
 /* ---- tensor-parallel exchange step over NVLink peer memory (SURVEY 8e) --------------------------------------------
  * One-shot sum all-reduce replacing reduce_add / ne_all_reduce (core/parallel_context.cpp:47, ne_layers.c:5466) for the

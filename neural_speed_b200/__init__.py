@@ -67,6 +67,8 @@ EXPORTS = [
     "ns_sample_expf_host", "ns_llama_eval_all", "ns_llama_logprob_workspace_bytes", "ns_llama_logprob", "ns_logprob_row_host",
     "ns_llama_beam_search", "ns_llama_kv_copy", "ns_llama_kv_cache", "ns_llama_beam_candidates_workspace_bytes", "ns_llama_beam_candidates",
     "ns_beam_candidates_row_host", "ns_logf_host", "ns_beam_search_host",
+    "ns_llama_set_kv_type", "ns_llama_kv_type", "ns_llama_kv_planes", "ns_llama_attention_q8_0", "ns_llama_attention_batch_q8_0",
+    "ns_llama_attention_ragged_q8_0",
     "ns_comm_handle_bytes", "ns_comm_create", "ns_comm_get_handle", "ns_comm_open_peers", "ns_comm_link_local", "ns_comm_all_reduce_f32",
     "ns_comm_status", "ns_comm_free",
 ]
@@ -224,6 +226,13 @@ def lib() -> C.CDLL:
     L.ns_llama_beam_search.argtypes = [vp, i, vp, vp, vp, vp, vp, vp]
     L.ns_llama_kv_copy.argtypes = [vp, i, vp, vp, i, i]
     L.ns_llama_kv_cache.argtypes = [vp, vp, vp]
+    L.ns_llama_set_kv_type.argtypes = [vp, i]
+    L.ns_llama_kv_type.argtypes = [vp]
+    L.ns_llama_kv_planes.argtypes = [vp, vp, vp, vp, vp]
+    L.ns_llama_attention_q8_0.argtypes = [i, vp, vp, vp, vp, vp, vp, vp, i, i, i, i, i, i, C.c_float, C.c_float, vp, vp, vp]
+    L.ns_llama_attention_batch_q8_0.argtypes = [vp, vp, vp, vp, vp, vp, vp, i, i, vp, vp, i, i, i, i, C.c_float, C.c_float, vp, vp, vp]
+    L.ns_llama_attention_ragged_q8_0.argtypes = [vp, vp, vp, vp, vp, vp, vp, i, i, vp, vp, vp, i, i, i, i, C.c_float, C.c_float, vp, vp,
+                                                 vp]
     L.ns_llama_beam_candidates_workspace_bytes.restype = sz
     L.ns_llama_beam_candidates_workspace_bytes.argtypes = [i, i]
     L.ns_llama_beam_candidates.argtypes = [vp, i, i, i, vp, vp, C.c_int32, vp, vp, vp]
@@ -678,6 +687,24 @@ class Llama:
         _check(lib().ns_llama_kv_cache(self.h, C.byref(k), C.byref(v)), "ns_llama_kv_cache")
         return k.value, v.value
 
+    def set_kv_type(self, kind: str):
+        """the KV cache's element format, "f16" (the default) or "q8_0" (ggml Q8_0 blocks of 32 per row); every block is
+        reallocated and restarts empty (include/ns_b200.h, ns_llama_set_kv_type)"""
+        if kind not in KV_TYPES:
+            raise ValueError(f"set_kv_type: {kind!r} (one of {sorted(KV_TYPES)})")
+        _check(lib().ns_llama_set_kv_type(self.h, KV_TYPES[kind]), "ns_llama_set_kv_type")
+
+    def kv_type(self) -> str:
+        code = lib().ns_llama_kv_type(self.h)
+        return next(k for k, v in KV_TYPES.items() if v == code)
+
+    def kv_planes(self):
+        """(K, K scales, V, V scales) device pointers: for "q8_0" the int8 codes [n_layer][n_seq][n_head_kv][n_ctx][head size] and
+        the fp16 scales [n_layer][n_seq][n_head_kv][kv_d_stride(n_ctx, head size)]; for "f16" the caches and two Nones"""
+        p = [C.c_void_p() for _ in range(4)]
+        _check(lib().ns_llama_kv_planes(self.h, *(C.byref(x) for x in p)), "ns_llama_kv_planes")
+        return tuple(x.value for x in p)
+
     def close(self):
         if self.h:
             lib().ns_llama_free(self.h)
@@ -688,6 +715,49 @@ class Llama:
             self.close()
         except Exception:
             pass
+
+
+KV_TYPES = {"f16": 0, "q8_0": 1}  # NS_KV_F16, NS_KV_Q8_0
+
+
+def kv_d_stride(n_ctx: int, hd: int) -> int:
+    """halves of one (layer, block, kv head) unit of a Q8_0 scale plane: n_ctx * hd / 32, padded to a multiple of 8"""
+    return (n_ctx * (hd // 32) + 7) // 8 * 8
+
+
+def kv_bytes(kind: str, n_layer: int, n_seq: int, n_head_kv: int, n_ctx: int, hd: int) -> int:
+    """bytes of a KV cache (K and V, every plane) as ns_llama_kv_bytes reports them"""
+    units = n_layer * n_seq * n_head_kv
+    per = n_ctx * hd * 2 if kind == "f16" else n_ctx * hd + 2 * kv_d_stride(n_ctx, hd)
+    return 2 * units * per
+
+
+def attention_q8_0(kernel: int, q_ptr: int, k_ptr: int, v_ptr: int, planes, n_head: int, n_head_kv: int, hd: int, n_ctx: int, n_past: int,
+                   m: int, out_ptr: int, ws_ptr: int, rope_theta=10000.0, rope_scale=1.0, queue=None) -> int:
+    """ns_llama_attention_q8_0 on device pointers, planes = (K codes, K scales, V codes, V scales); returns the status code"""
+    kq, kd, vq, vd = (C.c_void_p(x) for x in planes)
+    return lib().ns_llama_attention_q8_0(kernel, C.c_void_p(q_ptr), C.c_void_p(k_ptr), C.c_void_p(v_ptr), kq, kd, vq, vd, n_head, n_head_kv,
+                                         hd, n_ctx, n_past, m, rope_theta, rope_scale, C.c_void_p(out_ptr), C.c_void_p(ws_ptr), queue)
+
+
+def attention_batch_q8_0(q_ptr: int, k_ptr: int, v_ptr: int, planes, n_seq: int, seqs, n_past, n_head: int, n_head_kv: int, hd: int,
+                         n_ctx: int, out_ptr: int, ws_ptr: int, rope_theta=10000.0, rope_scale=1.0, queue=None) -> int:
+    """ns_llama_attention_batch_q8_0 on device pointers, planes as attention_q8_0; returns the status code"""
+    s, p = np.ascontiguousarray(seqs, np.int32), np.ascontiguousarray(n_past, np.int32)
+    kq, kd, vq, vd = (C.c_void_p(x) for x in planes)
+    return lib().ns_llama_attention_batch_q8_0(C.c_void_p(q_ptr), C.c_void_p(k_ptr), C.c_void_p(v_ptr), kq, kd, vq, vd, n_seq, s.size,
+                                               _np_ptr(s), _np_ptr(p), n_head, n_head_kv, hd, n_ctx, rope_theta, rope_scale,
+                                               C.c_void_p(out_ptr), C.c_void_p(ws_ptr), queue)
+
+
+def attention_ragged_q8_0(q_ptr: int, k_ptr: int, v_ptr: int, planes, n_seq: int, seqs, n_tokens, n_past, n_head: int, n_head_kv: int,
+                          hd: int, n_ctx: int, out_ptr: int, ws_ptr: int, rope_theta=10000.0, rope_scale=1.0, queue=None) -> int:
+    """ns_llama_attention_ragged_q8_0 on device pointers, planes as attention_q8_0; returns the status code"""
+    s, t, p = (np.ascontiguousarray(a, np.int32) for a in (seqs, n_tokens, n_past))
+    kq, kd, vq, vd = (C.c_void_p(x) for x in planes)
+    return lib().ns_llama_attention_ragged_q8_0(C.c_void_p(q_ptr), C.c_void_p(k_ptr), C.c_void_p(v_ptr), kq, kd, vq, vd, n_seq, s.size,
+                                                _np_ptr(s), _np_ptr(t), _np_ptr(p), n_head, n_head_kv, hd, n_ctx, rope_theta, rope_scale,
+                                                C.c_void_p(out_ptr), C.c_void_p(ws_ptr), queue)
 
 
 def attention_batch(q_ptr: int, k_ptr: int, v_ptr: int, kc_ptr: int, vc_ptr: int, n_seq: int, seqs, n_past, n_head: int, n_head_kv: int,

@@ -4,6 +4,7 @@
 
 #include "async_copy.cuh"
 #include "attention.cuh"
+#include "kv_cache.cuh"
 
 namespace {
 
@@ -13,10 +14,14 @@ constexpr int kAttnThreads = 128;
 // grid (n_head + n_head_kv, n_tokens), hd/2 threads.  pos = state[1] + t.
 // RAGGED: the rows belong to segments of several sequences (ns_llama_eval_batch); row t takes its position and its KV block
 // ([n_seq][n_head_kv][n_ctx][hd]) from rows[2 t], rows[2 t + 1] instead.
-template <bool RAGGED = false>
+// KV = NS_KV_Q8_0: kc / vc are the code planes, kd / vd the scale planes (kv_cache.cuh); the rotated k and the projected v rows are
+// quantised in fp32, one 32-block per 16 threads.
+template <bool RAGGED = false, int KV = NS_KV_F16>
 __global__ void rope_kv_kernel(float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk, const float* __restrict__ v, int ldv,
-                               __half* __restrict__ kc, __half* __restrict__ vc, const int* __restrict__ state, int n_head, int n_head_kv,
-                               int hd, int n_ctx, float theta_scale, float freq_scale, const int* __restrict__ rows) {
+                               kv_elem_t<KV>* __restrict__ kc, kv_elem_t<KV>* __restrict__ vc, const int* __restrict__ state, int n_head,
+                               int n_head_kv, int hd, int n_ctx, float theta_scale, float freq_scale, const int* __restrict__ rows,
+                               __half* __restrict__ kd, __half* __restrict__ vd) {
+  constexpr bool Q8 = KV == NS_KV_Q8_0;
   pdl_launch_dependents();
   pdl_wait();
   const int h = blockIdx.x, t = blockIdx.y, i = threadIdx.x;  // pair index
@@ -26,6 +31,10 @@ __global__ void rope_kv_kernel(float* __restrict__ q, int ldq, const float* __re
     const size_t blk = (size_t)rows[2 * t + 1] * n_head_kv * n_ctx * hd;
     kc += blk;
     vc += blk;
+    if constexpr (Q8) {
+      kd += (size_t)rows[2 * t + 1] * n_head_kv * kv_d_stride(n_ctx, hd);
+      vd += (size_t)rows[2 * t + 1] * n_head_kv * kv_d_stride(n_ctx, hd);
+    }
   } else {
     pos = state[1] + t;
   }
@@ -45,13 +54,20 @@ __global__ void rope_kv_kernel(float* __restrict__ q, int ldq, const float* __re
     const float* p = k + (size_t)t * ldk + (size_t)hk * hd + 2 * i;
     const float x0 = p[0], x1 = p[1];
     if (pos < n_ctx) {
-      __half* kd = kc + ((size_t)hk * n_ctx + pos) * hd + 2 * i;
-      kd[0] = __float2half_rn(x0 * cs - x1 * sn);
-      kd[1] = __float2half_rn(x0 * sn + x1 * cs);
-      const float* pv = v + (size_t)t * ldv + (size_t)hk * hd + 2 * i;
-      __half* vd = vc + ((size_t)hk * n_ctx + pos) * hd + 2 * i;
-      vd[0] = __float2half_rn(pv[0]);
-      vd[1] = __float2half_rn(pv[1]);
+      if constexpr (Q8) {  // whole warps: hd / 2 threads, the branch uniform over the CTA
+        const float* pv = v + (size_t)t * ldv + (size_t)hk * hd + 2 * i;
+        const size_t drow = (size_t)hk * kv_d_stride(n_ctx, hd) + (size_t)pos * (hd / kKvQ8Block);
+        kv_q8_store_pair(kc + ((size_t)hk * n_ctx + pos) * hd, kd + drow, i, kv_q8_quant_pair(x0 * cs - x1 * sn, x0 * sn + x1 * cs));
+        kv_q8_store_pair(vc + ((size_t)hk * n_ctx + pos) * hd, vd + drow, i, kv_q8_quant_pair(pv[0], pv[1]));
+      } else {
+        __half* kr = kc + ((size_t)hk * n_ctx + pos) * hd + 2 * i;
+        kr[0] = __float2half_rn(x0 * cs - x1 * sn);
+        kr[1] = __float2half_rn(x0 * sn + x1 * cs);
+        const float* pv = v + (size_t)t * ldv + (size_t)hk * hd + 2 * i;
+        __half* vr = vc + ((size_t)hk * n_ctx + pos) * hd + 2 * i;
+        vr[0] = __float2half_rn(pv[0]);
+        vr[1] = __float2half_rn(pv[1]);
+      }
     }
   }
 }
@@ -319,20 +335,28 @@ __global__ void __launch_bounds__(kAW * 32) attn_fast_kernel(const float* __rest
 // (n_head, ranges, n).  CTA z serves row z: its position is state[4 z + 1] (the row's {token, n_past, n_recorded, pick}), its
 // KV block seqs[z] ([n_seq][n_head_kv][n_ctx][hd] per layer), and its q / k / v / out rows, partials and tickets are row z's.
 // Everything after those offsets is the RING = false kernel's code, so each row's arithmetic is the single-sequence step's.
+//
+// KV = NS_KV_Q8_0 (RING = false): kc / vc are the code planes, kd / vd the scale planes (kv_cache.cuh).  A range arrives as four
+// bulk copies (codes and scales of K and V, the codes in the first half of the fp16 tile's space, the scales after them) and
+// is dequantised on use.  The new k / v rows are quantised here (one 32-block per 16 threads) and the kernel scores and sums
+// their dequantised values, as if read back from the cache.
 constexpr int kSplitKeys = 256;
 constexpr int kDW = 16;  // warps per CTA
 template <int HD>
 static constexpr size_t attn_decode_smem() {
   return (size_t)2 * kSplitKeys * HD * 2 + (size_t)(3 + kDW) * HD * 4 + (size_t)(kSplitKeys + 8) * 4 + 16;
 }
-template <int HD, bool RING, bool BATCH = false>
+template <int HD, bool RING, bool BATCH = false, int KV = NS_KV_F16>
 __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __restrict__ q, const float* __restrict__ knew,
-                                                            const float* __restrict__ vnew, __half* __restrict__ kc, __half* __restrict__ vc,
-                                                            const int* __restrict__ state, float* __restrict__ out, float* __restrict__ part_ws,
-                                                            unsigned* __restrict__ tickets, int n_head, int n_head_kv, int n_ctx, int nsplit,
-                                                            float scale, float theta_scale, float freq_scale, int n_keep, const ShiftTable tab,
-                                                            const int* __restrict__ seqs) {
+                                                            const float* __restrict__ vnew, kv_elem_t<KV>* __restrict__ kc,
+                                                            kv_elem_t<KV>* __restrict__ vc, const int* __restrict__ state,
+                                                            float* __restrict__ out, float* __restrict__ part_ws, unsigned* __restrict__ tickets,
+                                                            int n_head, int n_head_kv, int n_ctx, int nsplit, float scale, float theta_scale,
+                                                            float freq_scale, int n_keep, const ShiftTable tab, const int* __restrict__ seqs,
+                                                            __half* __restrict__ kd, __half* __restrict__ vd) {
   static_assert(!(RING && BATCH), "the ring serves one sequence");
+  constexpr bool Q8 = KV == NS_KV_Q8_0;
+  static_assert(!(RING && Q8), "the ring shifts fp16 keys");
   constexpr int EPL = HD / 32;
   extern __shared__ __align__(128) unsigned char smraw[];
   __half* Kt = reinterpret_cast<__half*>(smraw);  // [kSplitKeys][HD]
@@ -365,6 +389,10 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
     const size_t blk = (size_t)seqs[row] * n_head_kv * n_ctx * HD;
     kc += blk;
     vc += blk;
+    if constexpr (Q8) {
+      kd += (size_t)seqs[row] * n_head_kv * kv_d_stride(n_ctx, HD);
+      vd += (size_t)seqs[row] * n_head_kv * kv_d_stride(n_ctx, HD);
+    }
     q += (size_t)row * n_head * HD;
     knew += (size_t)row * n_head_kv * HD;
     vnew += (size_t)row * n_head_kv * HD;
@@ -378,8 +406,10 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   const bool tail_new = has_new && !wrapped;  // ... after the staged rows, its k / v from registers (else staged over its slot)
   const int ncache = (tail_new ? i1 - 1 : i1) - i0;  // rows staged from the cache
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __half* kh = kc + (size_t)hk * n_ctx * HD;
-  __half* vh = vc + (size_t)hk * n_ctx * HD;
+  kv_elem_t<KV>* kh = kc + (size_t)hk * n_ctx * HD;
+  kv_elem_t<KV>* vh = vc + (size_t)hk * n_ctx * HD;
+  __half* kdh = Q8 ? kd + (size_t)hk * kv_d_stride(n_ctx, HD) : nullptr;  // Q8_0: the head's scales
+  __half* vdh = Q8 ? vd + (size_t)hk * kv_d_stride(n_ctx, HD) : nullptr;
   const uint32_t bar_a = smem_u32(bar);
   if (threadIdx.x == 0) {
     mbar_init(bar_a, 1);
@@ -389,10 +419,19 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
     // likewise last written by this layer's launch of the previous token -- the launch whose appended row the plain step
     // already reads here -- so the same ordering covers them.
     if (ncache > 0) {
-      const uint32_t bytes = (uint32_t)ncache * HD * 2;
-      mbar_expect_tx(bar_a, 2 * bytes);
-      bulk_g2s(smem_u32(Kt), kh + (size_t)i0 * HD, bytes, bar_a);
-      bulk_g2s(smem_u32(Vt), vh + (size_t)i0 * HD, bytes, bar_a);
+      if constexpr (Q8) {
+        const uint32_t qbytes = (uint32_t)ncache * HD, dbytes = kv_q8_d_bytes(ncache, HD);
+        mbar_expect_tx(bar_a, 2 * (qbytes + dbytes));
+        bulk_g2s(smem_u32(Kt), kh + (size_t)i0 * HD, qbytes, bar_a);
+        bulk_g2s(smem_u32(Kt) + kSplitKeys * HD, kdh + (size_t)i0 * (HD / kKvQ8Block), dbytes, bar_a);
+        bulk_g2s(smem_u32(Vt), vh + (size_t)i0 * HD, qbytes, bar_a);
+        bulk_g2s(smem_u32(Vt) + kSplitKeys * HD, vdh + (size_t)i0 * (HD / kKvQ8Block), dbytes, bar_a);
+      } else {
+        const uint32_t bytes = (uint32_t)ncache * HD * 2;
+        mbar_expect_tx(bar_a, 2 * bytes);
+        bulk_g2s(smem_u32(Kt), kh + (size_t)i0 * HD, bytes, bar_a);
+        bulk_g2s(smem_u32(Vt), vh + (size_t)i0 * HD, bytes, bar_a);
+      }
     }
   }
   __syncthreads();
@@ -414,6 +453,18 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
       if (wrapped) rope_angle(n_ctx, i, &sn, &cs);  // llama.cpp:353-354: the new k enters at n_ctx, shifted back below
       const float* kr = knew + (size_t)hk * HD;
       const float k0 = kr[2 * i], k1 = kr[2 * i + 1];
+      if constexpr (Q8) {  // threads < HD / 2 are whole warps; has_new is uniform over the CTA
+        const float* vr = vnew + (size_t)hk * HD;
+        const KvQ8Pair a = kv_q8_quant_pair(k0 * cs - k1 * sn, k0 * sn + k1 * cs), b = kv_q8_quant_pair(vr[2 * i], vr[2 * i + 1]);
+        sk[2 * i] = kv_q8_value(a.q0, a.d);
+        sk[2 * i + 1] = kv_q8_value(a.q1, a.d);
+        sv[2 * i] = kv_q8_value(b.q0, b.d);
+        sv[2 * i + 1] = kv_q8_value(b.q1, b.d);
+        if (h0 % group == 0) {
+          kv_q8_store_pair(kh + (size_t)pos * HD, kdh + (size_t)pos * (HD / kKvQ8Block), i, a);
+          kv_q8_store_pair(vh + (size_t)pos * HD, vdh + (size_t)pos * (HD / kKvQ8Block), i, b);
+        }
+      } else {
       const __half r0 = __float2half_rn(k0 * cs - k1 * sn), r1 = __float2half_rn(k0 * sn + k1 * cs);
       sk[2 * i] = __half2float(r0);
       sk[2 * i + 1] = __half2float(r1);
@@ -426,6 +477,7 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
       if (!wrapped && (RING || h0 % group == 0)) {
         *reinterpret_cast<__half2*>(kh + (size_t)pos * HD + 2 * i) = knew_h;
         *reinterpret_cast<__half2*>(vh + (size_t)pos * HD + 2 * i) = vnew_h;
+      }
       }
     }
   }
@@ -470,7 +522,11 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
   for (int e = 0; e < EPL; ++e) ql[e] = sq[lane * EPL + e];
   if (ncache > 0) mbar_wait(bar_a, 0);
   auto row = [&](const __half* base, int r, float* dst) {
-    if (EPL == 4) {
+    if constexpr (Q8) {  // base: the tile's space, codes [kSplitKeys][HD] then scales [kSplitKeys][HD / 32]
+      const int8_t* qt = reinterpret_cast<const int8_t*>(base);
+      const __half* dt = reinterpret_cast<const __half*>(qt + kSplitKeys * HD);
+      kv_q8_load<EPL>(qt + (size_t)r * HD + lane * EPL, dt[r * (HD / kKvQ8Block) + lane * EPL / kKvQ8Block], dst);
+    } else if (EPL == 4) {
       const uint2 u = *reinterpret_cast<const uint2*>(base + (size_t)r * HD + lane * 4);
       const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
       dst[0] = a.x, dst[1] = a.y, dst[2] = b.x, dst[3] = b.y;
@@ -608,6 +664,9 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
 // (tiles, n_head).  CTA x reads tiles[5 x] = {segment's first row, its length, its n_past, its KV block, the tile's first query row
 // inside the segment}, offsets q / out by the first row and kc / vc by the block, and takes pos0 = n_past, m = length.  Everything
 // after those offsets is the single-sequence code, so each segment is bit-identical to a launch of its own.
+//
+// KV = NS_KV_Q8_0: kc / vc are the code planes, kd / vd the scale planes (kv_cache.cuh); the tile loads write the dequantised
+// values fp16(q * d) into the same padded fp16 tiles, and everything after them is the fp16 kernel's.
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   const __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&h);
@@ -617,11 +676,13 @@ __device__ __forceinline__ void mma_f16_16816(float (&c)[4], const uint32_t (&a)
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-template <int HD, bool RAGGED = false>
-__global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__ q, int ldq, const __half* __restrict__ kc,
-                                                       const __half* __restrict__ vc, const int* __restrict__ state, float* __restrict__ out,
+template <int HD, bool RAGGED = false, int KV = NS_KV_F16>
+__global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__ q, int ldq, const kv_elem_t<KV>* __restrict__ kc,
+                                                       const kv_elem_t<KV>* __restrict__ vc, const int* __restrict__ state, float* __restrict__ out,
                                                        int ldo, int n_head, int n_head_kv, int n_ctx, int m, float scale,
-                                                       const int* __restrict__ tiles) {
+                                                       const int* __restrict__ tiles, const __half* __restrict__ kd,
+                                                       const __half* __restrict__ vd) {
+  constexpr bool Q8 = KV == NS_KV_Q8_0;
   constexpr int LD = HD + 8;  // halves per shared-memory row: 16 bytes of padding rotate the banks by 4 words per row
   constexpr int KS = HD / 16, NT = HD / 8;
   __shared__ __align__(16) __half Ks[kAttnMmaKeys * LD];
@@ -638,6 +699,10 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
     const size_t blk = (size_t)tl[3] * n_head_kv * n_ctx * HD;
     kc += blk;
     vc += blk;
+    if constexpr (Q8) {
+      kd += (size_t)tl[3] * n_head_kv * kv_d_stride(n_ctx, HD);
+      vd += (size_t)tl[3] * n_head_kv * kv_d_stride(n_ctx, HD);
+    }
     m = tl[1];
     pos0 = tl[2];
     q0 = tl[4];
@@ -647,8 +712,10 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
   }
   const int row0 = q0 + warp * 16 + g, row1 = row0 + 8;  // this thread's two query rows (token indices of the batch)
   const int total = min(pos0 + m, n_ctx);                // keys that exist
-  const __half* kh = kc + (size_t)hk * n_ctx * HD;
-  const __half* vh = vc + (size_t)hk * n_ctx * HD;
+  const kv_elem_t<KV>* kh = kc + (size_t)hk * n_ctx * HD;
+  const kv_elem_t<KV>* vh = vc + (size_t)hk * n_ctx * HD;
+  const __half* kdh = Q8 ? kd + (size_t)hk * kv_d_stride(n_ctx, HD) : nullptr;  // Q8_0: the head's scales
+  const __half* vdh = Q8 ? vd + (size_t)hk * kv_d_stride(n_ctx, HD) : nullptr;
 
   // Q A-fragments, rounded to fp16 as the reference's mul_mat does with src1 (rows past the batch: zeros)
   uint32_t qa[KS][4];
@@ -672,14 +739,19 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
   const int nkt = min(pos0 + last_row, total - 1) / kAttnMmaKeys + 1;  // key tiles this CTA needs
   const int warp_last_key = pos0 + q0 + warp * 16 + 15;                // beyond it every key is masked for the whole warp
 
-  auto load_tile = [&](const __half* base, __half* dst, int key0) {
+  auto load_tile = [&](const kv_elem_t<KV>* base, const __half* dbase, __half* dst, int key0) {
     constexpr int C16 = HD / 8;  // 16-byte chunks per row
 #pragma unroll
     for (int i = 0; i < kAttnMmaKeys * C16 / 128; ++i) {
       const int idx = i * 128 + (int)threadIdx.x;
       const int r = idx / C16, c = idx % C16;
       uint4 v = make_uint4(0u, 0u, 0u, 0u);
-      if (key0 + r < total) v = *reinterpret_cast<const uint4*>(base + (size_t)(key0 + r) * HD + c * 8);
+      if constexpr (Q8) {
+        if (key0 + r < total)
+          v = kv_q8_load8_h(base + (size_t)(key0 + r) * HD + c * 8, dbase[(size_t)(key0 + r) * (HD / kKvQ8Block) + c * 8 / kKvQ8Block]);
+      } else {
+        if (key0 + r < total) v = *reinterpret_cast<const uint4*>(base + (size_t)(key0 + r) * HD + c * 8);
+      }
       *reinterpret_cast<uint4*>(dst + r * LD + c * 8) = v;
     }
   };
@@ -701,7 +773,7 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
   float mx0 = -INFINITY, mx1 = -INFINITY;
   for (int kt = 0; kt < nkt; ++kt) {
     __syncthreads();
-    load_tile(kh, Ks, kt * kAttnMmaKeys);
+    load_tile(kh, kdh, Ks, kt * kAttnMmaKeys);
     __syncthreads();
     if (kt * kAttnMmaKeys > warp_last_key) continue;
     float s[8][4];
@@ -734,8 +806,8 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
   float l0 = 0.f, l1 = 0.f;
   for (int kt = 0; kt < nkt; ++kt) {
     __syncthreads();
-    load_tile(kh, Ks, kt * kAttnMmaKeys);
-    load_tile(vh, Vs, kt * kAttnMmaKeys);
+    load_tile(kh, kdh, Ks, kt * kAttnMmaKeys);
+    load_tile(vh, vdh, Vs, kt * kAttnMmaKeys);
     __syncthreads();
     if (kt * kAttnMmaKeys > warp_last_key) continue;
     float s[8][4];
@@ -794,14 +866,42 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
 //   hd 64 / 128, >= 8 rows  rope_kv_kernel + attn_mma_kernel unless NS_ATTN_SCALAR is set
 //   hd 64 / 128, otherwise  rope_kv_kernel + attn_fast_kernel
 //   any other (even) hd     rope_kv_kernel + attn_kernel
+// A Q8_0 cache (kv_cache.cuh) takes the split decode attention for one row and rope_kv_kernel + attn_mma_kernel for more, at head
+// sizes 64 / 128; attn_fast_kernel and attn_kernel have no Q8_0 form.
 
 static size_t attn_generic_smem(int hd, int n_ctx) { return (size_t)(hd + n_ctx) * sizeof(float); }
 extern size_t attn_rows_smem(int hd, int n_ctx) { return (size_t)((3 + kAW) * hd + n_ctx) * sizeof(float); }
 extern int attn_ranges(int n_ctx) { return (n_ctx + kSplitKeys - 1) / kSplitKeys; }
 
-// the kernel `kind` resolves to for this shape, or NS_E_UNSUPPORTED when a forced kernel cannot take it
-static int attn_resolve(int kind, int hd, int m, int n_ctx) {
+// the Q8_0 cache's kernel for `kind`, or NS_E_UNSUPPORTED
+static int attn_resolve_q8(int kind, int hd, int m, int n_ctx) {
+  if (hd != 64 && hd != 128) {
+    ns_set_error("ns_llama: the Q8_0 KV cache needs head size 64 or 128, got %d", hd);
+    return NS_E_UNSUPPORTED;
+  }
+  if (kind == NS_ATTN_AUTO) {
+    if (getenv("NS_ATTN_OLD_DECODE") || getenv("NS_ATTN_SCALAR")) {
+      ns_set_error("ns_llama: NS_ATTN_OLD_DECODE / NS_ATTN_SCALAR select kernels without a Q8_0 KV form");
+      return NS_E_UNSUPPORTED;
+    }
+    kind = m == 1 ? NS_ATTN_SPLIT_DECODE : NS_ATTN_MMA;
+  }
+  if (kind == NS_ATTN_ROWS || kind == NS_ATTN_GENERIC) {
+    ns_set_error("ns_llama: attention kernel %d has no Q8_0 KV form (NS_ATTN_SPLIT_DECODE / NS_ATTN_MMA read Q8_0)", kind);
+    return NS_E_UNSUPPORTED;
+  }
+  if (kind == NS_ATTN_SPLIT_DECODE && attn_ranges(n_ctx) > 1024) {
+    ns_set_error("ns_llama: n_ctx %d too large for the split decode attention over a Q8_0 KV cache", n_ctx);
+    return NS_E_UNSUPPORTED;
+  }
+  return kind;
+}
+
+// the kernel `kind` resolves to for this shape and cache format, or NS_E_UNSUPPORTED when a forced kernel cannot take it
+static int attn_resolve(int kind, int hd, int m, int n_ctx, int kv = NS_KV_F16) {
   const bool fast = hd == 128 || hd == 64;
+  if (kv == NS_KV_Q8_0 && kind >= NS_ATTN_AUTO && kind <= NS_ATTN_GENERIC) kind = attn_resolve_q8(kind, hd, m, n_ctx);
+  if (kind < 0) return kind;
   if (kind == NS_ATTN_AUTO) {
     // debugging aids, read per call (not per process) so that a test can compare kernels on one engine
     const bool old_decode = getenv("NS_ATTN_OLD_DECODE") != nullptr;  // decode attention: one CTA per head, dependent row loads
@@ -853,11 +953,19 @@ static int grant_decode_smem(AttnAttr& attr) {
                                    (int)attn_decode_smem<128>()));
   NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    (int)attn_decode_smem<64>()));
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128, false, false, NS_KV_Q8_0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)attn_decode_smem<128>()));
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, false, false, NS_KV_Q8_0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)attn_decode_smem<64>()));
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<128, false, true, NS_KV_Q8_0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)attn_decode_smem<128>()));
+  NS_CUDA_TRY(cudaFuncSetAttribute(attn_decode_kernel<64, false, true, NS_KV_Q8_0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)attn_decode_smem<64>()));
   attr.decode = true;
   return NS_OK;
 }
 
-extern int launch_attention_batch(const float* q, const float* k, const float* v, __half* kc, __half* vc, const int* rstate,
+extern int launch_attention_batch(const float* q, const float* k, const float* v, const KvPtrs& kv, const int* rstate,
                                   const int* seqs, float* out, float* part, unsigned* tickets, int n, int n_head, int n_head_kv, int hd,
                                   int n_ctx, float rope_theta, float rope_scale, AttnAttr& attr, cudaStream_t st) {
   if (hd != 64 && hd != 128) {
@@ -869,21 +977,35 @@ extern int launch_attention_batch(const float* q, const float* k, const float* v
   const float freq_scale = 1.f / rope_scale;
   const float attn_scale = 1.0f / sqrtf((float)hd);
   const int nsplit = attn_ranges(n_ctx);
-  auto kern = hd == 128 ? attn_decode_kernel<128, false, true> : attn_decode_kernel<64, false, true>;
-  NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)n_head, (unsigned)nsplit, (unsigned)n), dim3(kDW * 32),
-                            hd == 128 ? attn_decode_smem<128>() : attn_decode_smem<64>(), st, q, k,
-                            v, kc, vc, rstate, out, part, tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale, theta_scale, freq_scale,
-                            -1, ShiftTable{}, seqs));
+  const dim3 grid((unsigned)n_head, (unsigned)nsplit, (unsigned)n);
+  const size_t dsm = hd == 128 ? attn_decode_smem<128>() : attn_decode_smem<64>();
+  if (kv.type == NS_KV_Q8_0) {
+    auto kern = hd == 128 ? attn_decode_kernel<128, false, true, NS_KV_Q8_0> : attn_decode_kernel<64, false, true, NS_KV_Q8_0>;
+    NS_CUDA_TRY(ns_launch_pdl(kern, grid, dim3(kDW * 32), dsm, st, q, k, v, static_cast<int8_t*>(kv.k), static_cast<int8_t*>(kv.v), rstate,
+                              out, part, tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale, theta_scale, freq_scale, -1, ShiftTable{},
+                              seqs, kv.kd, kv.vd));
+  } else {
+    auto kern = hd == 128 ? attn_decode_kernel<128, false, true> : attn_decode_kernel<64, false, true>;
+    NS_CUDA_TRY(ns_launch_pdl(kern, grid, dim3(kDW * 32), dsm, st, q, k, v, static_cast<__half*>(kv.k), static_cast<__half*>(kv.v), rstate,
+                              out, part, tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale, theta_scale, freq_scale, -1, ShiftTable{},
+                              seqs, (__half*)nullptr, (__half*)nullptr));
+  }
   ns_count_launch();
   return NS_OK;
 }
 
-extern int launch_attention(int kind, float* q, const float* k, const float* v, __half* kc, __half* vc, const int* state, float* out,
+extern int launch_attention(int kind, float* q, const float* k, const float* v, const KvPtrs& kv, const int* state, float* out,
                             float* part, unsigned* tickets, int n_head, int n_head_kv, int hd, int n_ctx, int m, float rope_theta,
                             float rope_scale, AttnAttr& attr, cudaStream_t st, const Ring* ring = nullptr) {
+  if (ring && kv.type != NS_KV_F16) {
+    ns_set_error("ns_llama: the streaming ring shifts an fp16 KV cache only");
+    return NS_E_UNSUPPORTED;
+  }
   if (ring && m == 1) kind = NS_ATTN_SPLIT_DECODE;  // the only kernel that carries the shift
-  kind = attn_resolve(kind, hd, m, n_ctx);
+  kind = attn_resolve(kind, hd, m, n_ctx, kv.type);
   if (kind < 0) return kind;
+  __half* kc = static_cast<__half*>(kv.k);
+  __half* vc = static_cast<__half*>(kv.v);
   const int ldq = n_head * hd, ldk = n_head_kv * hd;
   const float theta_scale = powf(rope_theta, -2.0f / (float)hd);  // n_rot == head_size (llama.cpp:131)
   const float freq_scale = 1.f / rope_scale;  // the angle is divided by hparams.freq_scale (ne_layers.c:9263, 9207)
@@ -904,9 +1026,16 @@ extern int launch_attention(int kind, float* q, const float* k, const float* v, 
     auto kern = ring ? (hd == 128 ? attn_decode_kernel<128, true> : attn_decode_kernel<64, true>)
                      : (hd == 128 ? attn_decode_kernel<128, false> : attn_decode_kernel<64, false>);
     const unsigned gx = (unsigned)(ring ? n_head_kv : n_head);  // ring: one CTA per (kv head, range)
-    NS_CUDA_TRY(ns_launch_pdl(kern, dim3(gx, (unsigned)nsplit), dim3(kDW * 32), dsm, st, (const float*)q, k, v, kc, vc, state, out, part,
-                              tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale, theta_scale, freq_scale, ring ? ring->n_keep : -1,
-                              ring ? ring->tab : ShiftTable{}, (const int*)nullptr));
+    if (kv.type == NS_KV_Q8_0) {
+      auto qk = hd == 128 ? attn_decode_kernel<128, false, false, NS_KV_Q8_0> : attn_decode_kernel<64, false, false, NS_KV_Q8_0>;
+      NS_CUDA_TRY(ns_launch_pdl(qk, dim3(gx, (unsigned)nsplit), dim3(kDW * 32), dsm, st, (const float*)q, k, v, static_cast<int8_t*>(kv.k),
+                                static_cast<int8_t*>(kv.v), state, out, part, tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale,
+                                theta_scale, freq_scale, -1, ShiftTable{}, (const int*)nullptr, kv.kd, kv.vd));
+    } else {
+      NS_CUDA_TRY(ns_launch_pdl(kern, dim3(gx, (unsigned)nsplit), dim3(kDW * 32), dsm, st, (const float*)q, k, v, kc, vc, state, out, part,
+                                tickets, n_head, n_head_kv, n_ctx, nsplit, attn_scale, theta_scale, freq_scale, ring ? ring->n_keep : -1,
+                                ring ? ring->tab : ShiftTable{}, (const int*)nullptr, (__half*)nullptr, (__half*)nullptr));
+    }
     ns_count_launch();
     return NS_OK;
   }
@@ -917,14 +1046,27 @@ extern int launch_attention(int kind, float* q, const float* k, const float* v, 
     ns_count_launch();
     return NS_OK;
   }
+  if (kv.type == NS_KV_Q8_0) {  // attn_resolve left NS_ATTN_MMA
+    NS_CUDA_TRY(ns_launch_pdl(rope_kv_kernel<false, NS_KV_Q8_0>, dim3((unsigned)(n_head + n_head_kv), (unsigned)m), dim3((unsigned)(hd / 2)),
+                              0, st, q, ldq, k, ldk, v, ldk, static_cast<int8_t*>(kv.k), static_cast<int8_t*>(kv.v), state, n_head, n_head_kv,
+                              hd, n_ctx, theta_scale, freq_scale, (const int*)nullptr, kv.kd, kv.vd));
+    ns_count_launch();
+    auto kern = hd == 128 ? attn_mma_kernel<128, false, NS_KV_Q8_0> : attn_mma_kernel<64, false, NS_KV_Q8_0>;
+    NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)((m + kAttnMmaRows - 1) / kAttnMmaRows), (unsigned)n_head), dim3(128), 0, st,
+                              (const float*)q, ldq, static_cast<const int8_t*>(kv.k), static_cast<const int8_t*>(kv.v), state, out, ldq,
+                              n_head, n_head_kv, n_ctx, m, attn_scale, (const int*)nullptr, (const __half*)kv.kd, (const __half*)kv.vd));
+    ns_count_launch();
+    return NS_OK;
+  }
   NS_CUDA_TRY(ns_launch_pdl(rope_kv_kernel<false>, dim3((unsigned)(n_head + n_head_kv), (unsigned)m), dim3((unsigned)(hd / 2)), 0, st, q,
-                            ldq, k, ldk, v, ldk, kc, vc, state, n_head, n_head_kv, hd, n_ctx, theta_scale, freq_scale, (const int*)nullptr));
+                            ldq, k, ldk, v, ldk, kc, vc, state, n_head, n_head_kv, hd, n_ctx, theta_scale, freq_scale, (const int*)nullptr,
+                            (__half*)nullptr, (__half*)nullptr));
   ns_count_launch();
   if (kind == NS_ATTN_MMA) {  // causal attention on the tensor cores, 64 query rows per CTA
     auto kern = hd == 128 ? attn_mma_kernel<128> : attn_mma_kernel<64>;
     NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)((m + kAttnMmaRows - 1) / kAttnMmaRows), (unsigned)n_head), dim3(128), 0, st,
                               (const float*)q, ldq, (const __half*)kc, (const __half*)vc, state, out, ldq, n_head, n_head_kv, n_ctx, m,
-                              attn_scale, (const int*)nullptr));
+                              attn_scale, (const int*)nullptr, (const __half*)nullptr, (const __half*)nullptr));
   } else if (kind == NS_ATTN_ROWS) {
     auto kern = hd == 128 ? attn_fast_kernel<128, false> : attn_fast_kernel<64, false>;
     NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)n_head, (unsigned)m), dim3(kAW * 32), rows_smem, st, (const float*)q, ldq, k, ldk, v, ldk,
@@ -952,26 +1094,55 @@ extern "C" size_t ns_llama_attention_workspace_bytes(int n_head, int hd, int n_c
   return attn_ws_part_offset(n_head) + (size_t)n_head * attn_ranges(n_ctx) * (hd + 2) * sizeof(float);
 }
 
-extern "C" int ns_llama_attention(int kernel, float* q, const float* k, const float* v, void* kc, void* vc, int n_head, int n_head_kv,
-                                  int hd, int n_ctx, int n_past, int m, float rope_theta, float rope_scale, float* out, void* ws,
-                                  void* queue) {
+static int attention_entry(const char* who, int kernel, float* q, const float* k, const float* v, const KvPtrs& kv, int n_head,
+                           int n_head_kv, int hd, int n_ctx, int n_past, int m, float rope_theta, float rope_scale, float* out, void* ws,
+                           void* queue) {
   if (int rc = ns_ensure_device()) return rc;
-  if (!q || !k || !v || !kc || !vc || !out || !ws || n_head <= 0 || n_head_kv <= 0 || n_head % n_head_kv || hd <= 0 || hd % 2 ||
-      n_ctx <= 0 || m <= 0 || n_past < 0 || n_past + m > n_ctx || !(rope_theta > 0.f) || !(rope_scale > 0.f)) {
-    ns_set_error("ns_llama_attention: invalid arguments (n_head=%d n_head_kv=%d hd=%d n_ctx=%d n_past=%d m=%d)", n_head, n_head_kv, hd,
-                 n_ctx, n_past, m);
+  if (!q || !k || !v || !kv.k || !kv.v || (kv.type == NS_KV_Q8_0 && (!kv.kd || !kv.vd)) || !out || !ws || n_head <= 0 || n_head_kv <= 0 ||
+      n_head % n_head_kv || hd <= 0 || hd % 2 || n_ctx <= 0 || m <= 0 || n_past < 0 || n_past + m > n_ctx || !(rope_theta > 0.f) ||
+      !(rope_scale > 0.f)) {
+    ns_set_error("%s: invalid arguments (n_head=%d n_head_kv=%d hd=%d n_ctx=%d n_past=%d m=%d)", who, n_head, n_head_kv, hd, n_ctx, n_past, m);
     return NS_E_INVALID;
   }
-  if (int rc = attn_resolve(kernel, hd, m, n_ctx); rc < 0) return rc;
+  if (int rc = attn_resolve(kernel, hd, m, n_ctx, kv.type); rc < 0) return rc;
   cudaStream_t st = ns_stream_of(queue);
   char* w = static_cast<char*>(ws);
   const int state[4] = {0, n_past, 0, 0};
   NS_CUDA_TRY(cudaMemcpyAsync(w, state, sizeof(state), cudaMemcpyHostToDevice, st));  // pageable source: staged before the call returns
   AttnAttr attr;
-  return launch_attention(kernel, q, k, v, static_cast<__half*>(kc), static_cast<__half*>(vc), reinterpret_cast<const int*>(w), out,
-                          reinterpret_cast<float*>(w + attn_ws_part_offset(n_head)),
+  return launch_attention(kernel, q, k, v, kv, reinterpret_cast<const int*>(w), out, reinterpret_cast<float*>(w + attn_ws_part_offset(n_head)),
                           reinterpret_cast<unsigned*>(w + attn_ws_tickets_offset()), n_head, n_head_kv, hd, n_ctx, m, rope_theta,
                           rope_scale, attr, st);
+}
+
+static KvPtrs f16_planes(void* kc, void* vc) {
+  KvPtrs p;
+  p.k = kc;
+  p.v = vc;
+  return p;
+}
+static KvPtrs q8_planes(void* kq, void* kd, void* vq, void* vd) {
+  KvPtrs p;
+  p.type = NS_KV_Q8_0;
+  p.k = kq;
+  p.v = vq;
+  p.kd = static_cast<__half*>(kd);
+  p.vd = static_cast<__half*>(vd);
+  return p;
+}
+
+extern "C" int ns_llama_attention(int kernel, float* q, const float* k, const float* v, void* kc, void* vc, int n_head, int n_head_kv,
+                                  int hd, int n_ctx, int n_past, int m, float rope_theta, float rope_scale, float* out, void* ws,
+                                  void* queue) {
+  return attention_entry("ns_llama_attention", kernel, q, k, v, f16_planes(kc, vc), n_head, n_head_kv, hd, n_ctx, n_past, m, rope_theta,
+                         rope_scale, out, ws, queue);
+}
+
+extern "C" int ns_llama_attention_q8_0(int kernel, float* q, const float* k, const float* v, void* kq, void* kd, void* vq, void* vd,
+                                       int n_head, int n_head_kv, int hd, int n_ctx, int n_past, int m, float rope_theta, float rope_scale,
+                                       float* out, void* ws, void* queue) {
+  return attention_entry("ns_llama_attention_q8_0", kernel, q, k, v, q8_planes(kq, kd, vq, vd), n_head, n_head_kv, hd, n_ctx, n_past, m,
+                         rope_theta, rope_scale, out, ws, queue);
 }
 
 extern "C" int ns_llama_attention_ring(float* q, const float* k, const float* v, void* kc, void* vc, int n_head, int n_head_kv, int hd,
@@ -990,8 +1161,7 @@ extern "C" int ns_llama_attention_ring(float* q, const float* k, const float* v,
   NS_CUDA_TRY(cudaMemcpyAsync(w, state, sizeof(state), cudaMemcpyHostToDevice, st));  // pageable source: staged before the call returns
   AttnAttr attr;
   const Ring ring{n_keep, shift_table(hd, rope_theta)};
-  return launch_attention(NS_ATTN_SPLIT_DECODE, q, k, v, static_cast<__half*>(kc), static_cast<__half*>(vc), reinterpret_cast<const int*>(w),
-                          out, reinterpret_cast<float*>(w + attn_ws_part_offset(n_head)),
+  return launch_attention(NS_ATTN_SPLIT_DECODE, q, k, v, f16_planes(kc, vc), reinterpret_cast<const int*>(w), out, reinterpret_cast<float*>(w + attn_ws_part_offset(n_head)),
                           reinterpret_cast<unsigned*>(w + attn_ws_tickets_offset()), n_head, n_head_kv, hd, n_ctx, 1, rope_theta, 1.f, attr,
                           st, &ring);
 }
@@ -1033,19 +1203,19 @@ extern "C" size_t ns_llama_attention_batch_workspace_bytes(int n, int n_head, in
   return attnb_ws_part_offset(n, n_head) + (size_t)n * n_head * attn_ranges(n_ctx) * (hd + 2) * sizeof(float);
 }
 
-extern "C" int ns_llama_attention_batch(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n, const int* seq,
-                                        const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx, float rope_theta,
-                                        float rope_scale, float* out, void* ws, void* queue) {
+static int attention_batch_entry(const char* who, float* q, const float* k, const float* v, const KvPtrs& kv, int n_seq, int n,
+                                 const int* seq, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx, float rope_theta,
+                                 float rope_scale, float* out, void* ws, void* queue) {
   if (int rc = ns_ensure_device()) return rc;
-  if (!q || !k || !v || !kc || !vc || !seq || !n_past || !out || !ws || n_seq < 1 || n_seq > 32 || n_head <= 0 || n_head_kv <= 0 ||
-      n_head % n_head_kv || hd <= 0 || hd % 2 || n_ctx <= 0 || !(rope_theta > 0.f) || !(rope_scale > 0.f)) {
-    ns_set_error("ns_llama_attention_batch: invalid arguments (n_seq=%d n=%d n_head=%d n_head_kv=%d hd=%d n_ctx=%d)", n_seq, n, n_head,
-                 n_head_kv, hd, n_ctx);
+  if (!q || !k || !v || !kv.k || !kv.v || (kv.type == NS_KV_Q8_0 && (!kv.kd || !kv.vd)) || !seq || !n_past || !out || !ws || n_seq < 1 ||
+      n_seq > 32 || n_head <= 0 || n_head_kv <= 0 || n_head % n_head_kv || hd <= 0 || hd % 2 || n_ctx <= 0 || !(rope_theta > 0.f) ||
+      !(rope_scale > 0.f)) {
+    ns_set_error("%s: invalid arguments (n_seq=%d n=%d n_head=%d n_head_kv=%d hd=%d n_ctx=%d)", who, n_seq, n, n_head, n_head_kv, hd, n_ctx);
     return NS_E_INVALID;
   }
-  if (int rc = check_rows("ns_llama_attention_batch", n_seq, n, seq, n_past, 1, n_ctx)) return rc;
+  if (int rc = check_rows(who, n_seq, n, seq, n_past, 1, n_ctx)) return rc;
   if (hd != 64 && hd != 128) {
-    ns_set_error("ns_llama_attention_batch: head size %d (the batched decode attention takes 64 or 128)", hd);
+    ns_set_error("%s: head size %d (the batched decode attention takes 64 or 128)", who, hd);
     return NS_E_UNSUPPORTED;
   }
   cudaStream_t st = ns_stream_of(queue);
@@ -1057,11 +1227,24 @@ extern "C" int ns_llama_attention_batch(float* q, const float* k, const float* v
   }
   NS_CUDA_TRY(cudaMemcpyAsync(w, rows.data(), rows.size() * sizeof(int), cudaMemcpyHostToDevice, st));  // pageable: staged now
   AttnAttr attr;
-  return launch_attention_batch(q, k, v, static_cast<__half*>(kc), static_cast<__half*>(vc), reinterpret_cast<const int*>(w),
-                                reinterpret_cast<const int*>(w + attnb_ws_seq_offset(n)), out,
+  return launch_attention_batch(q, k, v, kv, reinterpret_cast<const int*>(w), reinterpret_cast<const int*>(w + attnb_ws_seq_offset(n)), out,
                                 reinterpret_cast<float*>(w + attnb_ws_part_offset(n, n_head)),
                                 reinterpret_cast<unsigned*>(w + attnb_ws_tickets_offset(n)), n, n_head, n_head_kv, hd, n_ctx, rope_theta,
                                 rope_scale, attr, st);
+}
+
+extern "C" int ns_llama_attention_batch(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n, const int* seq,
+                                        const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx, float rope_theta,
+                                        float rope_scale, float* out, void* ws, void* queue) {
+  return attention_batch_entry("ns_llama_attention_batch", q, k, v, f16_planes(kc, vc), n_seq, n, seq, n_past, n_head, n_head_kv, hd, n_ctx,
+                               rope_theta, rope_scale, out, ws, queue);
+}
+
+extern "C" int ns_llama_attention_batch_q8_0(float* q, const float* k, const float* v, void* kq, void* kd, void* vq, void* vd, int n_seq,
+                                             int n, const int* seq, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
+                                             float rope_theta, float rope_scale, float* out, void* ws, void* queue) {
+  return attention_batch_entry("ns_llama_attention_batch_q8_0", q, k, v, q8_planes(kq, kd, vq, vd), n_seq, n, seq, n_past, n_head, n_head_kv,
+                               hd, n_ctx, rope_theta, rope_scale, out, ws, queue);
 }
 
 // ---- mixed batches: token segments of several sequences in one pass (ns_llama_eval_batch) ------------------------------------
@@ -1148,7 +1331,7 @@ extern "C" int ns_llama_batch_plan(int n_seq, int n_ctx, int n, const int* seq, 
   return NS_OK;
 }
 
-extern int launch_attention_ragged(float* q, const float* k, const float* v, __half* kc, __half* vc, const int* rows, const int* tiles,
+extern int launch_attention_ragged(float* q, const float* k, const float* v, const KvPtrs& kv, const int* rows, const int* tiles,
                                    int n_rows, int n_tiles, float* out, int n_head, int n_head_kv, int hd, int n_ctx, float rope_theta,
                                    float rope_scale, cudaStream_t st) {
   if (hd != 64 && hd != 128) {
@@ -1159,13 +1342,27 @@ extern int launch_attention_ragged(float* q, const float* k, const float* v, __h
   const float theta_scale = powf(rope_theta, -2.0f / (float)hd);  // as launch_attention
   const float freq_scale = 1.f / rope_scale;
   const float attn_scale = 1.0f / sqrtf((float)hd);
-  NS_CUDA_TRY(ns_launch_pdl(rope_kv_kernel<true>, dim3((unsigned)(n_head + n_head_kv), (unsigned)n_rows), dim3((unsigned)(hd / 2)), 0, st,
-                            q, ldq, k, ldk, v, ldk, kc, vc, (const int*)nullptr, n_head, n_head_kv, hd, n_ctx, theta_scale, freq_scale,
-                            rows));
+  const dim3 rgrid((unsigned)(n_head + n_head_kv), (unsigned)n_rows), mgrid((unsigned)n_tiles, (unsigned)n_head);
+  if (kv.type == NS_KV_Q8_0) {
+    int8_t* kc = static_cast<int8_t*>(kv.k);
+    int8_t* vc = static_cast<int8_t*>(kv.v);
+    NS_CUDA_TRY(ns_launch_pdl(rope_kv_kernel<true, NS_KV_Q8_0>, rgrid, dim3((unsigned)(hd / 2)), 0, st, q, ldq, k, ldk, v, ldk, kc, vc,
+                              (const int*)nullptr, n_head, n_head_kv, hd, n_ctx, theta_scale, freq_scale, rows, kv.kd, kv.vd));
+    ns_count_launch();
+    auto kern = hd == 128 ? attn_mma_kernel<128, true, NS_KV_Q8_0> : attn_mma_kernel<64, true, NS_KV_Q8_0>;
+    NS_CUDA_TRY(ns_launch_pdl(kern, mgrid, dim3(128), 0, st, (const float*)q, ldq, (const int8_t*)kc, (const int8_t*)vc, (const int*)nullptr,
+                              out, ldq, n_head, n_head_kv, n_ctx, 0, attn_scale, tiles, (const __half*)kv.kd, (const __half*)kv.vd));
+    ns_count_launch();
+    return NS_OK;
+  }
+  __half* kc = static_cast<__half*>(kv.k);
+  __half* vc = static_cast<__half*>(kv.v);
+  NS_CUDA_TRY(ns_launch_pdl(rope_kv_kernel<true>, rgrid, dim3((unsigned)(hd / 2)), 0, st, q, ldq, k, ldk, v, ldk, kc, vc, (const int*)nullptr,
+                            n_head, n_head_kv, hd, n_ctx, theta_scale, freq_scale, rows, (__half*)nullptr, (__half*)nullptr));
   ns_count_launch();
   auto kern = hd == 128 ? attn_mma_kernel<128, true> : attn_mma_kernel<64, true>;
-  NS_CUDA_TRY(ns_launch_pdl(kern, dim3((unsigned)n_tiles, (unsigned)n_head), dim3(128), 0, st, (const float*)q, ldq, (const __half*)kc,
-                            (const __half*)vc, (const int*)nullptr, out, ldq, n_head, n_head_kv, n_ctx, 0, attn_scale, tiles));
+  NS_CUDA_TRY(ns_launch_pdl(kern, mgrid, dim3(128), 0, st, (const float*)q, ldq, (const __half*)kc, (const __half*)vc, (const int*)nullptr,
+                            out, ldq, n_head, n_head_kv, n_ctx, 0, attn_scale, tiles, (const __half*)nullptr, (const __half*)nullptr));
   ns_count_launch();
   return NS_OK;
 }
@@ -1176,20 +1373,19 @@ extern "C" size_t ns_llama_attention_ragged_workspace_bytes(int n, int n_rows) {
   return ((size_t)2 * n_rows + (size_t)(n_rows / kAttnMmaRows + n) * kTileInts) * sizeof(int);
 }
 
-extern "C" int ns_llama_attention_ragged(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n, const int* seq,
-                                         const int* n_tokens, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
-                                         float rope_theta, float rope_scale, float* out, void* ws, void* queue) {
+static int attention_ragged_entry(const char* who, float* q, const float* k, const float* v, const KvPtrs& kv, int n_seq, int n,
+                                  const int* seq, const int* n_tokens, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
+                                  float rope_theta, float rope_scale, float* out, void* ws, void* queue) {
   if (int rc = ns_ensure_device()) return rc;
-  if (!q || !k || !v || !kc || !vc || !out || !ws || n_seq < 1 || n_seq > 32 || n_head <= 0 || n_head_kv <= 0 || n_head % n_head_kv ||
-      hd <= 0 || hd % 2 || n_ctx <= 0 || !(rope_theta > 0.f) || !(rope_scale > 0.f)) {
-    ns_set_error("ns_llama_attention_ragged: invalid arguments (n_seq=%d n=%d n_head=%d n_head_kv=%d hd=%d n_ctx=%d)", n_seq, n, n_head,
-                 n_head_kv, hd, n_ctx);
+  if (!q || !k || !v || !kv.k || !kv.v || (kv.type == NS_KV_Q8_0 && (!kv.kd || !kv.vd)) || !out || !ws || n_seq < 1 || n_seq > 32 ||
+      n_head <= 0 || n_head_kv <= 0 || n_head % n_head_kv || hd <= 0 || hd % 2 || n_ctx <= 0 || !(rope_theta > 0.f) || !(rope_scale > 0.f)) {
+    ns_set_error("%s: invalid arguments (n_seq=%d n=%d n_head=%d n_head_kv=%d hd=%d n_ctx=%d)", who, n_seq, n, n_head, n_head_kv, hd, n_ctx);
     return NS_E_INVALID;
   }
   int n_rows = 0;
-  if (int rc = check_segments("ns_llama_attention_ragged", n_seq, n_ctx, n, seq, n_tokens, n_past, &n_rows)) return rc;
+  if (int rc = check_segments(who, n_seq, n_ctx, n, seq, n_tokens, n_past, &n_rows)) return rc;
   if (hd != 64 && hd != 128) {
-    ns_set_error("ns_llama_attention_ragged: head size %d (the ragged prompt attention takes 64 or 128)", hd);
+    ns_set_error("%s: head size %d (the ragged prompt attention takes 64 or 128)", who, hd);
     return NS_E_UNSUPPORTED;
   }
   std::vector<int> order(n), first, rows, tiles;
@@ -1200,7 +1396,20 @@ extern "C" int ns_llama_attention_ragged(float* q, const float* k, const float* 
   // pageable sources: staged before the calls return
   NS_CUDA_TRY(cudaMemcpyAsync(w, rows.data(), rows.size() * sizeof(int), cudaMemcpyHostToDevice, st));
   NS_CUDA_TRY(cudaMemcpyAsync(w + (size_t)2 * n_rows * sizeof(int), tiles.data(), tiles.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  return launch_attention_ragged(q, k, v, static_cast<__half*>(kc), static_cast<__half*>(vc), reinterpret_cast<const int*>(w),
-                                 reinterpret_cast<const int*>(w + (size_t)2 * n_rows * sizeof(int)), n_rows, (int)tiles.size() / kTileInts,
-                                 out, n_head, n_head_kv, hd, n_ctx, rope_theta, rope_scale, st);
+  return launch_attention_ragged(q, k, v, kv, reinterpret_cast<const int*>(w), reinterpret_cast<const int*>(w + (size_t)2 * n_rows * sizeof(int)),
+                                 n_rows, (int)tiles.size() / kTileInts, out, n_head, n_head_kv, hd, n_ctx, rope_theta, rope_scale, st);
+}
+
+extern "C" int ns_llama_attention_ragged(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n, const int* seq,
+                                         const int* n_tokens, const int* n_past, int n_head, int n_head_kv, int hd, int n_ctx,
+                                         float rope_theta, float rope_scale, float* out, void* ws, void* queue) {
+  return attention_ragged_entry("ns_llama_attention_ragged", q, k, v, f16_planes(kc, vc), n_seq, n, seq, n_tokens, n_past, n_head, n_head_kv,
+                                hd, n_ctx, rope_theta, rope_scale, out, ws, queue);
+}
+
+extern "C" int ns_llama_attention_ragged_q8_0(float* q, const float* k, const float* v, void* kq, void* kd, void* vq, void* vd, int n_seq,
+                                              int n, const int* seq, const int* n_tokens, const int* n_past, int n_head, int n_head_kv,
+                                              int hd, int n_ctx, float rope_theta, float rope_scale, float* out, void* ws, void* queue) {
+  return attention_ragged_entry("ns_llama_attention_ragged_q8_0", q, k, v, q8_planes(kq, kd, vq, vd), n_seq, n, seq, n_tokens, n_past,
+                                n_head, n_head_kv, hd, n_ctx, rope_theta, rope_scale, out, ws, queue);
 }

@@ -5,6 +5,7 @@
 
 #include <vector>
 
+#include "kv_cache.cuh"
 #include "nsb.cuh"
 
 constexpr int kMaxSeq = 32;  // KV blocks of one context (ns_llama_set_sequences)
@@ -32,20 +33,21 @@ struct Ring {
   int n_keep;
   ShiftTable tab;
 };
-int launch_attention(int kind, float* q, const float* k, const float* v, __half* kc, __half* vc, const int* state, float* out,
+// kv: the layer's caches of the sequence's block (kv_cache.cuh)
+int launch_attention(int kind, float* q, const float* k, const float* v, const KvPtrs& kv, const int* state, float* out,
                      float* part, unsigned* tickets, int n_head, int n_head_kv, int hd, int n_ctx, int m, float rope_theta,
                      float rope_scale, AttnAttr& attr, cudaStream_t st, const Ring* ring);
 
 // Batched decode attention: one new token for each of n sequences, one launch (attn_decode_kernel<HD, false, true>).  rstate:
-// [n][4] row states (n_past in slot 1), seqs [n] KV block per row, caches [n_seq][n_head_kv][n_ctx][hd] fp16, q / out
+// [n][4] row states (n_past in slot 1), seqs [n] KV block per row, caches from the layer's block 0 on, q / out
 // [n][n_head * hd], k / v [n][n_head_kv * hd], part [n][n_head][ranges][hd + 2], tickets [n][n_head].  hd 64 / 128 only.
-int launch_attention_batch(const float* q, const float* k, const float* v, __half* kc, __half* vc, const int* rstate,
+int launch_attention_batch(const float* q, const float* k, const float* v, const KvPtrs& kv, const int* rstate,
                            const int* seqs, float* out, float* part, unsigned* tickets, int n, int n_head, int n_head_kv, int hd,
                            int n_ctx, float rope_theta, float rope_scale, AttnAttr& attr, cudaStream_t st);
 
 // Ragged prompt attention: RoPE + KV append of n_rows rows (rows [n_rows][2] = {position, block}), then attn_mma_kernel<RAGGED> over
-// n_tiles tile entries.  q / out [n_rows][n_head * hd], k / v [n_rows][n_head_kv * hd], caches [n_seq][n_head_kv][n_ctx][hd] fp16.
-int launch_attention_ragged(float* q, const float* k, const float* v, __half* kc, __half* vc, const int* rows, const int* tiles,
+// n_tiles tile entries.  q / out [n_rows][n_head * hd], k / v [n_rows][n_head_kv * hd], caches from the layer's block 0 on.
+int launch_attention_ragged(float* q, const float* k, const float* v, const KvPtrs& kv, const int* rows, const int* tiles,
                             int n_rows, int n_tiles, float* out, int n_head, int n_head_kv, int hd, int n_ctx, float rope_theta,
                             float rope_scale, cudaStream_t st);
 

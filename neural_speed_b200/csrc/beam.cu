@@ -9,9 +9,12 @@
 // the arithmetic.
 //
 // kv_copy_kernel: grid (chunks, layer x KV head x {K, V}, pairs); a (layer, head) range of positions is contiguous in the
-// [layer][seq][kv head][n_ctx][hd] fp16 cache, copied in 16-byte vectors.
+// [layer][seq][kv head][n_ctx][hd] fp16 cache, copied in 16-byte vectors.  On a Q8_0 cache (kv_cache.cuh) grid y runs over
+// layer x KV head x {K codes, V codes, K scales, V scales}: the codes in 16-byte vectors, the scales (hd / 32 halves per row,
+// 4-byte aligned) in 4-byte words.
 #include "nsb.cuh"
 #include "beam.h"
+#include "kv_cache.cuh"
 #include "vocab_slices.cuh"
 
 #include <algorithm>
@@ -68,10 +71,31 @@ __global__ void __launch_bounds__(kLogprobThreads) beam_candidates_kernel(const 
   }
 }
 
-__global__ void __launch_bounds__(256) kv_copy_kernel(const KvCopyPairs a, __half* __restrict__ kc, __half* __restrict__ vc, int n_seq,
-                                                      int n_head_kv, int n_ctx, int hd) {
+template <int KV = NS_KV_F16>
+__global__ void __launch_bounds__(256) kv_copy_kernel(const KvCopyPairs a, kv_elem_t<KV>* __restrict__ kc, kv_elem_t<KV>* __restrict__ vc,
+                                                      int n_seq, int n_head_kv, int n_ctx, int hd, __half* __restrict__ kd,
+                                                      __half* __restrict__ vd) {
   pdl_launch_dependents();
   pdl_wait();
+  if constexpr (KV == NS_KV_Q8_0) {
+    const int pr = blockIdx.z, lh = blockIdx.y >> 2, plane = blockIdx.y & 3, layer = lh / n_head_kv, h = lh % n_head_kv;
+    const size_t us = ((size_t)layer * n_seq + a.src[pr]) * n_head_kv + h, ud = ((size_t)layer * n_seq + a.dst[pr]) * n_head_kv + h;
+    const int p0 = a.p0[pr], rows = a.p1[pr] - a.p0[pr];
+    if (plane < 2) {
+      int8_t* base = plane ? vc : kc;
+      const int4* src = reinterpret_cast<const int4*>(base + us * n_ctx * hd + (size_t)p0 * hd);
+      int4* dst = reinterpret_cast<int4*>(base + ud * n_ctx * hd + (size_t)p0 * hd);
+      const int n16 = rows * hd / 16;
+      for (int i = blockIdx.x * 256 + threadIdx.x; i < n16; i += gridDim.x * 256) dst[i] = src[i];
+    } else {
+      __half* base = plane == 3 ? vd : kd;
+      const size_t ds = kv_d_stride(n_ctx, hd);
+      const uint32_t* src = reinterpret_cast<const uint32_t*>(base + us * ds + (size_t)p0 * (hd / kKvQ8Block));
+      uint32_t* dst = reinterpret_cast<uint32_t*>(base + ud * ds + (size_t)p0 * (hd / kKvQ8Block));
+      const int n4 = rows * (hd / kKvQ8Block) / 2;
+      for (int i = blockIdx.x * 256 + threadIdx.x; i < n4; i += gridDim.x * 256) dst[i] = src[i];
+    }
+  } else {
   const int pr = blockIdx.z, lh = blockIdx.y >> 1, layer = lh / n_head_kv, h = lh % n_head_kv;
   __half* base = (blockIdx.y & 1) ? vc : kc;
   auto at = [&](int blk, int pos) { return base + (((size_t)layer * n_seq + blk) * n_head_kv + h) * n_ctx * hd + (size_t)pos * hd; };
@@ -79,6 +103,7 @@ __global__ void __launch_bounds__(256) kv_copy_kernel(const KvCopyPairs a, __hal
   int4* dst = reinterpret_cast<int4*>(at(a.dst[pr], a.p0[pr]));
   const int n16 = (a.p1[pr] - a.p0[pr]) * hd / 8;
   for (int i = blockIdx.x * 256 + threadIdx.x; i < n16; i += gridDim.x * 256) dst[i] = src[i];
+  }
 }
 
 }  // namespace
@@ -102,8 +127,7 @@ int ns_launch_beam_candidates(const BeamLaunch& a, cudaStream_t st) {
   return NS_OK;
 }
 
-int ns_launch_kv_copy(const KvCopyPairs& a, __half* kc, __half* vc, int n_layer, int n_seq, int n_head_kv, int n_ctx, int hd,
-                      cudaStream_t st) {
+int ns_launch_kv_copy(const KvCopyPairs& a, const KvPtrs& kv, int n_layer, int n_seq, int n_head_kv, int n_ctx, int hd, cudaStream_t st) {
   if (a.n < 1 || a.n > kBeamMaxRows || a.n > n_seq) {
     ns_set_error("ns_llama_kv_copy: %d pairs (1 .. %d)", a.n, std::min(n_seq, kBeamMaxRows));
     return NS_E_INVALID;
@@ -126,8 +150,13 @@ int ns_launch_kv_copy(const KvCopyPairs& a, __half* kc, __half* vc, int n_layer,
   const int n16 = longest * hd / 8;
   if (n16 == 0) return NS_OK;  // nothing to copy
   const unsigned gx = (unsigned)std::min((n16 + 255) / 256, 16);
-  NS_CUDA_TRY(ns_launch_pdl(kv_copy_kernel, dim3(gx, (unsigned)(n_layer * n_head_kv * 2), (unsigned)a.n), dim3(256), 0, st, a, kc, vc,
-                            n_seq, n_head_kv, n_ctx, hd));
+  if (kv.type == NS_KV_Q8_0)
+    NS_CUDA_TRY(ns_launch_pdl(kv_copy_kernel<NS_KV_Q8_0>, dim3(gx, (unsigned)(n_layer * n_head_kv * 4), (unsigned)a.n), dim3(256), 0, st, a,
+                              static_cast<int8_t*>(kv.k), static_cast<int8_t*>(kv.v), n_seq, n_head_kv, n_ctx, hd, kv.kd, kv.vd));
+  else
+    NS_CUDA_TRY(ns_launch_pdl(kv_copy_kernel<>, dim3(gx, (unsigned)(n_layer * n_head_kv * 2), (unsigned)a.n), dim3(256), 0, st, a,
+                              static_cast<__half*>(kv.k), static_cast<__half*>(kv.v), n_seq, n_head_kv, n_ctx, hd, (__half*)nullptr,
+                              (__half*)nullptr));
   ns_count_launch();
   return NS_OK;
 }

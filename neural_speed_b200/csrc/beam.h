@@ -41,6 +41,8 @@ struct KvCopyPairs {
 
 #ifdef __CUDACC__
 #include <cuda_fp16.h>
+
+#include "kv_cache.cuh"
 // ---- the device kernels (beam.cu) ------------------------------------------------------------------------------------------
 struct BeamLaunch {  // beam_candidates_kernel: grid (kVocabSlices, rows), kLogprobThreads threads, one launch per beam step
   const float* logits;  // [rows][n_vocab]
@@ -61,9 +63,8 @@ int ns_launch_beam_candidates(const BeamLaunch& a, cudaStream_t st);  // counts 
 size_t ns_beam_scratch_bytes(int rows, int k);                          // the scratch after the tickets
 void ns_beam_scratch(BeamLaunch& a, void* scratch, int rows, int k);    // points pmax .. pkeys into it
 // one launch for all pairs; refuses (NS_E_INVALID, nothing launched) a pair list in which a destination is also a source or
-// appears twice, a block outside [0, n_seq) or a range outside [0, n_ctx); counts its launch
-int ns_launch_kv_copy(const KvCopyPairs& a, __half* kc, __half* vc, int n_layer, int n_seq, int n_head_kv, int n_ctx, int hd,
-                      cudaStream_t st);
+// appears twice, a block outside [0, n_seq) or a range outside [0, n_ctx); counts its launch.  kv: the caches from layer 0, block 0
+int ns_launch_kv_copy(const KvCopyPairs& a, const KvPtrs& kv, int n_layer, int n_seq, int n_head_kv, int n_ctx, int hd, cudaStream_t st);
 #endif
 
 // ---- the flow (beam.cu): beam_search_flow::loop restated over an engine ------------------------------------------------------

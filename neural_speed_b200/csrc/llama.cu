@@ -134,7 +134,10 @@ struct ns_llama {
   const ns_weight* output = nullptr;
   std::vector<void*> owned;  // device allocations freed with the context
   int n_seq = 0;             // KV blocks: ns_llama_set_sequences (1 from ns_llama_create)
-  __half *kc = nullptr, *vc = nullptr;  // [n_layer][n_seq][n_head_kv][n_ctx][hd] fp16
+  int kv_type = NS_KV_F16;              // ns_llama_set_kv_type
+  void *kc = nullptr, *vc = nullptr;    // [n_layer][n_seq][n_head_kv][n_ctx][hd] fp16, or the Q8_0 codes (kv_cache.cuh)
+  __half *kd = nullptr, *vd = nullptr;  // Q8_0: the scale planes [n_layer][n_seq][n_head_kv][kv_d_stride]
+
   int* state = nullptr;   // device: {token, n_past, n_recorded, last_pick}
   int* tokens = nullptr;  // device: prompt tokens of the current eval
   int tok_cap = 0;        // ... their capacity: n_ctx, grown to the rows of a larger ns_llama_eval_batch pass
@@ -224,19 +227,29 @@ static void drop_graphs(ns_llama* c) {
 static int alloc_sequences(ns_llama* c, int n_seq) {
   const ns_llama_hparams& hp = c->hp;
   const int hd = hp.n_embd / hp.n_head;
-  void* old[6] = {c->kc, c->vc, c->logits, c->attn_part, c->attn_tickets, c->brecord};
+  void* old[8] = {c->kc, c->vc, c->kd, c->vd, c->logits, c->attn_part, c->attn_tickets, c->brecord};
   for (void* p : old) dev_free(c, p);
   c->kc = c->vc = nullptr;
+  c->kd = c->vd = nullptr;
   c->logits = c->attn_part = nullptr;
   c->attn_tickets = nullptr;
   c->brecord = nullptr;
   if (c->h_logits) cudaFreeHost(c->h_logits);
   c->h_logits = nullptr;
   c->n_seq = 0;
-  const size_t kv_elems = (size_t)n_seq * hp.n_layer * hp.n_head_kv * hp.n_ctx * hd;
+  const size_t units = (size_t)n_seq * hp.n_layer * hp.n_head_kv;
+  const size_t vbytes = units * hp.n_ctx * hd * (c->kv_type == NS_KV_Q8_0 ? 1 : 2);  // value plane (fp16 or Q8_0 codes)
+  const size_t dbytes = c->kv_type == NS_KV_Q8_0 ? kv_cache_bytes(NS_KV_Q8_0, units, hp.n_ctx, hd) - vbytes : 0;  // Q8_0 scales
   c->attn_nsplit = attn_ranges(hp.n_ctx);
-  c->kc = (__half*)dev_alloc(c, kv_elems * 2);
-  c->vc = (__half*)dev_alloc(c, kv_elems * 2);
+  c->kc = dev_alloc(c, vbytes);
+  c->vc = dev_alloc(c, vbytes);
+  if (dbytes) {
+    c->kd = (__half*)dev_alloc(c, dbytes);
+    c->vd = (__half*)dev_alloc(c, dbytes);
+    if (!c->kd || !c->vd) return NS_E_CUDA;
+    NS_CUDA_TRY(cudaMemsetAsync(c->kd, 0, dbytes, c->st));
+    NS_CUDA_TRY(cudaMemsetAsync(c->vd, 0, dbytes, c->st));
+  }
   c->logits = (float*)dev_alloc(c, (size_t)n_seq * hp.n_vocab * 4);
   c->attn_part = (float*)dev_alloc(c, (size_t)n_seq * hp.n_head * c->attn_nsplit * (hd + 2) * sizeof(float));
   c->attn_tickets = (unsigned*)dev_alloc(c, (size_t)n_seq * hp.n_head * sizeof(unsigned));
@@ -247,8 +260,8 @@ static int alloc_sequences(ns_llama* c, int n_seq) {
     return NS_E_CUDA;
   }
   NS_CUDA_TRY(cudaMemsetAsync(c->attn_tickets, 0, (size_t)n_seq * hp.n_head * sizeof(unsigned), c->st));
-  NS_CUDA_TRY(cudaMemsetAsync(c->kc, 0, kv_elems * 2, c->st));
-  NS_CUDA_TRY(cudaMemsetAsync(c->vc, 0, kv_elems * 2, c->st));
+  NS_CUDA_TRY(cudaMemsetAsync(c->kc, 0, vbytes, c->st));
+  NS_CUDA_TRY(cudaMemsetAsync(c->vc, 0, vbytes, c->st));
   c->n_seq = n_seq;
   return NS_OK;
 }
@@ -473,6 +486,17 @@ static Pass rows_pass(ns_llama* c, int n) {
   return s;
 }
 
+// the caches from unit 0 (layer 0, block 0, kv head 0) on
+static KvPtrs kv_base(const ns_llama* c) {
+  KvPtrs p;
+  p.type = c->kv_type;
+  p.k = c->kc;
+  p.v = c->vc;
+  p.kd = c->kd;
+  p.vd = c->vd;
+  return p;
+}
+
 // the embedding and every layer: leaves the last layer's output rows in c->x
 static int enqueue_body(ns_llama* c, const Pass& p) {
   const ns_llama_hparams& hp = c->hp;
@@ -484,11 +508,9 @@ static int enqueue_body(ns_llama* c, const Pass& p) {
   NS_CUDA_TRY(ns_launch_pdl(p.tok_stride == 4 ? embed_kernel<4> : embed_kernel<1>, dim3((unsigned)((E / 4 + 255) / 256), (unsigned)m),
                             dim3(256), 0, st, (const float*)c->tok_embd, p.toks, E, hp.n_vocab, c->x));
   ns_count_launch();
-  const size_t blk = (size_t)hp.n_head_kv * hp.n_ctx * hd;  // one sequence's cache of one layer
   for (int il = 0; il < hp.n_layer; ++il) {
     const Layer& L = c->layers[il];
-    __half* kc = c->kc + ((size_t)il * c->n_seq + p.seq) * blk;  // segments: block 0 of the layer
-    __half* vc = c->vc + ((size_t)il * c->n_seq + p.seq) * blk;
+    const KvPtrs kv = kv_base(c).at(((size_t)il * c->n_seq + p.seq) * hp.n_head_kv, hp.n_ctx, hd);  // segments: block 0 of the layer
     // Decode rows: the attention RMSNorm (llama.cpp:205-210) rides in the activation quantiser of the Q/K/V launch(es) -- every
     // CTA reads the whole row anyway -- instead of a one-CTA kernel and a launch boundary of its own.
     const ns_weight* qkvw[3] = {L.wq, L.wk, L.wv};
@@ -512,16 +534,16 @@ static int enqueue_body(ns_llama* c, const Pass& p) {
     if (p.segs) {
       const int d = p.d;
       if (d > 0)
-        if (int rc = launch_attention_batch(q, k, v, kc, vc, c->bstate, c->bstate + 4 * kMaxSeq, c->attn, c->attn_part, c->attn_tickets, d,
+        if (int rc = launch_attention_batch(q, k, v, kv, c->bstate, c->bstate + 4 * kMaxSeq, c->attn, c->attn_part, c->attn_tickets, d,
                                             hp.n_head, hp.n_head_kv, hd, hp.n_ctx, hp.rope_theta, hp.rope_scale, c->attn_attr, st))
           return rc;
       if (d < m)
-        if (int rc = launch_attention_ragged(q + (size_t)d * E, k + (size_t)d * kvd, v + (size_t)d * kvd, kc, vc, p.rows + 2 * d, p.tiles,
+        if (int rc = launch_attention_ragged(q + (size_t)d * E, k + (size_t)d * kvd, v + (size_t)d * kvd, kv, p.rows + 2 * d, p.tiles,
                                              m - d, p.n_tiles, c->attn + (size_t)d * E, hp.n_head, hp.n_head_kv, hd, hp.n_ctx,
                                              hp.rope_theta, hp.rope_scale, st))
           return rc;
     } else {
-      if (int rc = launch_attention(NS_ATTN_AUTO, q, k, v, kc, vc, c->state, c->attn, c->attn_part, c->attn_tickets, hp.n_head, hp.n_head_kv,
+      if (int rc = launch_attention(NS_ATTN_AUTO, q, k, v, kv, c->state, c->attn, c->attn_part, c->attn_tickets, hp.n_head, hp.n_head_kv,
                                     hd, hp.n_ctx, m, hp.rope_theta, hp.rope_scale, c->attn_attr, st, p.ring ? &c->ring : nullptr))
         return rc;
     }
@@ -667,6 +689,10 @@ extern "C" int ns_llama_set_streaming(ns_llama* c, int n_keep) {
   }
   if (n_keep >= 0 && hd != 64 && hd != 128) {
     ns_set_error("ns_llama_set_streaming: head size %d (the shift rides in the split decode attention: 64 or 128)", hd);
+    return NS_E_UNSUPPORTED;
+  }
+  if (n_keep >= 0 && c->kv_type != NS_KV_F16) {
+    ns_set_error("ns_llama_set_streaming: the KV cache is Q8_0 (the ring's shift would re-quantise every key on each wrap; set NS_KV_F16)");
     return NS_E_UNSUPPORTED;
   }
   NS_CUDA_TRY(cudaStreamSynchronize(c->st));  // nothing in flight replays the graph dropped below
@@ -1241,7 +1267,7 @@ struct DeviceBeams : BeamEngine {
   }
   int copy(const KvCopyPairs& p) override {
     const ns_llama_hparams& hp = c->hp;
-    return ns_launch_kv_copy(p, c->kc, c->vc, hp.n_layer, c->n_seq, hp.n_head_kv, hp.n_ctx, hp.n_embd / hp.n_head, c->st);
+    return ns_launch_kv_copy(p, kv_base(c), hp.n_layer, c->n_seq, hp.n_head_kv, hp.n_ctx, hp.n_embd / hp.n_head, c->st);
   }
 };
 }  // namespace
@@ -1315,19 +1341,60 @@ extern "C" int ns_llama_kv_copy(ns_llama* c, int n, const int* src, const int* d
     a.p1[i] = p1;
   }
   const ns_llama_hparams& hp = c->hp;
-  if (int rc = ns_launch_kv_copy(a, c->kc, c->vc, hp.n_layer, c->n_seq, hp.n_head_kv, hp.n_ctx, hp.n_embd / hp.n_head, c->st)) return rc;
+  if (int rc = ns_launch_kv_copy(a, kv_base(c), hp.n_layer, c->n_seq, hp.n_head_kv, hp.n_ctx, hp.n_embd / hp.n_head, c->st)) return rc;
   NS_CUDA_TRY(cudaStreamSynchronize(c->st));
   return NS_OK;
 }
 
 extern "C" int ns_llama_kv_cache(const ns_llama* c, void** k, void** v) {
   if (!c || !k || !v) return NS_E_INVALID;
+  if (c->kv_type != NS_KV_F16) {
+    ns_set_error("ns_llama_kv_cache: the KV cache is Q8_0 (ns_llama_kv_planes)");
+    return NS_E_UNSUPPORTED;
+  }
   *k = c->kc;
   *v = c->vc;
   return NS_OK;
 }
 
+extern "C" int ns_llama_kv_planes(const ns_llama* c, void** k, void** kd, void** v, void** vd) {
+  if (!c || !k || !kd || !v || !vd) return NS_E_INVALID;
+  *k = c->kc;
+  *kd = c->kd;
+  *v = c->vc;
+  *vd = c->vd;
+  return NS_OK;
+}
+
 extern "C" unsigned long long ns_llama_kv_bytes(const ns_llama* c) {
   if (!c) return 0;
-  return (unsigned long long)2 * c->n_seq * c->hp.n_layer * c->hp.n_head_kv * c->hp.n_ctx * (c->hp.n_embd / c->hp.n_head) * 2;
+  const size_t units = (size_t)c->n_seq * c->hp.n_layer * c->hp.n_head_kv;
+  return (unsigned long long)2 * kv_cache_bytes(c->kv_type, units, c->hp.n_ctx, c->hp.n_embd / c->hp.n_head);
+}
+
+extern "C" int ns_llama_kv_type(const ns_llama* c) { return c ? c->kv_type : NS_E_INVALID; }
+
+// every block reallocated in the new format and empty, the graphs dropped (as ns_llama_set_sequences)
+extern "C" int ns_llama_set_kv_type(ns_llama* c, int type) {
+  if (!c || (type != NS_KV_F16 && type != NS_KV_Q8_0)) {
+    ns_set_error("ns_llama_set_kv_type: type %d (NS_KV_F16 %d or NS_KV_Q8_0 %d)", type, NS_KV_F16, NS_KV_Q8_0);
+    return NS_E_INVALID;
+  }
+  const int hd = c->hp.n_embd / c->hp.n_head;
+  if (type == NS_KV_Q8_0 && c->streaming) {
+    ns_set_error("ns_llama_set_kv_type: streaming is on (the ring's shift would re-quantise every key on each wrap)");
+    return NS_E_UNSUPPORTED;
+  }
+  if (type == NS_KV_Q8_0 && hd != 64 && hd != 128) {
+    ns_set_error("ns_llama_set_kv_type: head size %d (the Q8_0 KV cache is read by the head size 64 / 128 kernels)", hd);
+    return NS_E_UNSUPPORTED;
+  }
+  NS_CUDA_TRY(cudaStreamSynchronize(c->st));  // nothing in flight uses the blocks or graphs released below
+  drop_graphs(c);
+  c->n_total = 0;
+  c->wrapped = false;
+  c->kv_type = type;
+  if (int rc = alloc_sequences(c, c->n_seq > 0 ? c->n_seq : 1)) return rc;
+  if (c->win) NS_CUDA_TRY(cudaMemsetAsync(c->win, 0, (size_t)kMaxSeq * kSampleMaxWindow * sizeof(int), c->st));
+  return NS_OK;
 }
