@@ -435,7 +435,8 @@ NS_API int ns_logprob_row_host(const float* logits, int n_vocab, int32_t target,
  * logit <= 0 ? logit * penalty : logit / penalty), the top_k largest logits (ties: lower id first), top-p on their fp32 softmax
  * (the first i >= 1 whose running sum passes top_p is dropped with everything after it), logits / temperature, an fp32 softmax,
  * and a draw of std::discrete_distribution on one std::mt19937(seed) for the whole context (GCC libstdc++'s arithmetic; a list
- * of one candidate takes it without drawing).  Rows of a batch draw in the caller's order.  The exp is the library's own
+ * of one candidate takes it without drawing).  Rows of a batch draw in the caller's order.  In per-sequence mode
+ * (ns_llama_set_sequence_sampling) each KV block has its own parameters, generator and window instead.  The exp is the library's own
  * (ns_sample_expf_host), within 1 ulp of glibc's expf.
  * Window of a sequence: its last W = min(repeat_last_n, n_ctx) evaluated tokens, preceded by zeros (the reference's history
  * starts as n_ctx zeros, application/main_pybind.cpp:460-474), including every token of the pass that samples.  Windows are kept
@@ -453,8 +454,29 @@ typedef struct ns_llama_sampling {
  * the captured graphs.  Picks returned and fed back by ns_llama_eval, ns_llama_eval_seq, ns_llama_generate (also past n_ctx on
  * the streaming ring), ns_llama_decode_batch, ns_llama_generate_batch and ns_llama_eval_batch are then sampled; returned
  * logits stay the raw logits.  The sampler takes the argmax's launch, so every step launches as many kernels as greedy.
- * NS_E_INVALID (mode unchanged) for a field out of range; NS_E_UNSUPPORTED for top_k > 1024. */
+ * NS_E_INVALID (mode unchanged) for a field out of range; NS_E_UNSUPPORTED for top_k > 1024.  Either call also leaves
+ * per-sequence mode (below): from then on the context picks exactly as one that never entered it. */
 NS_API int ns_llama_set_sampling(ns_llama* ctx, const ns_llama_sampling* s);
+/* Per-sequence sampling: each KV block its own parameters, generator and window, so greedy and sampled requests with any
+ * settings share a batch and a request's draws depend on nothing but its own seed and logits.
+ *   - The first call puts the context in per-sequence mode, where every block is greedy until it is given a config; entering
+ *     the mode drops the captured graphs, once.
+ *   - s non-null: block seq samples with s (the per-row arithmetic above) from its own std::mt19937(s->seed); its window
+ *     restarts as zeros and holds W = min(s->repeat_last_n, n_ctx) tokens.  s NULL: block seq is greedy again and keeps no
+ *     window.  A greedy block picks the argmax (lowest id on ties) and draws nothing.
+ *   - A change after entering drops and recaptures no graph: each block's parameters, generator and window live in device
+ *     tables that the captured steps read at replay.  The call synchronises the context's stream, so the change applies
+ *     exactly from the next step.
+ *   - Every entry point that picks -- ns_llama_eval, ns_llama_eval_seq, ns_llama_generate (block 0, also on the streaming
+ *     ring), ns_llama_decode_batch, ns_llama_generate_batch and ns_llama_eval_batch -- samples each row with its block's
+ *     config and draws from its block's generator, in whichever order the rows come; a row left with one candidate does
+ *     not draw.  A segment evaluated at n_past == 0 restarts its block's window.  Every step launches as many kernels as
+ *     greedy.
+ *   - ns_llama_set_sequences makes every block greedy again and stays in the mode; ns_llama_set_sampling leaves it.
+ *     ns_llama_eval_all and ns_llama_beam_search return NS_E_UNSUPPORTED while any block has a config.
+ * NS_E_INVALID for seq outside [0, n_seq) or a field out of range; NS_E_UNSUPPORTED for top_k > 1024.  A refused call changes
+ * nothing. */
+NS_API int ns_llama_set_sequence_sampling(ns_llama* ctx, int seq, const ns_llama_sampling* s);
 /* The sampler on its own, for parity tests: one launch over device logits [n][n_vocab] (1 <= n <= 32), device windows
  * [n][n_window] (0 <= n_window <= 256; every entry counts, repeat_last_n is not read) and a device generator mt_state[625] (as
  * ns_sample_seed_host writes it; advanced by the call).  picks [n] device; kept [n], ids [n][top_k] (the top_k list in selection
@@ -465,6 +487,15 @@ NS_API int ns_llama_set_sampling(ns_llama* ctx, const ns_llama_sampling* s);
 NS_API size_t ns_llama_sample_workspace_bytes(int n, int top_k);
 NS_API int ns_llama_sample(const float* logits, int n, int n_vocab, const int32_t* windows, int n_window, const ns_llama_sampling* s,
                            uint32_t* mt_state, int32_t* picks, int* kept, int32_t* ids, float* probs, void* ws, void* queue);
+/* The per-sequence sampler on its own, for parity tests: one launch as ns_llama_sample, but row r samples with its own config
+ * s[r] (s: host [n]) and draws from its own generator mt_states + 625 r (device [n][625], each advanced by its row's draw
+ * only).  Row r's window is the last min(s[r].repeat_last_n, n_window) entries of windows[r].  ids and probs are
+ * [n][max top_k]; ws holds ns_llama_sample_workspace_bytes(n, max top_k) bytes, zeroed once, its tickets where
+ * ns_llama_sample keeps them.  Codes as ns_llama_sample (the first refused row's); a refused call launches nothing and writes
+ * nothing. */
+NS_API int ns_llama_sample_rows(const float* logits, int n, int n_vocab, const int32_t* windows, int n_window,
+                                const ns_llama_sampling* s, uint32_t* mt_states, int32_t* picks, int* kept, int32_t* ids,
+                                float* probs, void* ws, void* queue);
 /* Host restatements (no device needed): std::mt19937(seed) as 625 words; steps 2-7 for one row of n_vocab logits with the window
  * window[0 .. n_window) -- pick, kept count, ids [top_k] and probs [top_k] as ns_llama_sample writes them -- advancing `state`;
  * and the sampler's exp. */

@@ -64,6 +64,7 @@ EXPORTS = [
     "ns_llama_attention_batch_workspace_bytes", "ns_llama_attention_batch",
     "ns_llama_eval_batch", "ns_llama_batch_plan", "ns_llama_attention_ragged_workspace_bytes", "ns_llama_attention_ragged",
     "ns_llama_set_sampling", "ns_llama_sample_workspace_bytes", "ns_llama_sample", "ns_sample_seed_host", "ns_sample_row_host",
+    "ns_llama_set_sequence_sampling", "ns_llama_sample_rows",
     "ns_sample_expf_host", "ns_llama_eval_all", "ns_llama_logprob_workspace_bytes", "ns_llama_logprob", "ns_logprob_row_host",
     "ns_llama_beam_search", "ns_llama_kv_copy", "ns_llama_kv_cache", "ns_llama_beam_candidates_workspace_bytes", "ns_llama_beam_candidates",
     "ns_beam_candidates_row_host", "ns_logf_host", "ns_beam_search_host",
@@ -213,6 +214,8 @@ def lib() -> C.CDLL:
     L.ns_llama_sample_workspace_bytes.restype = sz
     L.ns_llama_sample_workspace_bytes.argtypes = [i, i]
     L.ns_llama_sample.argtypes = [vp, i, i, vp, i, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.ns_llama_set_sequence_sampling.argtypes = [vp, i, vp]
+    L.ns_llama_sample_rows.argtypes = [vp, i, i, vp, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.ns_sample_seed_host.restype = None
     L.ns_sample_seed_host.argtypes = [C.c_uint32, vp]
     L.ns_sample_row_host.argtypes = [vp, i, vp, i, vp, vp, vp, vp, vp, vp]
@@ -591,6 +594,14 @@ class Llama:
         s = sampling(top_k, top_p, temperature, repeat_penalty, repeat_last_n, seed)
         _check(lib().ns_llama_set_sampling(self.h, C.byref(s)), "ns_llama_set_sampling")
 
+    def set_sequence_sampling(self, seq: int, top_k=40, top_p=0.95, temperature=0.8, repeat_penalty=1.1, repeat_last_n=64, seed=0):
+        """KV block `seq` samples with these settings from its own std::mt19937(seed), its window restarted; top_k=None makes it
+        greedy.  The first call enters per-sequence mode (every other block greedy); later calls recapture no graph
+        (include/ns_b200.h, ns_llama_set_sequence_sampling)"""
+        s = None if top_k is None else sampling(top_k, top_p, temperature, repeat_penalty, repeat_last_n, seed)
+        _check(lib().ns_llama_set_sequence_sampling(self.h, seq, C.byref(s) if s is not None else None),
+               "ns_llama_set_sequence_sampling")
+
     def set_sequences(self, n_seq: int):
         """n_seq KV blocks for continuous batching; every sequence restarts empty (include/ns_b200.h, ns_llama_set_sequences)"""
         _check(lib().ns_llama_set_sequences(self.h, n_seq), "ns_llama_set_sequences")
@@ -843,6 +854,17 @@ def sample(logits_ptr: int, n: int, n_vocab: int, windows_ptr, n_window: int, s:
                                  C.byref(s), C.c_void_p(mt_ptr), C.c_void_p(picks_ptr), C.c_void_p(kept_ptr) if kept_ptr else None,
                                  C.c_void_p(ids_ptr) if ids_ptr else None, C.c_void_p(probs_ptr) if probs_ptr else None,
                                  C.c_void_p(ws_ptr), queue)
+
+
+def sample_rows(logits_ptr: int, n: int, n_vocab: int, windows_ptr, n_window: int, configs, mt_ptr: int, picks_ptr: int, kept_ptr,
+                ids_ptr, probs_ptr, ws_ptr: int, queue=None) -> int:
+    """ns_llama_sample_rows on device pointers: row r samples with configs[r] from the generator at mt_ptr + 625 r words;
+    returns the status code"""
+    cfg = (Sampling * max(len(configs), 1))(*configs)
+    return lib().ns_llama_sample_rows(C.c_void_p(logits_ptr), n, n_vocab, C.c_void_p(windows_ptr) if windows_ptr else None, n_window,
+                                      cfg, C.c_void_p(mt_ptr), C.c_void_p(picks_ptr), C.c_void_p(kept_ptr) if kept_ptr else None,
+                                      C.c_void_p(ids_ptr) if ids_ptr else None, C.c_void_p(probs_ptr) if probs_ptr else None,
+                                      C.c_void_p(ws_ptr), queue)
 
 
 def beam_candidates_row_host(logits, k: int, prev=0.0, mask=False, eos=2):

@@ -12,6 +12,8 @@
 // Greedy sampling = argmax with the lowest index on ties (model_utils.cpp:2963-2985).
 // ns_llama_set_sampling swaps the argmax's launch for sample_kernel (sample.cu): model_post_sample_top_k_top_p_repeat
 // (model_utils.cpp:2987-3032) with its generator and the sequences' repetition windows in device memory.
+// ns_llama_set_sequence_sampling swaps it for the per-sequence instantiation instead: each KV block's parameters and generator
+// in device tables that the captured graphs read at replay, so changing a block's config recaptures nothing.
 //
 // One token (n_tokens == 1) is ONE CUDA graph: the token id and n_past live in device memory (`state`), so the same graph
 // replays for every position; ns_llama_generate chains graph launches with the argmax feeding the next embedding
@@ -178,6 +180,12 @@ struct ns_llama {
   int* s_kept = nullptr;              // [kMaxSeq]
   int* s_ids = nullptr;               // [kMaxSeq][kSampleMaxK]
   float* s_probs = nullptr;           // [kMaxSeq][kSampleMaxK]
+  // ns_llama_set_sequence_sampling: while `per_seq`, block b samples with seq_cfg[b] (greedy when !seq_on[b]) from its own
+  // generator; its window is the last seq_cfg[b].W entries of its slot of `win`.  Allocated on first use.
+  bool per_seq = false;
+  bool seq_on[kMaxSeq] = {};
+  SampleCfg* seq_cfg = nullptr;       // [kMaxSeq]
+  uint32_t* seq_mt = nullptr;         // std::mt19937 [kMaxSeq][kMtWords]
   // ns_llama_eval_all (allocated on first use): the lm_head's logits of one chunk of rows, the log-prob kernel's tickets and
   // partials, the rows' targets / log-probs / picks in internal order, and pinned staging for those and two chunks of logits
   float* all_logits = nullptr;        // [kAllChunk][n_vocab]
@@ -594,12 +602,12 @@ static int enqueue_forward(ns_llama* c, const Pass& p) {
   if (int rc = launch_lm_head(c, xl, rows, fold, 0, c->logits)) return rc;
   int* state = p.segs ? c->bstate : c->state;  // a segments pass: a pick per row
   const int n_tokens = p.segs ? 1 : p.m;
-  if (c->sampling) {
+  if (c->sampling || c->per_seq) {
     SampleLaunch a{};
     a.logits = c->logits;
     a.n_vocab = hp.n_vocab;
     a.rows = rows;
-    a.k = c->smp.top_k;
+    a.k = c->per_seq ? kSampleMaxK : c->smp.top_k;  // per block: the scratch stride, and the shared memory of any top_k
     a.top_p = c->smp.top_p;
     a.temp = c->smp.temperature;
     a.penalty = c->smp.repeat_penalty;
@@ -615,7 +623,8 @@ static int enqueue_forward(ns_llama* c, const Pass& p) {
     a.order = p.draw;
     a.store = p.sample >= 1;
     a.draw = p.sample >= 2;
-    a.mt = c->mt;
+    a.mt = c->per_seq ? c->seq_mt : c->mt;
+    a.cfg = c->per_seq ? c->seq_cfg : nullptr;
     a.pkeys = c->s_keys;
     a.pcnt = c->s_pcnt;
     a.cp = c->s_cp;
@@ -703,13 +712,9 @@ extern "C" int ns_llama_set_streaming(ns_llama* c, int n_keep) {
   return NS_OK;
 }
 
-// Sampling in place of greedy (model_post_sample_top_k_top_p_repeat): the generator is reseeded and every window restarts;
-// NULL returns to greedy.  Either way the captured graphs, which bake in the pick kernel and its parameters, are dropped.
-extern "C" int ns_llama_set_sampling(ns_llama* c, const ns_llama_sampling* s) {
-  if (!c) return NS_E_INVALID;
-  if (s)
-    if (int rc = ns_sample_check("ns_llama_set_sampling", s)) return rc;
-  if (s && !c->mt) {
+// the sampler's generator, windows and scratch, allocated on first use
+static int ensure_sampler(ns_llama* c) {
+  if (!c->mt) {
     c->mt = (uint32_t*)dev_alloc(c, kMtWords * sizeof(uint32_t));
     c->win = (int*)dev_alloc(c, (size_t)kMaxSeq * kSampleMaxWindow * sizeof(int));
     c->s_keys = (unsigned long long*)dev_alloc(c, (size_t)kMaxSeq * kVocabSlices * kSampleMaxK * sizeof(unsigned long long));
@@ -723,12 +728,33 @@ extern "C" int ns_llama_set_sampling(ns_llama* c, const ns_llama_sampling* s) {
       void* got[9] = {c->mt, c->win, c->s_keys, c->s_pcnt, c->s_cp, c->s_tickets, c->s_kept, c->s_ids, c->s_probs};
       for (void* p : got) dev_free(c, p);
       c->mt = nullptr;
+      c->win = nullptr;
+      c->s_keys = nullptr;
+      c->s_pcnt = nullptr;
+      c->s_cp = nullptr;
+      c->s_tickets = nullptr;
+      c->s_kept = nullptr;
+      c->s_ids = nullptr;
+      c->s_probs = nullptr;
       return NS_E_CUDA;
     }
     NS_CUDA_TRY(cudaMemsetAsync(c->s_tickets, 0, (kMaxSeq + 1) * sizeof(unsigned), c->st));
   }
+  return NS_OK;
+}
+
+// Sampling in place of greedy (model_post_sample_top_k_top_p_repeat): the generator is reseeded and every window restarts;
+// NULL returns to greedy.  Either way the context leaves per-sequence mode, and the captured graphs, which bake in the pick
+// kernel and its parameters, are dropped.
+extern "C" int ns_llama_set_sampling(ns_llama* c, const ns_llama_sampling* s) {
+  if (!c) return NS_E_INVALID;
+  if (s)
+    if (int rc = ns_sample_check("ns_llama_set_sampling", s)) return rc;
+  if (s)
+    if (int rc = ensure_sampler(c)) return rc;
   NS_CUDA_TRY(cudaStreamSynchronize(c->st));  // nothing in flight replays the graphs dropped below or reads the generator
   drop_graphs(c);
+  c->per_seq = false;
   c->sampling = s != nullptr;
   if (!s) return NS_OK;
   c->smp = *s;
@@ -738,6 +764,71 @@ extern "C" int ns_llama_set_sampling(ns_llama* c, const ns_llama_sampling* s) {
   NS_CUDA_TRY(cudaMemsetAsync(c->win, 0, (size_t)kMaxSeq * kSampleMaxWindow * sizeof(int), c->st));
   NS_CUDA_TRY(cudaStreamSynchronize(c->st));
   return NS_OK;
+}
+
+// per-sequence mode: every block greedy, every window zero (stream-ordered)
+static int greedy_blocks(ns_llama* c) {
+  SampleCfg g[kMaxSeq];
+  for (int b = 0; b < kMaxSeq; ++b) {
+    g[b] = ns_sample_cfg(nullptr, 0);
+    c->seq_on[b] = false;
+  }
+  NS_CUDA_TRY(cudaMemcpyAsync(c->seq_cfg, g, sizeof(g), cudaMemcpyHostToDevice, c->st));
+  NS_CUDA_TRY(cudaMemsetAsync(c->win, 0, (size_t)kMaxSeq * kSampleMaxWindow * sizeof(int), c->st));
+  return NS_OK;
+}
+
+// Block seq samples with s from the next step on (its generator reseeded, its window restarted), or is greedy for s NULL.  The
+// first call enters per-sequence mode and drops the graphs once; later calls only rewrite the block's table entry, generator and
+// window, which the captured graphs read at replay.
+extern "C" int ns_llama_set_sequence_sampling(ns_llama* c, int seq, const ns_llama_sampling* s) {
+  const char* who = "ns_llama_set_sequence_sampling";
+  if (!c) return NS_E_INVALID;
+  if (seq < 0 || seq >= c->n_seq) {
+    ns_set_error("%s: sequence id %d outside [0, %d)", who, seq, c->n_seq);
+    return NS_E_INVALID;
+  }
+  if (s)
+    if (int rc = ns_sample_check(who, s)) return rc;
+  if (int rc = ensure_sampler(c)) return rc;
+  if (!c->seq_cfg) {
+    c->seq_cfg = (SampleCfg*)dev_alloc(c, kMaxSeq * sizeof(SampleCfg));
+    c->seq_mt = (uint32_t*)dev_alloc(c, (size_t)kMaxSeq * kMtWords * sizeof(uint32_t));
+    if (!c->seq_cfg || !c->seq_mt) {
+      dev_free(c, c->seq_cfg);
+      dev_free(c, c->seq_mt);
+      c->seq_cfg = nullptr;
+      c->seq_mt = nullptr;
+      return NS_E_CUDA;
+    }
+  }
+  cudaStream_t st = c->st;
+  if (!c->per_seq) {
+    NS_CUDA_TRY(cudaStreamSynchronize(st));  // nothing in flight replays the graphs dropped below
+    drop_graphs(c);
+    c->sampling = false;
+    c->per_seq = true;
+    if (int rc = greedy_blocks(c)) return rc;
+  }
+  const SampleCfg cfg = ns_sample_cfg(s, c->hp.n_ctx);
+  NS_CUDA_TRY(cudaMemcpyAsync(c->seq_cfg + seq, &cfg, sizeof(cfg), cudaMemcpyHostToDevice, st));
+  if (s) {
+    uint32_t mt[kMtWords];
+    ns_mt_seed(s->seed, mt);
+    NS_CUDA_TRY(cudaMemcpyAsync(c->seq_mt + (size_t)seq * kMtWords, mt, sizeof(mt), cudaMemcpyHostToDevice, st));
+  }
+  NS_CUDA_TRY(cudaMemsetAsync(c->win + (size_t)seq * kSampleMaxWindow, 0, kSampleMaxWindow * sizeof(int), st));
+  NS_CUDA_TRY(cudaStreamSynchronize(st));  // the host sources are consumed; the next step samples with the new config
+  c->seq_on[seq] = s != nullptr;
+  return NS_OK;
+}
+
+// a block samples: the context-wide sampler is on, or a block has its own config
+static bool any_sampling(const ns_llama* c) {
+  if (c->sampling) return true;
+  for (int b = 0; c->per_seq && b < kMaxSeq; ++b)
+    if (c->seq_on[b]) return true;
+  return false;
 }
 
 // Positions of a streaming context: n_past is n_total.  Steps that reach past n_ctx take one token and continue the sequence;
@@ -769,7 +860,7 @@ static void advance_position(ns_llama* c, int n_past, int n) {
 // the sequences seq[i] evaluated at n_past[i] 0 restart their sampling windows as zeros (the reference's fresh history); nothing
 // while greedy
 static int reset_windows(ns_llama* c, int n, const int* seq, const int* n_past) {
-  if (!c->sampling) return NS_OK;
+  if (!c->sampling && !c->per_seq) return NS_OK;
   for (int i = 0; i < n; ++i)
     if (n_past[i] == 0) NS_CUDA_TRY(cudaMemsetAsync(c->win + (size_t)seq[i] * kSampleMaxWindow, 0, kSampleMaxWindow * sizeof(int), c->st));
   return NS_OK;
@@ -876,6 +967,7 @@ extern "C" int ns_llama_set_sequences(ns_llama* c, int n_seq) {
   c->n_total = 0;
   c->wrapped = false;
   if (int rc = alloc_sequences(c, n_seq)) return rc;
+  if (c->per_seq) return greedy_blocks(c);
   if (c->win) NS_CUDA_TRY(cudaMemsetAsync(c->win, 0, (size_t)kMaxSeq * kSampleMaxWindow * sizeof(int), c->st));
   return NS_OK;
 }
@@ -1116,7 +1208,7 @@ extern "C" int ns_llama_eval_all(ns_llama* c, int n, const int* seq, const int* 
         ns_set_error("%s: target %d of row %d outside [0, n_vocab %d)", who, targets[r], r, V);
         return NS_E_INVALID;
       }
-  if (c->sampling) {
+  if (any_sampling(c)) {
     ns_set_error("%s: sampling is on (a scoring pass draws nothing; set greedy first)", who);
     return NS_E_UNSUPPORTED;
   }
@@ -1302,8 +1394,8 @@ extern "C" int ns_llama_beam_search(ns_llama* c, int n, const int* n_tokens, con
     return NS_E_INVALID;
   }
   const int hd = c->hp.n_embd / c->hp.n_head;
-  if (c->sampling || c->streaming || (hd != 64 && hd != 128)) {
-    ns_set_error("%s: %s", who, c->sampling ? "sampling is on (the reference searches beams only with do_sample off)"
+  if (any_sampling(c) || c->streaming || (hd != 64 && hd != 128)) {
+    ns_set_error("%s: %s", who, any_sampling(c) ? "sampling is on (the reference searches beams only with do_sample off)"
                                 : c->streaming ? "streaming is on (the reference's beam search has no shifted cache, model_utils.cpp:2245)"
                                                : "head size other than 64 / 128 (the batched decode attention)");
     return NS_E_UNSUPPORTED;

@@ -186,6 +186,12 @@ NS_HD int ns_sample_pick(const double* cp, int n, uint32_t* mt) {
 
 #ifdef __CUDACC__
 // ---- the device sampler (sample.cu), one launch in place of the eval step's argmax ------------------------------------------
+// one entry of the per-sequence sampler's parameter table; greedy is {1, 1, 1, 1, 0}: one candidate, no penalty, no window
+struct SampleCfg {
+  int k;            // top_k, 1 .. kSampleMaxK
+  float top_p, temp, penalty;
+  int W;            // window length (0: no penalty, no window kept)
+};
 struct SampleLaunch {  // grid (kVocabSlices, rows): each CTA selects the top k of one slice of the vocabulary
   const float* logits;  // [rows][n_vocab]
   int n_vocab, rows;
@@ -218,7 +224,14 @@ struct SampleLaunch {  // grid (kVocabSlices, rows): each CTA selects the top k 
   int rowwise, n_tokens, advance;
   int* record;
   int rec_stride;
+  // non-null: the per-sequence sampler.  Row r's slot s (as its window's) selects its parameters cfg[s] and its generator
+  // mt + s kMtWords; k, top_p, temp, penalty and W above are not read, k is the stride of the scratch rows (>= every cfg k)
+  // and the window is the last cfg[s].W of the win_stride entries at win + s win_stride.  Each row draws in its own last CTA;
+  // order is not read.
+  const SampleCfg* cfg;
 };
 int ns_launch_sample(const SampleLaunch& a, cudaStream_t st);  // counts its launch
 int ns_sample_check(const char* who, const struct ns_llama_sampling* s);
+// the table entry of a checked config, its window min(repeat_last_n, max_window); greedy for null
+SampleCfg ns_sample_cfg(const struct ns_llama_sampling* s, int max_window);
 #endif
