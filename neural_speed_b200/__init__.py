@@ -20,7 +20,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "libns_b200.so")
 
 # enums (include/ns_b200.h)
-W_S4, W_S8, W_NF4, W_Q6K = 0, 1, 2, 3
+W_S4, W_S8, W_NF4, W_Q6K, W_Q8_0 = 0, 1, 2, 3, 4
 S_F32, S_BF16, S_F16 = 0, 1, 2
 COMP_F32, COMP_BF16, COMP_INT8, COMP_Q8_0, COMP_INT8_S8 = 0, 1, 2, 3, 4
 NE_COMP_UNDEF, NE_COMP_F32, NE_COMP_BF16, NE_COMP_F16, NE_COMP_INT8 = 0, 1, 2, 3, 4
@@ -50,12 +50,12 @@ EXPORTS = [
     "bestla_device_malloc", "bestla_device_free", "bestla_device_memcpy", "bestla_device_memcpy_sync", "bestla_device_sync",
     "bestla_device_storage_size", "ns_device_storage_bytes", "bestla_device_load_storage", "ns_device_workspace_bytes",
     "bestla_device_f32f32_forward",
-    "ns_weight_from_q4_0", "ns_weight_from_q6_K", "ns_weight_from_btla_blob", "ns_weight_from_btla_blob_n", "ns_weight_random", "ns_weight_from_unpacked", "ns_weight_free", "ns_weight_info",
+    "ns_weight_from_q4_0", "ns_weight_from_q6_K", "ns_weight_from_q8_0", "ns_weight_from_btla_blob", "ns_weight_from_btla_blob_n", "ns_weight_random", "ns_weight_from_unpacked", "ns_weight_free", "ns_weight_info",
     "ns_weight_set_comp", "ns_weight_algorithmic_bytes", "ns_weight_dequant_f32",
     "ns_mul_mat", "ns_mul_qkv", "ns_ffn_silu", "ns_ffn_gelu",
     "ns_mul_mat_id", "ns_ffn_id", "ns_mul_mat_id_q4_0_f32_host", "ns_moe_plan",
-    "ns_rmsnorm_fusable", "ns_rmsnorm_mul_mat", "ns_rmsnorm_mul_qkv", "ns_rmsnorm_ffn_silu", "ns_mul_mat_q4_0_f32_host", "ns_mul_mat_q6_K_f32_host",
-    "ns_prepare_activation", "ns_matmul_prepared", "ns_gemv_ring_plan", "ns_mul_mat_engine_image", "ns_graph_begin", "ns_graph_end", "ns_graph_launch", "ns_graph_free",
+    "ns_rmsnorm_fusable", "ns_rmsnorm_mul_mat", "ns_rmsnorm_mul_qkv", "ns_rmsnorm_ffn_silu", "ns_mul_mat_q4_0_f32_host", "ns_mul_mat_q6_K_f32_host", "ns_mul_mat_q8_0_f32_host",
+    "ns_prepare_activation", "ns_matmul_prepared", "ns_gemv_ring_plan", "ns_gemv_ring_plan_q8_0", "ns_mul_mat_engine_image", "ns_graph_begin", "ns_graph_end", "ns_graph_launch", "ns_graph_free",
     "ns_device_quantize_q4_0", "ns_device_quantize_act",
     "BTLAGemmPackBSize", "BTLAGemmQuantPackB", "BTLAGemmPackB", "BTLAGemmUnPackB", "ns_quantize_row_q4_0", "ns_split_weight_size", "ns_split_weight",
     "ns_llama_create", "ns_llama_free", "ns_llama_set_f32", "ns_llama_set_weight", "ns_llama_eval", "ns_llama_generate", "ns_llama_set_exact_prefill",
@@ -131,6 +131,9 @@ def lib() -> C.CDLL:
     L.ns_weight_from_q6_K.restype = vp
     L.ns_weight_from_q6_K.argtypes = [vp, i, i, sz, i, vp]
     L.ns_mul_mat_q6_K_f32_host.argtypes = [vp, sz, vp, vp, i, i, i]
+    L.ns_weight_from_q8_0.restype = vp
+    L.ns_weight_from_q8_0.argtypes = [vp, i, i, sz, i, vp]
+    L.ns_mul_mat_q8_0_f32_host.argtypes = [vp, sz, vp, vp, i, i, i]
     L.ns_weight_from_btla_blob.restype = vp
     L.ns_weight_from_btla_blob.argtypes = [vp, vp]
     L.ns_weight_random.restype = vp
@@ -175,6 +178,7 @@ def lib() -> C.CDLL:
     L.ns_prepare_activation.argtypes = [vp, vp, i, i, vp, vp]
     L.ns_matmul_prepared.argtypes = [vp, i, i, vp, vp, i, i, vp, i, vp, vp, vp]
     L.ns_gemv_ring_plan.argtypes = [i] * 9 + [vp]
+    L.ns_gemv_ring_plan_q8_0.argtypes = [i] * 5 + [vp]
     L.ns_mul_mat_engine_image.argtypes = [vp, vp, i, vp, i, i, vp, vp, vp]
     L.ns_graph_begin.argtypes = [vp]
     L.ns_graph_end.restype = vp
@@ -387,6 +391,16 @@ class Weight:
         """rows: uint8 [n, k/256*210] block_q6_K rows (the Q6_K output.weight of llama.cpp "Q4_0" GGUF files)."""
         rows = np.ascontiguousarray(rows, np.uint8)
         return cls(lib().ns_weight_from_q6_K(_np_ptr(rows), n, k, rows.shape[1], 0, queue))
+
+    @classmethod
+    def from_q8_0_host(cls, rows: np.ndarray, n: int, k: int, queue=None):
+        """rows: uint8 [n, k/32*34] block_q8_0 rows (every 2-D tensor of llama.cpp "Q8_0" GGUF files)."""
+        rows = np.ascontiguousarray(rows, np.uint8)
+        return cls(lib().ns_weight_from_q8_0(_np_ptr(rows), n, k, rows.shape[1], 0, queue))
+
+    @classmethod
+    def from_q8_0_device(cls, dev_ptr: int, n: int, k: int, nb01: int, queue=None):
+        return cls(lib().ns_weight_from_q8_0(C.c_void_p(dev_ptr), n, k, nb01, 1, queue))
 
     @classmethod
     def random(cls, n, k, group=32, wfmt=W_S4, stype=S_F32, comp=COMP_INT8, asym=False, seed=1, queue=None):

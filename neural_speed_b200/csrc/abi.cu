@@ -137,11 +137,13 @@ static void weight_carve(ns_weight* w, void* base, bool with_shuffle) {
   p += ns_round_up((size_t)w->n * w->pitch, 256);
   w->shuffle = with_shuffle ? (int*)p : nullptr;
 }
-static int weight_alloc(ns_weight* w, bool with_shuffle) {
+// st: the stream the weight is then filled on.  The clearing is ordered before the fill on that stream: a plain cudaMemset runs on
+// the legacy default stream, which the library's non-blocking streams do not wait for, and could land after (or during) the repack.
+static int weight_alloc(ns_weight* w, bool with_shuffle, cudaStream_t st) {
   w->total_bytes = weight_image_bytes(w, with_shuffle);
   NS_CUDA_TRY(cudaMalloc(&w->base, w->total_bytes));
   // padding bytes of each row are streamed by the GEMV too: keep them defined
-  NS_CUDA_TRY(cudaMemset(w->base, 0, w->total_bytes));
+  NS_CUDA_TRY(cudaMemsetAsync(w->base, 0, w->total_bytes, st));
   w->external = 0;
   weight_carve(w, w->base, with_shuffle);
   return NS_OK;
@@ -170,20 +172,31 @@ extern "C" int ns_weight_set_comp(ns_weight* w, int comp) {
     ns_set_error("NF4 weights support float compute only (docs/advanced_usage.md:82-83)");
     return NS_E_UNSUPPORTED;
   }
+  if (w->wfmt == NS_W_Q8_0 && comp != NS_COMP_Q8_0) {
+    ns_set_error("ggml Q8_0 weights have the fixed compute type NS_COMP_Q8_0");
+    return NS_E_UNSUPPORTED;
+  }
   w->comp = comp;
   return NS_OK;
 }
 extern "C" size_t ns_weight_algorithmic_bytes(const ns_weight* w) {
   if (w->wfmt == NS_W_Q6K) return (size_t)w->n * (w->k / 256) * 210;  // block_q6_K bytes
   // SURVEY.md 8(d): N*K*bits/8 + N*ceil(K/g)*(scale_bytes [+1 if asym])
-  const size_t bits = (w->wfmt == NS_W_S8) ? 8 : 4;
+  const size_t bits = (w->wfmt == NS_W_S8 || w->wfmt == NS_W_Q8_0) ? 8 : 4;  // Q8_0: N*K + N*K/32*2, block_q8_0's bytes
   return (size_t)w->n * w->k * bits / 8 + (size_t)w->n * w->ngroups * (stype_size(w->stype) + (w->asym ? 1 : 0));
 }
 
-extern "C" ns_weight* ns_weight_from_q4_0(const void* rows, int n, int k, size_t nb01, int rows_on_device, void* queue) {
+// ggml rows of 32-element blocks (block_q4_0: 18 bytes, block_q8_0: 34 bytes) -> NSB rows, repacked on the device
+static ns_weight* weight_from_ggml32(bool q8, const void* rows, int n, int k, size_t nb01, int rows_on_device, void* queue) {
+  const char* who = q8 ? "ns_weight_from_q8_0" : "ns_weight_from_q4_0";
   if (ns_ensure_device()) return nullptr;
-  if (!rows || n <= 0 || k <= 0 || k % 32 != 0 || nb01 < (size_t)k / 32 * 18) {
-    ns_set_error("ns_weight_from_q4_0: invalid arguments (n=%d k=%d nb01=%zu)", n, k, nb01);
+  if (!rows || n <= 0 || k <= 0 || k % 32 != 0 || nb01 < (size_t)k / 32 * (q8 ? 34 : 18)) {
+    ns_set_error("%s: invalid arguments (n=%d k=%d nb01=%zu)", who, n, k, nb01);
+    return nullptr;
+  }
+  // the repack kernels read blocks as 16-bit words (fp16 d, then the codes): rows must start on even addresses
+  if (nb01 % 2 != 0 || (rows_on_device && ((uintptr_t)rows & 1))) {
+    ns_set_error("%s: rows must be 2-byte aligned (nb01=%zu, rows=%p)", who, nb01, rows);
     return nullptr;
   }
   cudaStream_t st = stream_of(queue);
@@ -192,12 +205,12 @@ extern "C" ns_weight* ns_weight_from_q4_0(const void* rows, int n, int k, size_t
   w->n = n;
   w->k = k;
   w->group = 32;
-  w->wfmt = NS_W_S4;
+  w->wfmt = q8 ? NS_W_Q8_0 : NS_W_S4;
   w->stype = NS_S_F16;
   w->comp = NS_COMP_Q8_0;
   w->asym = 0;
   weight_layout(w);
-  if (weight_alloc(w, false)) {
+  if (weight_alloc(w, false, st)) {
     delete w;
     return nullptr;
   }
@@ -205,15 +218,15 @@ extern "C" ns_weight* ns_weight_from_q4_0(const void* rows, int n, int k, size_t
   void* tmp = nullptr;
   if (!rows_on_device) {
     const size_t bytes = (size_t)n * nb01;
-    if (!ns_cuda_ok(cudaMalloc(&tmp, bytes), "cudaMalloc(q4_0 staging)") ||
-        !ns_cuda_ok(cudaMemcpyAsync(tmp, rows, bytes, cudaMemcpyHostToDevice, st), "H2D q4_0 rows")) {
+    if (!ns_cuda_ok(cudaMalloc(&tmp, bytes), q8 ? "cudaMalloc(q8_0 staging)" : "cudaMalloc(q4_0 staging)") ||
+        !ns_cuda_ok(cudaMemcpyAsync(tmp, rows, bytes, cudaMemcpyHostToDevice, st), q8 ? "H2D q8_0 rows" : "H2D q4_0 rows")) {
       if (tmp) cudaFree(tmp);
       ns_weight_free(w);
       return nullptr;
     }
     src = tmp;
   }
-  int rc = ns_launch_repack_q4_0(src, nb01, w, st);
+  int rc = q8 ? ns_launch_repack_q8_0(src, nb01, w, st) : ns_launch_repack_q4_0(src, nb01, w, st);
   if (tmp) {
     cudaStreamSynchronize(st);
     cudaFree(tmp);
@@ -223,6 +236,12 @@ extern "C" ns_weight* ns_weight_from_q4_0(const void* rows, int n, int k, size_t
     return nullptr;
   }
   return w;
+}
+extern "C" ns_weight* ns_weight_from_q4_0(const void* rows, int n, int k, size_t nb01, int rows_on_device, void* queue) {
+  return weight_from_ggml32(false, rows, n, k, nb01, rows_on_device, queue);
+}
+extern "C" ns_weight* ns_weight_from_q8_0(const void* rows, int n, int k, size_t nb01, int rows_on_device, void* queue) {
+  return weight_from_ggml32(true, rows, n, k, nb01, rows_on_device, queue);
 }
 
 extern "C" ns_weight* ns_weight_from_q6_K(const void* rows, int n, int k, size_t nb01, int rows_on_device, void* queue) {
@@ -241,7 +260,7 @@ extern "C" ns_weight* ns_weight_from_q6_K(const void* rows, int n, int k, size_t
   w->comp = NS_COMP_Q8_0;  // ggml integer path (Q8_K activations)
   w->asym = 0;
   ns_q6k_layout(w);
-  if (weight_alloc(w, false)) {
+  if (weight_alloc(w, false, st)) {
     delete w;
     return nullptr;
   }
@@ -292,7 +311,7 @@ extern "C" ns_weight* ns_weight_from_unpacked(const int8_t* q, const float* scal
     delete w;
     return nullptr;
   }
-  if (weight_alloc(w, shuffle != nullptr)) {
+  if (weight_alloc(w, shuffle != nullptr, st)) {
     delete w;
     return nullptr;
   }
@@ -550,7 +569,7 @@ extern "C" ns_weight* ns_weight_from_btla_blob_n(const void* blob, size_t nbytes
   BlobView v;
   if (!parse_blob(blob, &v, nbytes)) return nullptr;
   ns_weight* w = new ns_weight();
-  if (blob_to_weight_meta(v, w) || weight_alloc(w, v.shuffle != nullptr)) {
+  if (blob_to_weight_meta(v, w) || weight_alloc(w, v.shuffle != nullptr, stream_of(queue))) {
     delete w;
     return nullptr;
   }
@@ -565,8 +584,9 @@ extern "C" ns_weight* ns_weight_from_btla_blob_n(const void* blob, size_t nbytes
 // bandwidth bound: speed does not depend on the values; parity tests never use this).
 extern "C" ns_weight* ns_weight_random(int n, int k, int group, int wfmt, int stype, int comp, int asym, unsigned seed, void* queue) {
   if (ns_ensure_device()) return nullptr;
-  if (n <= 0 || k <= 0 || !(wfmt == NS_W_S4 || wfmt == NS_W_S8 || wfmt == NS_W_NF4) || stype < 0 || stype > NS_S_F16 || comp < 0 ||
-      comp > NS_COMP_INT8_S8 || (wfmt == NS_W_NF4 && (asym || !(comp == NS_COMP_F32 || comp == NS_COMP_BF16)))) {
+  if (n <= 0 || k <= 0 || !(wfmt == NS_W_S4 || wfmt == NS_W_S8 || wfmt == NS_W_NF4 || wfmt == NS_W_Q8_0) || stype < 0 || stype > NS_S_F16 ||
+      comp < 0 || comp > NS_COMP_INT8_S8 || (wfmt == NS_W_NF4 && (asym || !(comp == NS_COMP_F32 || comp == NS_COMP_BF16))) ||
+      (wfmt == NS_W_Q8_0 && (k % 32 || group != 32 || stype != NS_S_F16 || comp != NS_COMP_Q8_0 || asym))) {
     ns_set_error("ns_weight_random: invalid geometry");
     return nullptr;
   }
@@ -580,7 +600,7 @@ extern "C" ns_weight* ns_weight_random(int n, int k, int group, int wfmt, int st
   w->comp = comp;
   w->asym = asym ? 1 : 0;
   weight_layout(w);
-  if (weight_alloc(w, false) || ns_launch_random_weight(w, seed, stream_of(queue))) {
+  if (weight_alloc(w, false, stream_of(queue)) || ns_launch_random_weight(w, seed, stream_of(queue))) {
     ns_weight_free(w);
     return nullptr;
   }
@@ -599,7 +619,8 @@ extern "C" int ns_weight_dequant_f32(const ns_weight* w, float* dst_dev, int ld,
 // ---------------------------------------------------------------------------------------------------- device matmuls
 // Every matmul node runs on one of four kernel paths, and the path fixes the node's numerics class (DESIGN.md section 4):
 //   NS_PATH_GEMV  GEMV tiles of <= 4 rows: the TMA ring, or the register GEMV for the formats the ring does not take
-//   NS_PATH_IMMA  integer tensor cores, 3..32 rows of int4 weights with an integer compute type: the GEMV's exact block sums
+//   NS_PATH_IMMA  integer tensor cores, 3..32 rows of int4 weights with an integer compute type or of ggml Q8_0 weights: the
+//                 GEMV's exact block sums
 //   NS_PATH_TC    wgmma GEMM, bf16 numerics
 //   NS_PATH_Q6K   ggml Q6_K x Q8_K in tiles of <= 4 rows, plain nodes only
 // ns_route is the one place that picks the path; the workspace of a node and whether an RMSNorm folds into it follow from it.
@@ -675,7 +696,7 @@ extern "C" size_t ns_device_workspace_bytes(int m, int k) {
 static void* pick_ws(void* workspace, cudaStream_t st, size_t bytes) { return workspace ? workspace : scratch_get(st, bytes); }
 
 static int norm_unsupported(const char* who) {
-  ns_set_error("%s: the RMSNorm can only be folded into the ring GEMV (int4 weights, integer compute type, <= 2 rows)", who);
+  ns_set_error("%s: the RMSNorm can only be folded into the ring GEMV (int4 weights with an integer compute type or Q8_0, <= 2 rows)", who);
   return NS_E_UNSUPPORTED;
 }
 
@@ -824,6 +845,24 @@ extern "C" int ns_rmsnorm_ffn_silu(const ns_weight* w1, const ns_weight* w2, con
   return ffn_impl(w1, w2, w3, NS_ELT_DEFAULT, nullptr, nullptr, 0, act, lda, tmp, dst, ldo, m, workspace, queue, residual, norm_w,
                   norm_eps);
 }
+// The plan of one ring launch of weight geometry w (n, k, group, wfmt, stype, comp, asym set; mode checked by the caller), as the
+// launchers would run it: ns_gemv_ring_plan and ns_gemv_ring_plan_q8_0 differ only in the weights they describe
+static int ring_plan_of(const char* who, ns_weight& w, int mode, int m, int fused, int norm, int* out) {
+  ns_weight_layout(&w);
+  if (w.group % 32 && w.group != w.k) {
+    ns_set_error("%s: group size %d is not a multiple of 32", who, w.group);
+    return NS_E_INVALID;
+  }
+  if (m < 1 || m > ns_gemv_tile_rows(&w) || (fused && !ns_gemv_fused_quant_ok(&w)) || (norm && (!fused || m > 2))) {
+    ns_set_error("%s: no such launch (m=%d of at most %d, fused=%d, norm=%d)", who, m, ns_gemv_tile_rows(&w), fused, norm);
+    return NS_E_INVALID;
+  }
+  RingChoice c;
+  const bool ok = ns_gemv_ring_choose(w.kpad, w.pitch, mode, m >= 3 ? 4 : m, fused != 0, norm != 0, &c);
+  out[0] = ok && c.wide, out[1] = ok ? c.plan.rows : 0, out[2] = ok ? c.plan.stages : 0, out[3] = ok ? c.plan.active : 0;
+  out[4] = ok ? c.plan.ctas : 0;
+  return ok ? 1 : 0;
+}
 extern "C" int ns_gemv_ring_plan(int k, int group, int stype, int asym, int comp, int mode, int m, int fused, int norm, int* out) {
   ns_weight w;
   memset(&w, 0, sizeof(w));
@@ -833,20 +872,17 @@ extern "C" int ns_gemv_ring_plan(int k, int group, int stype, int asym, int comp
     ns_set_error("ns_gemv_ring_plan: not a ring GEMV launch (k=%d stype=%d comp=%d mode=%d)", k, stype, comp, mode);
     return NS_E_INVALID;
   }
-  ns_weight_layout(&w);
-  if (w.group % 32 && w.group != w.k) {
-    ns_set_error("ns_gemv_ring_plan: group size %d is not a multiple of 32", w.group);
+  return ring_plan_of("ns_gemv_ring_plan", w, mode, m, fused, norm, out);
+}
+extern "C" int ns_gemv_ring_plan_q8_0(int k, int mode, int m, int fused, int norm, int* out) {
+  ns_weight w;
+  memset(&w, 0, sizeof(w));
+  w.n = 2, w.k = k, w.group = 32, w.wfmt = NS_W_Q8_0, w.stype = NS_S_F16, w.comp = NS_COMP_Q8_0, w.asym = 0;
+  if (k < 32 || k % 32 || mode < NS_GEMV_PLAIN || mode > NS_GEMV_GATE_UP_SILU || !out) {
+    ns_set_error("ns_gemv_ring_plan_q8_0: not a ring GEMV launch (k=%d mode=%d)", k, mode);
     return NS_E_INVALID;
   }
-  if (m < 1 || m > ns_gemv_tile_rows(&w) || (fused && !ns_gemv_fused_quant_ok(&w)) || (norm && (!fused || m > 2))) {
-    ns_set_error("ns_gemv_ring_plan: no such launch (m=%d of at most %d, fused=%d, norm=%d)", m, ns_gemv_tile_rows(&w), fused, norm);
-    return NS_E_INVALID;
-  }
-  RingChoice c;
-  const bool ok = ns_gemv_ring_choose(w.kpad, w.pitch, mode, m >= 3 ? 4 : m, fused != 0, norm != 0, &c);
-  out[0] = ok && c.wide, out[1] = ok ? c.plan.rows : 0, out[2] = ok ? c.plan.stages : 0, out[3] = ok ? c.plan.active : 0;
-  out[4] = ok ? c.plan.ctas : 0;
-  return ok ? 1 : 0;
+  return ring_plan_of("ns_gemv_ring_plan_q8_0", w, mode, m, fused, norm, out);
 }
 extern "C" int ns_rmsnorm_fusable(const ns_weight* const* weights, int nw, int m) {
   return (weights && nw >= 1 && nw <= 3 && norm_foldable(weights, nw, m)) ? 1 : 0;
@@ -1442,15 +1478,20 @@ extern "C" size_t ns_host_cache_entries(void) {
   return g_cache.size();
 }
 
-// ggml host drop-in
-static const ns_weight* ggml_cached_weight(int q6k, const void* src0_rows, size_t nb01, int ne00, int ne01) {
-  const size_t tag = blob_tag(src0_rows, (size_t)(ne01 - 1) * nb01 + (size_t)(ne00 / (q6k ? 256 : 32)) * (q6k ? 210 : 18)) ^
-                     ((size_t)ne00 << 32) ^ (size_t)ne01 ^ ((size_t)q6k << 63);
+// ggml host drop-in; type: which block the rows hold
+enum { GG_Q4_0 = 0, GG_Q6_K = 1, GG_Q8_0 = 2 };
+static int gg_block_elems(int type) { return type == GG_Q6_K ? 256 : 32; }
+static size_t gg_block_bytes(int type) { return type == GG_Q6_K ? 210 : type == GG_Q8_0 ? 34 : 18; }
+static const ns_weight* ggml_cached_weight(int type, const void* src0_rows, size_t nb01, int ne00, int ne01) {
+  const size_t tag = blob_tag(src0_rows, (size_t)(ne01 - 1) * nb01 + (size_t)(ne00 / gg_block_elems(type)) * gg_block_bytes(type)) ^
+                     ((size_t)ne00 << 32) ^ (size_t)ne01 ^ ((size_t)type << 62);
   std::unique_lock<std::mutex> lk(g_mu);
   auto it = g_cache.find(src0_rows);
   if (it != g_cache.end() && it->second.tag == tag) return it->second.w;
   lk.unlock();
-  ns_weight* nw = q6k ? ns_weight_from_q6_K(src0_rows, ne01, ne00, nb01, 0, nullptr) : ns_weight_from_q4_0(src0_rows, ne01, ne00, nb01, 0, nullptr);
+  ns_weight* nw = type == GG_Q6_K   ? ns_weight_from_q6_K(src0_rows, ne01, ne00, nb01, 0, nullptr)
+                  : type == GG_Q8_0 ? ns_weight_from_q8_0(src0_rows, ne01, ne00, nb01, 0, nullptr)
+                                    : ns_weight_from_q4_0(src0_rows, ne01, ne00, nb01, 0, nullptr);
   if (!nw) return nullptr;
   lk.lock();
   auto it2 = g_cache.find(src0_rows);
@@ -1458,13 +1499,13 @@ static const ns_weight* ggml_cached_weight(int q6k, const void* src0_rows, size_
   g_cache[src0_rows] = CacheEntry{nw, tag};
   return nw;
 }
-static int ggml_mul_mat_host(int q6k, const void* src0_rows, size_t nb01, const float* src1, float* dst, int ne00, int ne01, int ne11) {
+static int ggml_mul_mat_host(int type, const void* src0_rows, size_t nb01, const float* src1, float* dst, int ne00, int ne01, int ne11) {
   if (int rc = ns_ensure_device()) return rc;
-  if (!src0_rows || !src1 || !dst || ne00 % (q6k ? 256 : 32) != 0 || ne01 <= 0 || ne11 <= 0) {
+  if (!src0_rows || !src1 || !dst || ne00 % gg_block_elems(type) != 0 || ne01 <= 0 || ne11 <= 0) {
     ns_set_error("ggml host matmul: invalid arguments");
     return NS_E_INVALID;
   }
-  const ns_weight* w = ggml_cached_weight(q6k, src0_rows, nb01, ne00, ne01);
+  const ns_weight* w = ggml_cached_weight(type, src0_rows, nb01, ne00, ne01);
   if (!w) return NS_E_CUDA;
   cudaStream_t st = default_stream();
   if (!io_reserve(&g_io.act, &g_io.act_elems, (size_t)ne11 * ne00) || !io_reserve(&g_io.out, &g_io.out_elems, (size_t)ne11 * ne01)) {
@@ -1479,11 +1520,15 @@ static int ggml_mul_mat_host(int q6k, const void* src0_rows, size_t nb01, const 
 }
 extern "C" int ns_mul_mat_q4_0_f32_host(const void* src0_rows, size_t nb01, const float* src1, float* dst, int ne00, int ne01,
                                         int ne11) {
-  return ggml_mul_mat_host(0, src0_rows, nb01, src1, dst, ne00, ne01, ne11);
+  return ggml_mul_mat_host(GG_Q4_0, src0_rows, nb01, src1, dst, ne00, ne01, ne11);
 }
 extern "C" int ns_mul_mat_q6_K_f32_host(const void* src0_rows, size_t nb01, const float* src1, float* dst, int ne00, int ne01,
                                         int ne11) {
-  return ggml_mul_mat_host(1, src0_rows, nb01, src1, dst, ne00, ne01, ne11);
+  return ggml_mul_mat_host(GG_Q6_K, src0_rows, nb01, src1, dst, ne00, ne01, ne11);
+}
+extern "C" int ns_mul_mat_q8_0_f32_host(const void* src0_rows, size_t nb01, const float* src1, float* dst, int ne00, int ne01,
+                                        int ne11) {
+  return ggml_mul_mat_host(GG_Q8_0, src0_rows, nb01, src1, dst, ne00, ne01, ne11);
 }
 // ne_compute_forward_mul_mat_id_q_f32 (ne_layers.c:7345-7498) on host buffers: expert_rows[e] = dst->opt[e]->data (Q4_0 rows of
 // pitch nb01), ids = ids->data with ids_stride = ids->nb[1] / 4 int32 per token, id = dst->op_params[0]
@@ -1497,7 +1542,7 @@ extern "C" int ns_mul_mat_id_q4_0_f32_host(const void* const* expert_rows, int n
   std::vector<const ns_weight*> ws((size_t)n_as, nullptr);
   for (int e = 0; e < n_as; ++e) {
     if (!expert_rows[e]) return NS_E_INVALID;
-    ws[(size_t)e] = ggml_cached_weight(0, expert_rows[e], nb01, ne00, ne01);
+    ws[(size_t)e] = ggml_cached_weight(GG_Q4_0, expert_rows[e], nb01, ne00, ne01);
     if (!ws[(size_t)e]) return NS_E_CUDA;
   }
   cudaStream_t st = default_stream();

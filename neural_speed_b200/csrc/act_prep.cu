@@ -101,7 +101,7 @@ int ns_launch_act_prep(const float* act, int lda, int m, const ns_weight* w, voi
     return NS_OK;
   }
   uint8_t* aq = (uint8_t*)ws;
-  const int ring_layout = (w->wfmt == NS_W_S4) ? 1 : 0;  // consumed by gemv_ring.cu; other formats use natural rows
+  const int ring_layout = (w->wfmt == NS_W_S4 || w->wfmt == NS_W_Q8_0) ? 1 : 0;  // consumed by gemv_ring.cu; other formats use natural rows
   const int act_row = ring_layout ? (int)ns_round_up((size_t)kpad, 1024) : kpad;
   int2* meta = (int2*)((char*)ws + ns_round_up((size_t)m * act_row, 16));
   const int ms = ns_meta_stride(kpad);
@@ -110,7 +110,7 @@ int ns_launch_act_prep(const float* act, int lda, int m, const ns_weight* w, voi
   const int ngroups = (w->k + group - 1) / group;
   const int warps = m * ngroups;
   const int blocks = (warps + 7) / 8;
-  const int perm8 = (w->wfmt == NS_W_S8) ? 0 : 1;
+  const int perm8 = (w->wfmt == NS_W_S8 || w->wfmt == NS_W_Q8_0) ? 0 : 1;  // 8-bit codes keep natural order (nsb.cuh)
   cudaError_t e;
   if (w->comp == NS_COMP_Q8_0)
     e = ns_launch_pdl(act_quant_kernel<NS_COMP_Q8_0>, dim3(blocks), dim3(256), 0, st, act, lda, m, w->k, kpad, group,

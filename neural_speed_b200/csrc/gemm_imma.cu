@@ -1,4 +1,4 @@
-// gemm_imma.cu -- batched decode (3..32 activation rows): 4-bit weights x int8 activations on the INTEGER tensor cores.
+// gemm_imma.cu -- batched decode (3..32 activation rows): 4-bit weights (and ggml Q8_0) x int8 activations on the INTEGER tensor cores.
 //
 // Replaces, for 4 < M <= 32, what the reference runs through LauncherIntKBlock + the VNNI / AMX int8 GemmCores
 // (bestla/bestla/bestla_wrapper.h:214-350, bestla_gemm.h "ICoreRowNAvx512vnniKBlock" etc.): u8 (or s8) activations quantised
@@ -19,6 +19,9 @@
 // A word of packed nibbles (8 consecutive k) gives MMA k-slots 4t..4t+3 (low nibbles) and 16+4t..16+4t+3 (high nibbles) of
 // thread t of a quad; the activation image stores the matching bytes (nsb.cuh: (e0,e4,e1,e5) / (e2,e6,e3,e7)), so no
 // shuffling happens in the loop: ldmatrix, 4 LOP, one 8-byte shared load per 8 tokens, MMA.
+// ggml Q8_0 weights (W8): the codes are already s8 -- mma.sync m16n8k32 s8 x s8, no nibble expansion.  A stage holds the same
+// 256 k, now 256 bytes per row: two 128-byte swizzled boxes, and ldmatrix over one 32-byte chunk of 8 + 8 rows yields the A
+// fragment directly (k 4t..4t+3 and 16+4t..16+4t+3 of rows g, g+8); the activation image stores each chunk in that k-slot order.
 // Scales and zero points of the CTA's rows / K range are staged once, before griddepcontrol.wait (weights are constant).
 // Split-K: partial tiles go to a workspace; the last CTA of a tile (ticket) sums them in split order -- deterministic --
 // and runs the epilogue (bias, GELU, residual, QKV layout, SiLU(gate) * up).
@@ -85,6 +88,12 @@ __device__ __forceinline__ void imma0(int (&c)[4], const uint32_t (&a)[4], uint3
                  : "=r"(c[0]), "=r"(c[1]), "=r"(c[2]), "=r"(c[3])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1), "r"(0));
 }
+// s8 weights x s8 activations (ggml Q8_0 x Q8_0), zero accumulator input: every 32-chunk is one block
+__device__ __forceinline__ void imma_ss0(int (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%10,%10,%10};"
+               : "=r"(c[0]), "=r"(c[1]), "=r"(c[2]), "=r"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1), "r"(0));
+}
 // exact int -> float for |i| < 2^22 without the quarter-rate I2F: (float)(i + 0x4B400000 as float bits) - 12582912
 __device__ __forceinline__ float i2f_small(int i) { return __int_as_float(i + 0x4B400000) - 12582912.f; }
 
@@ -93,7 +102,9 @@ __device__ __forceinline__ float i2f_small(int i) { return __int_as_float(i + 0x
 // image of this kernel: per K-slice of 256, [8 chunks][MT tokens][32 B] codes then [8][MT] meta words, where Sa is the sum of
 // the codes of the WHOLE activation block (the matmul corrects per block, not per chunk).
 // Tokens >= M and chunks past K are written as zeros (scale 0): they contribute nothing.  Block 0 also clears the tickets.
-template <int COMP>
+// W8: 8-bit weight codes in natural order; byte 8t + 4h + i of a chunk holds k = 16h + 4t + i (the B fragment of thread t),
+// else the NSB4 pairing order (nsb.cuh).
+template <int COMP, bool W8 = false>
 __global__ void __launch_bounds__(256) act_quant_imma_kernel(const float* __restrict__ A, int lda, int M, int K, int qg, int MT, int nslices,
                                                              uint8_t* __restrict__ img, unsigned* __restrict__ tickets, int ntickets) {
   pdl_launch_dependents();
@@ -145,7 +156,7 @@ __global__ void __launch_bounds__(256) act_quant_imma_kernel(const float* __rest
     bq.za = 0;
     stot = 0;
   }
-  const int pos = (lane & ~7) | nsq::dp4a_pos(lane & 7);
+  const int pos = W8 ? (((lane & 15) >> 2) << 3) | ((lane >> 4) << 2) | (lane & 3) : (lane & ~7) | nsq::dp4a_pos(lane & 7);
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
     if (c < cpb) {
@@ -173,14 +184,17 @@ __device__ __forceinline__ float lds_scale_b(uint32_t a) {  // a: byte address o
 }
 
 // PER: 32-chunks per activation block, compile-time for the common cases (1: ggml Q8_0 / group 32, 4: group 128) so that the
-// eight chunks of a stage are one straight-line schedule; 0: read from the parameters (groups 64 / 256)
-template <bool ACT_U8, int MT, bool ASYM, int STYPE, int PER>
+// eight chunks of a stage are one straight-line schedule; 0: read from the parameters (groups 64 / 256).
+// W8: ggml Q8_0 weights (instantiated with s8 activations, symmetric, fp16 scales, PER 1 only).
+template <bool ACT_U8, int MT, bool ASYM, int STYPE, int PER, bool W8 = false>
 __global__ void __launch_bounds__(kThr, 2)
     gemm_imma_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1,
                      const __grid_constant__ CUtensorMap map2, const ImmaParams P) {
   constexpr int NTB = MT / 8;
   constexpr int kActStage = MT * 320;
-  constexpr int kStage = kQStage + ((kActStage + 1023) / 1024) * 1024;  // q boxes must stay 1024-B aligned (128B swizzle)
+  constexpr int QST = W8 ? 2 * kQStage : kQStage;  // weight bytes per stage
+  static_assert(!W8 || (!ACT_U8 && !ASYM && PER == 1), "8-bit codes: ggml Q8_0 only");
+  constexpr int kStage = QST + ((kActStage + 1023) / 1024) * 1024;  // q boxes must stay 1024-B aligned (128B swizzle)
   constexpr int SS = (STYPE == NS_S_F32) ? 4 : 2;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   // 128B-swizzled TMA boxes need 1024-byte aligned destinations: align by hand (the launcher adds the slack)
@@ -222,7 +236,16 @@ __global__ void __launch_bounds__(kThr, 2)
       const CUtensorMap* mp1 = &map1;
       auto issue_w = [&](int i, int s) {
         const uint32_t dst = base + (uint32_t)s * kStage;
-        mbar_expect_tx(full0 + 8 * s, (uint32_t)(kQStage + kActStage));
+        mbar_expect_tx(full0 + 8 * s, (uint32_t)(QST + kActStage));
+        if (W8) {  // two 128-byte boxes per row: k 0..127 and 128..255 of the slice
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int x = (sl0 + i) * KS + h * (KS / 2);
+            tma_2d(dst + h * kQStage, mp0, x, r0, full0 + 8 * s);
+            if (gate_up) tma_2d(dst + h * kQStage + (BN / 2) * (KS / 2), mp1, x, r0, full0 + 8 * s);
+          }
+          return;
+        }
         const int x = (sl0 + i) * (KS / 2);
         if (gate_up) {
           tma_2d(dst, mp0, x, r0, full0 + 8 * s);
@@ -232,7 +255,7 @@ __global__ void __launch_bounds__(kThr, 2)
         }
       };
       auto issue_a = [&](int i, int s) {
-        bulk_g2s(base + (uint32_t)s * kStage + kQStage, P.act_img + (size_t)(sl0 + i) * kActStage, (uint32_t)kActStage, full0 + 8 * s);
+        bulk_g2s(base + (uint32_t)s * kStage + QST, P.act_img + (size_t)(sl0 + i) * kActStage, (uint32_t)kActStage, full0 + 8 * s);
       };
       const int pre = nsl < stages ? nsl : stages;
       for (int i = 0; i < pre; ++i) issue_w(i, i);  // weights do not depend on the previous kernel
@@ -330,8 +353,30 @@ __global__ void __launch_bounds__(kThr, 2)
     const int gstage = (((sl0 + i) * 8) >> P.cpg_shift) - g0;  // first weight group of the stage (a stage holds whole groups)
     mbar_wait(full0 + 8 * s, phase);
     const uint32_t qs = base + (uint32_t)s * kStage;
-    const uint32_t as = qs + kQStage;
+    const uint32_t as = qs + QST;
     const uint32_t ms = as + MT * 256;
+    if constexpr (W8) {
+      // one 32-byte chunk per ldmatrix.x4: (rows g, g+8) x (bytes 4t.., 16+4t..) = the A fragment, s8 as stored
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        uint32_t a[4];
+        ldmatrix_x4(qs + (uint32_t)(j >> 2) * kQStage + (lthread ^ ((uint32_t)(2 * (j & 3)) << 4)), a[0], a[1], a[2], a[3]);
+        const int gi = gstage + j;
+        const float wsA = lds_scale_b<STYPE>(scA + SS * gi), wsB = lds_scale_b<STYPE>(scB + SS * gi);
+#pragma unroll
+        for (int tb = 0; tb < NTB; ++tb) {
+          const uint2 b = lds64(as + (uint32_t)j * (MT * 32) + (uint32_t)(tb * 8 + g) * 32u + 8u * t);
+          int ci8[4];
+          imma_ss0(ci8, a, b.x, b.y);
+          const uint4 mt = lds128(ms + (uint32_t)(j * MT + tb * 8 + 2 * t) * 8u);  // {scale, S} of tokens 2t, 2t+1
+          const float as0 = __uint_as_float(mt.x), as1 = __uint_as_float(mt.z);
+          acc[tb][0] = fmaf(i2f_small(ci8[0]), as0 * wsA, acc[tb][0]);  // |block sum| <= 32 x 128 x 127 < 2^22
+          acc[tb][1] = fmaf(i2f_small(ci8[1]), as1 * wsA, acc[tb][1]);
+          acc[tb][2] = fmaf(i2f_small(ci8[2]), as0 * wsB, acc[tb][2]);
+          acc[tb][3] = fmaf(i2f_small(ci8[3]), as1 * wsB, acc[tb][3]);
+        }
+      }
+    } else
 #pragma unroll
     for (int j2 = 0; j2 < 8; j2 += 2) {
       uint32_t w0, w1, w2, w3;
@@ -478,6 +523,7 @@ int mt_of(int m) { return m <= 8 ? 8 : (m <= 16 ? 16 : 32); }
 
 bool make_plan(const ns_weight* const* ws, int nw, int mode, int m, Plan* pl) {
   const ns_weight* w0 = ws[0];
+  const bool w8 = w0->wfmt == NS_W_Q8_0;
   pl->mt = mt_of(m);
   pl->nslices = (w0->kpad + KS - 1) / KS;
   int tiles = 0;
@@ -491,10 +537,11 @@ bool make_plan(const ns_weight* const* ws, int nw, int mode, int m, Plan* pl) {
   const int ss = ns_stype_size(w0->stype);
   const int cpg = w0->group / 32;
   const int kact = pl->mt * 320;
-  const int kstage = kQStage + (kact + 1023) / 1024 * 1024;
+  const int kstage = (w8 ? 2 : 1) * kQStage + (kact + 1023) / 1024 * 1024;
   // split K.  Two CTAs share an SM (16 consumer warps hide the MMA / shared-memory latencies; one CTA's prologue overlaps the
   // other's main loop), so a wave has 2 x SMs slots and a CTA gets half an SM's bandwidth: cost of a choice = waves x (2 x slices
-  // per CTA + ramp).  The staged scales must fit beside a ring of >= 3 stages in half an SM's shared memory.
+  // per CTA + ramp).  The staged scales must fit beside a ring of >= 3 stages in half an SM's shared memory (>= 2 of the
+  // twice as large stages of 8-bit codes: the same bytes in flight).
   static const int env_split = getenv("NS_IMMA_KSPLIT") ? atoi(getenv("NS_IMMA_KSPLIT")) : 0;
   static const int env_budget = getenv("NS_IMMA_SMEM_KB") ? atoi(getenv("NS_IMMA_SMEM_KB")) : 0;
   const int sms = ns_num_sms();
@@ -510,7 +557,8 @@ bool make_plan(const ns_weight* const* ws, int nw, int mode, int m, Plan* pl) {
     const int sc_zp = (int)ns_round_up((size_t)15 + (size_t)ss * ng, 16);
     const int sc_row = sc_zp + (w0->asym ? (int)ns_round_up((size_t)15 + ng, 16) : 0);
     const size_t fixed = (size_t)BN * sc_row + 16 * 16 + 64 + 1024;
-    const int need = max_sl < 3 ? max_sl : 3;
+    const int min_st = w8 ? 2 : 3;
+    const int need = max_sl < min_st ? max_sl : min_st;
     if (fixed + (size_t)need * kstage > budget) continue;
     const long waves = ((long)tiles * ks + per_sm * sms - 1) / (per_sm * sms);
     const long cost = waves * (per_sm * max_sl + 2) * 16 + ks;  // ties: fewer splits
@@ -534,9 +582,9 @@ bool make_plan(const ns_weight* const* ws, int nw, int mode, int m, Plan* pl) {
   return true;
 }
 
-template <bool ACT_U8, int MT, bool ASYM, int STYPE, int PER>
+template <bool ACT_U8, int MT, bool ASYM, int STYPE, int PER, bool W8 = false>
 int launch_p(const CUtensorMap* maps, const ImmaParams& P, const Plan& pl, cudaStream_t st) {
-  auto kern = gemm_imma_kernel<ACT_U8, MT, ASYM, STYPE, PER>;
+  auto kern = gemm_imma_kernel<ACT_U8, MT, ASYM, STYPE, PER, W8>;
   static bool attr = false;
   if (!attr) {
     NS_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
@@ -560,6 +608,14 @@ int launch_s(const CUtensorMap* maps, const ImmaParams& P, const Plan& pl, int s
     default: return launch_k<ACT_U8, MT, ASYM, NS_S_BF16>(maps, P, pl, st);
   }
 }
+// ggml Q8_0: s8 x s8, symmetric, fp16 scales, one block per 32-chunk
+int launch_q8_0(const CUtensorMap* maps, const ImmaParams& P, const Plan& pl, cudaStream_t st) {
+  switch (pl.mt) {
+    case 8: return launch_p<false, 8, false, NS_S_F16, 1, true>(maps, P, pl, st);
+    case 16: return launch_p<false, 16, false, NS_S_F16, 1, true>(maps, P, pl, st);
+    default: return launch_p<false, 32, false, NS_S_F16, 1, true>(maps, P, pl, st);
+  }
+}
 template <bool ACT_U8, bool ASYM>
 int launch_m(const CUtensorMap* maps, const ImmaParams& P, const Plan& pl, int stype, cudaStream_t st) {
   switch (pl.mt) {
@@ -579,8 +635,8 @@ bool ns_gemm_imma_supported(const ns_weight* const* ws, int nw, int m) {
   const ns_weight* w0 = ws[0];
   for (int i = 0; i < nw; ++i) {
     const ns_weight* w = ws[i];
-    if (!w || w->wfmt != NS_W_S4 || w->shuffle) return false;
-    if (w->k != w0->k || w->group != w0->group || w->stype != w0->stype || w->comp != w0->comp || w->asym != w0->asym) return false;
+    if (!w || !(w->wfmt == NS_W_S4 || w->wfmt == NS_W_Q8_0) || w->shuffle) return false;
+    if (w->wfmt != w0->wfmt || w->k != w0->k || w->group != w0->group || w->stype != w0->stype || w->comp != w0->comp || w->asym != w0->asym) return false;
   }
   if (!(w0->comp == NS_COMP_Q8_0 || w0->comp == NS_COMP_INT8 || w0->comp == NS_COMP_INT8_S8)) return false;
   if (!(w0->group == 32 || w0->group == 64 || w0->group == 128 || w0->group == 256) || w0->k % w0->group) return false;
@@ -633,7 +689,10 @@ int ns_launch_gemm_imma(const ns_weight* const* ws, int nw, int mode, const floa
     const int warps = pl.mt * nblk;
     const dim3 grid((unsigned)((warps + 7) / 8)), block(256);
     cudaError_t e;
-    if (w0->comp == NS_COMP_Q8_0)
+    if (w0->wfmt == NS_W_Q8_0)
+      e = ns_launch_pdl(act_quant_imma_kernel<NS_COMP_Q8_0, true>, grid, block, 0, st, act, lda, m, w0->k, qg, pl.mt, pl.nslices, img, tickets,
+                        pl.tiles);
+    else if (w0->comp == NS_COMP_Q8_0)
       e = ns_launch_pdl(act_quant_imma_kernel<NS_COMP_Q8_0>, grid, block, 0, st, act, lda, m, w0->k, qg, pl.mt, pl.nslices, img, tickets, pl.tiles);
     else if (w0->comp == NS_COMP_INT8)
       e = ns_launch_pdl(act_quant_imma_kernel<NS_COMP_INT8>, grid, block, 0, st, act, lda, m, w0->k, qg, pl.mt, pl.nslices, img, tickets, pl.tiles);
@@ -694,6 +753,7 @@ int ns_launch_gemm_imma(const ns_weight* const* ws, int nw, int mode, const floa
     fprintf(stderr, "gemm_imma: m=%d mt=%d k=%d g=%d tiles=%d ksplit=%d stages=%d smem=%zu sc_row=%d\n", m, pl.mt, w0->k, w0->group, pl.tiles,
             pl.ksplit, pl.stages, pl.smem, pl.sc_row);
   const bool asym = w0->asym != 0;
+  if (w0->wfmt == NS_W_Q8_0) return launch_q8_0(maps, P, pl, st);
   if (w0->comp == NS_COMP_INT8)
     return asym ? launch_m<true, true>(maps, P, pl, w0->stype, st) : launch_m<true, false>(maps, P, pl, w0->stype, st);
   return asym ? launch_m<false, true>(maps, P, pl, w0->stype, st) : launch_m<false, false>(maps, P, pl, w0->stype, st);

@@ -415,7 +415,7 @@ int launch_t(const CUtensorMap& mw, const CUtensorMap& ma, const GemmParams& P, 
 size_t ns_gemm_tc_workspace_bytes(int m, int kpad) { return ns_round_up((size_t)m * kpad * 2, 256); }
 
 bool ns_gemm_tc_supported(const ns_weight* w) {
-  return (w->wfmt == NS_W_S4 || w->wfmt == NS_W_NF4 || w->wfmt == NS_W_S8) && (w->group % 32 == 0 || w->group == w->k);
+  return (w->wfmt == NS_W_S4 || w->wfmt == NS_W_NF4 || w->wfmt == NS_W_S8 || w->wfmt == NS_W_Q8_0) && (w->group % 32 == 0 || w->group == w->k);
 }
 
 // phase 1: fp32 activations -> bf16 [m][kpad] in ws (ns_gemm_tc_workspace_bytes(m, kpad) bytes)
@@ -528,12 +528,12 @@ int ns_launch_gelu(float* x, size_t total, cudaStream_t st) {
 int ns_launch_gemm_tc(const ns_weight* w, const void* ws, float* dst, int ldo, int m, const float* bias, int bias_bcast,
                       const float* residual, cudaStream_t st) {
   if (!ns_gemm_tc_supported(w)) {
-    ns_set_error("tensor-core GEMM: int4 / NF4 / int8 weights with 32-multiple groups are supported");
+    ns_set_error("tensor-core GEMM: int4 / NF4 / int8 / Q8_0 weights with 32-multiple groups are supported");
     return NS_E_UNSUPPORTED;
   }
   const __nv_bfloat16* abf = (const __nv_bfloat16*)ws;
   const int T = m <= 32 ? 32 : (m <= 64 ? 64 : 128);
-  const bool w8 = w->wfmt == NS_W_S8;
+  const bool w8 = w->wfmt == NS_W_S8 || w->wfmt == NS_W_Q8_0;  // natural-order int8 codes (ggml Q8_0: zero point 0, fp16 d)
   CUtensorMap mw, ma;
   // packed nibbles: uint8 [n][q_bytes] with row pitch `pitch`; box = 32 bytes (64 k) x 128 rows, no swizzle
   int rc = ns_tensor_map_2d(&mw, CU_TENSOR_MAP_DATA_TYPE_UINT8, w->rows, w->q_bytes, w->n, w->pitch, w8 ? BLOCK_K : BLOCK_K / 2, BLOCK_N,

@@ -1,5 +1,5 @@
 // gemv.cu -- decode-shape (M <= 4) weight-only matmul: launcher + the register-staged GEMV used for the formats the
-// TMA-ring kernel (gemv_ring.cu) does not cover: fp32/bf16 compute (BesTLA CompFp32/CompBf16), NF4 and 8-bit weights.
+// TMA-ring kernel (gemv_ring.cu) does not cover: fp32/bf16 compute (BesTLA CompFp32/CompBf16), NF4 and BesTLA 8-bit weights.
 //
 // Replaces, for M <= 4 (the reference's own GEMV cut-off, bestla_wrapper.h:283/568 "M<=4"):
 //   ggml   ne_compute_forward_mul_mat_q_f32 + ne_vec_dot_q4_0_q8_0   (core/ne_layers.c:7085, core/layers/vec_dot.h:131)
@@ -348,7 +348,7 @@ int launch_asym(const GemvParams& P, bool asym, int mt, size_t smem, cudaStream_
 
 // Bytes of one activation row in the register GEMV's shared-memory image (fp32 values, or int8 codes + chunk meta)
 size_t act_row_bytes(const ns_weight* w) {
-  return (w->wfmt == NS_W_S4) ? ns_round_up((size_t)w->kpad, 1024) : (size_t)w->kpad;
+  return (w->wfmt == NS_W_S4 || w->wfmt == NS_W_Q8_0) ? ns_round_up((size_t)w->kpad, 1024) : (size_t)w->kpad;
 }
 bool float_mode(const ns_weight* w) { return w->comp == NS_COMP_F32 || w->comp == NS_COMP_BF16; }
 // Dynamic shared memory of a register-GEMV launch with an mt-row kernel template
@@ -375,7 +375,7 @@ int ns_gemv_tile_rows(const ns_weight* w) {
 // One tile: m <= ns_gemv_tile_rows(w).  act_ws is the image ns_launch_act_prep produced for exactly these m rows.
 // dst points at the tile's first output row; m_total is the full M (only used for the [nw][M][ldo] QKV layout).
 bool ns_gemv_fused_quant_ok(const ns_weight* w) {
-  if (w->wfmt != NS_W_S4 || w->shuffle) return false;
+  if (!(w->wfmt == NS_W_S4 || w->wfmt == NS_W_Q8_0) || w->shuffle) return false;
   if (!(w->comp == NS_COMP_Q8_0 || w->comp == NS_COMP_INT8 || w->comp == NS_COMP_INT8_S8)) return false;
   const int qg = w->comp == NS_COMP_Q8_0 ? 32 : w->group;  // one activation block must sit inside one warp
   return (qg == 32 || qg == 64 || qg == 128 || qg == 256) && w->k % qg == 0;
@@ -413,7 +413,7 @@ int ns_gemv_check(const ns_weight* const* ws_, int nw, int mode) {
       return NS_E_UNSUPPORTED;
     }
   // the register GEMV stages a whole activation row in shared memory: fp32 compute takes K <= 51200
-  if (!(w0->wfmt == NS_W_S4 && !float_mode(w0)) && gemv_smem(w0, 1) > kSmemMax) {
+  if (!ns_ring_format(w0) && gemv_smem(w0, 1) > kSmemMax) {
     ns_set_error("GEMV: one activation row of k=%d needs %zu B of shared memory, more than the %zu B the kernel has", w0->k,
                  gemv_smem(w0, 1), kSmemMax);
     return NS_E_UNSUPPORTED;
@@ -424,7 +424,7 @@ int ns_gemv_check(const ns_weight* const* ws_, int nw, int mode) {
 int ns_gemv_planned(const ns_weight* const* ws, int nw, int mode, int m, bool norm) {
   const ns_weight* w0 = ws[0];
   (void)nw;
-  if (!(w0->wfmt == NS_W_S4 && !float_mode(w0))) return NS_OK;  // the register GEMV: ns_gemv_check has sized its launch
+  if (!ns_ring_format(w0)) return NS_OK;  // the register GEMV: ns_gemv_check has sized its launch
   const int tile = ns_gemv_tile_rows(w0);
   const bool fused = ns_gemv_fused_quant_ok(w0);
   const int rows[2] = {m < tile ? m : tile, m % tile};  // the full tiles and the last one
@@ -515,6 +515,7 @@ int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* ac
   const size_t smem = gemv_smem(w0, mt);
   const bool asym = w0->asym != 0;
   if (w0->wfmt == NS_W_S4 && !fmode) return ns_launch_gemv_ring(P, amode, asym, mt, st);  // the hot decode path
+  if (w0->wfmt == NS_W_Q8_0) return ns_launch_gemv_ring_q8_0(P, mt, st);                    // its 8-bit-code form
   if (w0->wfmt == NS_W_S4) return launch_asym<NS_W_S4, A_F32>(P, asym, mt, smem, st);
   if (w0->wfmt == NS_W_S8) {
     return amode == A_F32  ? launch_asym<NS_W_S8, A_F32>(P, asym, mt, smem, st)

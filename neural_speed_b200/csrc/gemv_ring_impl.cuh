@@ -103,7 +103,8 @@ __device__ __forceinline__ void load_passes(const float* row, int eb, int tid, i
 
 // Called by the NT consumer threads (whole warps, named barrier 1).  A thread owns one 8-group (8 consecutive k); group/8
 // consecutive threads own one quantisation block.  NORM: red is shared float[NT/32], gw prefetch_norm_w's registers or NULL.
-template <int COMP, int NT, bool NORM>
+// NAT: the codes keep natural order inside their chunk (8-bit weights, act_prep.cu's perm8 = 0), else the NSB4 pairing order.
+template <int COMP, int NT, bool NORM, bool NAT = false>
 __device__ __forceinline__ void quantise_to_smem(const QuantIn& P, int M, uint32_t smem_base, float* red, const float (*gw)[8]) {
   constexpr int NI = 3;  // load passes kept in registers (3 x 512 threads x 8 = 12288 elements)
   const int tpb = (COMP == NS_COMP_Q8_0 ? 32 : P.group) >> 3;  // threads per quantisation block (4..32, power of two)
@@ -187,7 +188,10 @@ __device__ __forceinline__ void quantise_to_smem(const QuantIn& P, int M, uint32
         if (live) {
           uint32_t w[2] = {0u, 0u};
 #pragma unroll
-          for (int i = 0; i < 8; ++i) w[nsq::dp4a_pos(i) >> 2] |= (uint32_t)(q[i] & 0xff) << (8 * (nsq::dp4a_pos(i) & 3));
+          for (int i = 0; i < 8; ++i) {
+            const int pos = NAT ? i : nsq::dp4a_pos(i);
+            w[pos >> 2] |= (uint32_t)(q[i] & 0xff) << (8 * (pos & 3));
+          }
           const int c = e >> 2, i = e & 3;
           sts64(img + nsq::ring_offset((uint32_t)c, (uint32_t)i * 8u), w[0], w[1]);
           if (i == 0) {
@@ -262,12 +266,52 @@ __device__ __forceinline__ PairSrc resolve_single(const GemvParams& P, int u) {
   return s;
 }
 
+// The consumer loop over one ring stage for 8-bit codes (ggml Q8_0: symmetric, one fp16 scale per 32-chunk).  A chunk is 32
+// natural-order code bytes against the natural-order activation image (bytes 0..15 at nsq::ring_offset(c, 0), 16..31 at + 512),
+// so isum_c = sum a*q is one chain of eight s8 x s8 dp4a -- no nibble expansion, no offset term -- and the accumulation is the
+// 4-bit path's: acc = fmaf(isum_c, fp32(a_scale * w_scale), acc) over c = lane, lane + 32, ...
+template <int M, int ROWS, int STYPE>
+__device__ __forceinline__ void ring_chunks_w8(const GemvParams& P, const RingCfg& R, const uint32_t (&rb)[2], uint32_t smem_base,
+                                               uint32_t meta_s, int nchunks, int lane, float (&acc)[ROWS][M]) {
+#pragma unroll 2
+  for (int c = lane; c < nchunks; c += 32) {
+    uint4 wl[ROWS], wh[ROWS];
+    float ws[ROWS];
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) {
+      wl[r] = lds128(rb[r] + 32 * c);
+      wh[r] = lds128(rb[r] + 32 * c + 16);
+      ws[r] = lds_scale<STYPE>(rb[r] + P.sc_off, c);
+    }
+    const uint32_t a_off = (uint32_t)(c >> 5) * 1024u + (uint32_t)(c & 31) * 16u;
+#pragma unroll
+    for (int m = 0; m < M; ++m) {
+      const uint32_t ab = smem_base + (uint32_t)m * R.act_row + a_off;
+      const uint4 a0 = lds128(ab), a1 = lds128(ab + 512);
+      const float a_scale = __uint_as_float(lds64(meta_s + 8u * (uint32_t)(m * P.meta_stride + c)).x);
+#pragma unroll
+      for (int r = 0; r < ROWS; ++r) {
+        int isum = dp4a_ss((int)wl[r].x, (int)a0.x, 0);
+        isum = dp4a_ss((int)wl[r].y, (int)a0.y, isum);
+        isum = dp4a_ss((int)wl[r].z, (int)a0.z, isum);
+        isum = dp4a_ss((int)wl[r].w, (int)a0.w, isum);
+        isum = dp4a_ss((int)wh[r].x, (int)a1.x, isum);
+        isum = dp4a_ss((int)wh[r].y, (int)a1.y, isum);
+        isum = dp4a_ss((int)wh[r].z, (int)a1.z, isum);
+        isum = dp4a_ss((int)wh[r].w, (int)a1.w, isum);
+        acc[r][m] = fmaf((float)isum, a_scale * ws[r], acc[r][m]);  // |isum| <= 32 * 128 * 127: exact in fp32
+      }
+    }
+  }
+}
+
 // NORM: the fused-RMSNorm prologue is a separate instantiation, so the plain kernels (the headline path) keep the code and the
 // register allocation they had without it
 // NC consumer warps: 7 (+1 producer warp, two CTAs per SM) or 14 (+2 producer warps, ONE CTA per SM: the activation row is pulled
 // through L2 and quantised once per SM instead of twice -- the 16-44 KB broadcast to every CTA is what separates the fused launch
 // list from the pre-quantised one; the two producer warps take alternate ring stages)
-template <int AMODE, int M, bool ASYM, int STYPE, int ROWS, bool NORM, int NC>
+// W8: 8-bit codes (ggml Q8_0; instantiated with A_S8, symmetric, fp16 scales only), ring_chunks_w8 instead of the nibble loop
+template <int AMODE, int M, bool ASYM, int STYPE, int ROWS, bool NORM, int NC, bool W8 = false>
 __global__ void __launch_bounds__((NC + (NC > kConsumers ? 2 : 1)) * 32, NC > kConsumers ? 1 : 2)
     gemv_ring_kernel(const GemvParams P, const RingCfg R) {
   constexpr int NP = NC > kConsumers ? 2 : 1;  // producer warps
@@ -334,9 +378,13 @@ __global__ void __launch_bounds__((NC + (NC > kConsumers ? 2 : 1)) * 32, NC > kC
                      R.act_row, P.meta_off, P.meta_stride};
     float* red = reinterpret_cast<float*>(smem + R.red_off);
     const float(*gwp)[8] = gw_pref ? gw : nullptr;
-    if (AMODE == A_U8) quantise_to_smem<NS_COMP_INT8, NC * 32, NORM>(qi, P.m, smem_base, red, gwp);
-    else if (P.comp == NS_COMP_Q8_0) quantise_to_smem<NS_COMP_Q8_0, NC * 32, NORM>(qi, P.m, smem_base, red, gwp);
-    else quantise_to_smem<NS_COMP_INT8_S8, NC * 32, NORM>(qi, P.m, smem_base, red, gwp);
+    if constexpr (W8) {
+      quantise_to_smem<NS_COMP_Q8_0, NC * 32, NORM, true>(qi, P.m, smem_base, red, gwp);
+    } else {
+      if (AMODE == A_U8) quantise_to_smem<NS_COMP_INT8, NC * 32, NORM>(qi, P.m, smem_base, red, gwp);
+      else if (P.comp == NS_COMP_Q8_0) quantise_to_smem<NS_COMP_Q8_0, NC * 32, NORM>(qi, P.m, smem_base, red, gwp);
+      else quantise_to_smem<NS_COMP_INT8_S8, NC * 32, NORM>(qi, P.m, smem_base, red, gwp);
+    }
   } else {
     const uint4* src = reinterpret_cast<const uint4*>(P.act);
     uint4* dstv = reinterpret_cast<uint4*>(smem);
@@ -367,72 +415,76 @@ __global__ void __launch_bounds__((NC + (NC > kConsumers ? 2 : 1)) * 32, NC > kC
 #pragma unroll
       for (int m = 0; m < M; ++m) acc[r][m] = 0.f;
 
+    if constexpr (W8) {
+      ring_chunks_w8<M, ROWS, STYPE>(P, R, rb, smem_base, meta_s, nchunks, lane, acc);
+    } else {
 #pragma unroll 2
-    for (int c = lane; c < nchunks; c += 32) {
-      const int gi = (P.cpg == 1) ? c : (int)__umulhi((uint32_t)c, R.cpg_magic);
-      uint4 wv[ROWS];
-      float ws[ROWS];
-      int off[ROWS];
-#pragma unroll
-      for (int r = 0; r < ROWS; ++r) {
-        wv[r] = lds128(rb[r] + 16 * c);
-        ws[r] = lds_scale<STYPE>(rb[r] + P.sc_off, gi);
-        off[r] = 8;
-        if (ASYM) off[r] += lds8s(rb[r] + P.zp_off + gi);
-      }
-      // low nibbles as bytes, high nibbles as bytes * 16 (no shift): exact, divided out after the dot
-      uint32_t lo[ROWS][4], hi[ROWS][4];
-      int su[ROWS];
-#pragma unroll
-      for (int r = 0; r < ROWS; ++r) {
-        su[r] = 0;
-        const uint32_t ww[4] = {wv[r].x, wv[r].y, wv[r].z, wv[r].w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          lo[r][i] = ww[i] & 0x0F0F0F0Fu;
-          hi[r][i] = ww[i] & 0xF0F0F0F0u;
-        }
-        if (AMODE == A_U8) {  // sum of the weight codes, needed for the activation zero point
-          int sl = 0, sh = 0;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            sl = dp4a_uu(lo[r][i], 0x01010101u, sl);
-            sh = dp4a_uu(hi[r][i], 0x01010101u, sh);
-          }
-          su[r] = sl + (sh >> 4);
-        }
-      }
-      // activation image: bytes 0..15 and 16..31 of chunk c at nsq::ring_offset(c, 0) and + 512 (act_quant.cuh)
-      const uint32_t a_off = (uint32_t)(c >> 5) * 1024u + (uint32_t)(c & 31) * 16u;
-#pragma unroll
-      for (int m = 0; m < M; ++m) {
-        const uint32_t ab = smem_base + (uint32_t)m * R.act_row + a_off;
-        const uint4 a0 = lds128(ab), a1 = lds128(ab + 512);
-        const uint2 mt = lds64(meta_s + 8u * (uint32_t)(m * P.meta_stride + c));
-        const float a_scale = __uint_as_float(mt.x);
-        const int sa = (int)(short)(mt.y & 0xffff);
+      for (int c = lane; c < nchunks; c += 32) {
+        const int gi = (P.cpg == 1) ? c : (int)__umulhi((uint32_t)c, R.cpg_magic);
+        uint4 wv[ROWS];
+        float ws[ROWS];
+        int off[ROWS];
 #pragma unroll
         for (int r = 0; r < ROWS; ++r) {
-          int pl = 0, ph = 0;
-          // NSB4: word i pairs with activation words (Alo_i, Ahi_i) = ((a0,a4,a1,a5),(a2,a6,a3,a7)) of 8-group i
-          if (AMODE == A_U8) {
-            pl = dp4a_uu(a0.x, lo[r][0], pl); ph = dp4a_uu(a0.y, hi[r][0], ph);
-            pl = dp4a_uu(a0.z, lo[r][1], pl); ph = dp4a_uu(a0.w, hi[r][1], ph);
-            pl = dp4a_uu(a1.x, lo[r][2], pl); ph = dp4a_uu(a1.y, hi[r][2], ph);
-            pl = dp4a_uu(a1.z, lo[r][3], pl); ph = dp4a_uu(a1.w, hi[r][3], ph);
-          } else {  // signed activations x unsigned weight bytes
-            pl = dp4a_us(lo[r][0], (int)a0.x, pl); ph = dp4a_us(hi[r][0], (int)a0.y, ph);
-            pl = dp4a_us(lo[r][1], (int)a0.z, pl); ph = dp4a_us(hi[r][1], (int)a0.w, ph);
-            pl = dp4a_us(lo[r][2], (int)a1.x, pl); ph = dp4a_us(hi[r][2], (int)a1.y, ph);
-            pl = dp4a_us(lo[r][3], (int)a1.z, pl); ph = dp4a_us(hi[r][3], (int)a1.w, ph);
+          wv[r] = lds128(rb[r] + 16 * c);
+          ws[r] = lds_scale<STYPE>(rb[r] + P.sc_off, gi);
+          off[r] = 8;
+          if (ASYM) off[r] += lds8s(rb[r] + P.zp_off + gi);
+        }
+        // low nibbles as bytes, high nibbles as bytes * 16 (no shift): exact, divided out after the dot
+        uint32_t lo[ROWS][4], hi[ROWS][4];
+        int su[ROWS];
+#pragma unroll
+        for (int r = 0; r < ROWS; ++r) {
+          su[r] = 0;
+          const uint32_t ww[4] = {wv[r].x, wv[r].y, wv[r].z, wv[r].w};
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            lo[r][i] = ww[i] & 0x0F0F0F0Fu;
+            hi[r][i] = ww[i] & 0xF0F0F0F0u;
           }
-          // sum (a - za)(u - off) = sum a*u - off*Sa - za*(Su - 32*off): one exact integer per 32-element chunk
-          int isum = pl + (ph >> 4) - off[r] * sa;  // ph is an exact multiple of 16
-          if (AMODE == A_U8) {
-            const int za = (int)((mt.y >> 16) & 0xff);
-            isum -= za * (su[r] - 32 * off[r]);
+          if (AMODE == A_U8) {  // sum of the weight codes, needed for the activation zero point
+            int sl = 0, sh = 0;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              sl = dp4a_uu(lo[r][i], 0x01010101u, sl);
+              sh = dp4a_uu(hi[r][i], 0x01010101u, sh);
+            }
+            su[r] = sl + (sh >> 4);
           }
-          acc[r][m] = fmaf((float)isum, a_scale * ws[r], acc[r][m]);
+        }
+        // activation image: bytes 0..15 and 16..31 of chunk c at nsq::ring_offset(c, 0) and + 512 (act_quant.cuh)
+        const uint32_t a_off = (uint32_t)(c >> 5) * 1024u + (uint32_t)(c & 31) * 16u;
+#pragma unroll
+        for (int m = 0; m < M; ++m) {
+          const uint32_t ab = smem_base + (uint32_t)m * R.act_row + a_off;
+          const uint4 a0 = lds128(ab), a1 = lds128(ab + 512);
+          const uint2 mt = lds64(meta_s + 8u * (uint32_t)(m * P.meta_stride + c));
+          const float a_scale = __uint_as_float(mt.x);
+          const int sa = (int)(short)(mt.y & 0xffff);
+#pragma unroll
+          for (int r = 0; r < ROWS; ++r) {
+            int pl = 0, ph = 0;
+            // NSB4: word i pairs with activation words (Alo_i, Ahi_i) = ((a0,a4,a1,a5),(a2,a6,a3,a7)) of 8-group i
+            if (AMODE == A_U8) {
+              pl = dp4a_uu(a0.x, lo[r][0], pl); ph = dp4a_uu(a0.y, hi[r][0], ph);
+              pl = dp4a_uu(a0.z, lo[r][1], pl); ph = dp4a_uu(a0.w, hi[r][1], ph);
+              pl = dp4a_uu(a1.x, lo[r][2], pl); ph = dp4a_uu(a1.y, hi[r][2], ph);
+              pl = dp4a_uu(a1.z, lo[r][3], pl); ph = dp4a_uu(a1.w, hi[r][3], ph);
+            } else {  // signed activations x unsigned weight bytes
+              pl = dp4a_us(lo[r][0], (int)a0.x, pl); ph = dp4a_us(hi[r][0], (int)a0.y, ph);
+              pl = dp4a_us(lo[r][1], (int)a0.z, pl); ph = dp4a_us(hi[r][1], (int)a0.w, ph);
+              pl = dp4a_us(lo[r][2], (int)a1.x, pl); ph = dp4a_us(hi[r][2], (int)a1.y, ph);
+              pl = dp4a_us(lo[r][3], (int)a1.z, pl); ph = dp4a_us(hi[r][3], (int)a1.w, ph);
+            }
+            // sum (a - za)(u - off) = sum a*u - off*Sa - za*(Su - 32*off): one exact integer per 32-element chunk
+            int isum = pl + (ph >> 4) - off[r] * sa;  // ph is an exact multiple of 16
+            if (AMODE == A_U8) {
+              const int za = (int)((mt.y >> 16) & 0xff);
+              isum -= za * (su[r] - 32 * off[r]);
+            }
+            acc[r][m] = fmaf((float)isum, a_scale * ws[r], acc[r][m]);
+          }
         }
       }
     }
@@ -481,9 +533,9 @@ __global__ void __launch_bounds__((NC + (NC > kConsumers ? 2 : 1)) * 32, NC > kC
   }
 }
 
-template <int AMODE, int M, bool ASYM, int STYPE, int ROWS, bool NORM, int NC = kConsumers>
+template <int AMODE, int M, bool ASYM, int STYPE, int ROWS, bool NORM, int NC = kConsumers, bool W8 = false>
 int launch_rows(const GemvParams& P, const RingPlan& plan, size_t act_region, int act_row, int red_off, cudaStream_t st) {
-  auto kern = gemv_ring_kernel<AMODE, M, ASYM, STYPE, ROWS, NORM, NC>;
+  auto kern = gemv_ring_kernel<AMODE, M, ASYM, STYPE, ROWS, NORM, NC, W8>;
   constexpr int threads = (NC + (NC > kConsumers ? 2 : 1)) * 32;
   static bool attr_set = false;
   if (!attr_set) {

@@ -9,7 +9,7 @@
 
 namespace {
 
-template <int AMODE, bool ASYM, int STYPE>
+template <int AMODE, bool ASYM, int STYPE, bool W8 = false>
 int wide_launch(const GemvParams& P, const RingChoice& c, cudaStream_t st) {
   const RingPlan& wp = c.plan;
   const size_t act_region = c.act_region;
@@ -21,10 +21,10 @@ int wide_launch(const GemvParams& P, const RingChoice& c, cudaStream_t st) {
   const bool nrm = (P.norm_w || P.one_image) && P.act_f32;
   constexpr int NC = 2 * kConsumers;
   if (wp.rows == 2)
-    return nrm ? launch_rows<AMODE, 1, ASYM, STYPE, 2, true, NC>(P, wp, act_region, act_row, red_off, st)
-               : launch_rows<AMODE, 1, ASYM, STYPE, 2, false, NC>(P, wp, act_region, act_row, red_off, st);
-  return nrm ? launch_rows<AMODE, 1, ASYM, STYPE, 1, true, NC>(P, wp, act_region, act_row, red_off, st)
-             : launch_rows<AMODE, 1, ASYM, STYPE, 1, false, NC>(P, wp, act_region, act_row, red_off, st);
+    return nrm ? launch_rows<AMODE, 1, ASYM, STYPE, 2, true, NC, W8>(P, wp, act_region, act_row, red_off, st)
+               : launch_rows<AMODE, 1, ASYM, STYPE, 2, false, NC, W8>(P, wp, act_region, act_row, red_off, st);
+  return nrm ? launch_rows<AMODE, 1, ASYM, STYPE, 1, true, NC, W8>(P, wp, act_region, act_row, red_off, st)
+             : launch_rows<AMODE, 1, ASYM, STYPE, 1, false, NC, W8>(P, wp, act_region, act_row, red_off, st);
 }
 
 template <int AMODE, bool ASYM>
@@ -42,4 +42,8 @@ int wide_s(const GemvParams& P, const RingChoice& c, cudaStream_t st) {
 int ns_launch_gemv_ring_wide(const GemvParams& P, int amode, bool asym, const RingChoice& c, cudaStream_t st) {
   if (amode == A_U8) return asym ? wide_s<A_U8, true>(P, c, st) : wide_s<A_U8, false>(P, c, st);
   return asym ? wide_s<A_S8, true>(P, c, st) : wide_s<A_S8, false>(P, c, st);
+}
+// ggml Q8_0 (8-bit codes): s8 activations, symmetric, fp16 scales
+int ns_launch_gemv_ring_wide_q8_0(const GemvParams& P, const RingChoice& c, cudaStream_t st) {
+  return wide_launch<A_S8, false, NS_S_F16, true>(P, c, st);
 }

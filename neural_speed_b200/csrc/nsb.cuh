@@ -13,6 +13,9 @@
 //   -- one op per bf16x2 pair for the tensor-core dequant -- and w & 0x0F0F0F0F / (w>>4) & 0x0F0F0F0F yield bytes
 //   (e0,e4,e1,e5) / (e2,e6,e3,e7) for dp4a against activations stored in the same permuted order.
 //   Stored nibble u = q + 8 (ints) or the NF4 code; value semantics w = (u - 8 - zp) * scale.
+//   8-bit q (NS_W_S8, NS_W_Q8_0): natural order, byte k of the row is element k (int8), w = (q - zp) * scale.  A ggml Q8_0 row
+//   is block_q8_0's 32 codes of every block back to back, then the blocks' fp16 d: the activation images keep natural order
+//   for it too (perm8 = 0), so one byte order serves the ring GEMV's dp4a, the IMMA fragments and the wgmma dequant.
 //   shuffle [K] int32 (GPTQ desc_act): activation column gather applied before activation quantisation.
 #pragma once
 #include <cuda_bf16.h>
@@ -40,13 +43,17 @@ enum { NS_F4_NF4 = 0, NS_F4_BNB = 1, NS_F4_E2M1 = 2 };
 
 static inline size_t ns_round_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 static inline int ns_stype_size(int stype) { return stype == NS_S_F32 ? 4 : 2; }
+// the weights the ring GEMV takes: int4 codes with an integer compute type, and ggml Q8_0
+static inline bool ns_ring_format(const ns_weight* w) {
+  return w->wfmt == NS_W_Q8_0 || (w->wfmt == NS_W_S4 && !(w->comp == NS_COMP_F32 || w->comp == NS_COMP_BF16));
+}
 
 // fills kpad/group/ngroups/pitch/offsets from n,k,group,wfmt,stype,asym
 static inline void ns_weight_layout(ns_weight* w) {
   w->kpad = (int)ns_round_up((size_t)w->k, 32);
   if (w->group <= 0 || w->group > w->k) w->group = w->k;
   w->ngroups = (w->k + w->group - 1) / w->group;
-  w->q_bytes = (w->wfmt == NS_W_S8) ? w->kpad : w->kpad / 2;
+  w->q_bytes = (w->wfmt == NS_W_S8 || w->wfmt == NS_W_Q8_0) ? w->kpad : w->kpad / 2;
   w->sc_off = w->q_bytes;
   w->zp_off = (int)ns_round_up((size_t)w->sc_off + (size_t)w->ngroups * ns_stype_size(w->stype), 16);  // TMA-copyable
   w->pitch = (int)ns_round_up((size_t)w->zp_off + (w->asym ? w->ngroups : 0), 16);
@@ -82,6 +89,7 @@ int ns_launch_gemv(const ns_weight* const* ws_, int nw, int mode, const void* ac
 bool ns_gemv_fused_quant_ok(const ns_weight* w);  // can the GEMV quantise the activations itself (one launch)?
 int ns_gemv_check(const ns_weight* const* ws, int nw, int mode);  // can these weights share one GEMV launch? NS_OK or the error
 int ns_launch_repack_q4_0(const void* rows_dev, size_t nb01, ns_weight* w, cudaStream_t st);
+int ns_launch_repack_q8_0(const void* rows_dev, size_t nb01, ns_weight* w, cudaStream_t st);
 int ns_launch_repack_canonical(const int8_t* q_kn_dev, const float* sc_dev, const int8_t* zp_dev, ns_weight* w,
                                cudaStream_t st);
 int ns_launch_repack_btla(const void* qbuf_dev, const void* sc_dev, int src_stype, const int8_t* zp_dev, int cstep,
@@ -191,6 +199,9 @@ struct RingChoice {
 bool ns_gemv_ring_choose(int kpad, int pitch, int mode, int mt, bool fused, bool norm, RingChoice* c);  // gemv_ring.cu
 int ns_launch_gemv_ring(const GemvParams& P, int amode, bool asym, int mt, cudaStream_t st);                       // gemv_ring.cu
 int ns_launch_gemv_ring_wide(const GemvParams& P, int amode, bool asym, const RingChoice& c, cudaStream_t st);  // gemv_ring_wide.cu
+// ggml Q8_0 weights (8-bit codes x Q8_0 activations, fp16 scales, symmetric): the same ring, its own instantiations
+int ns_launch_gemv_ring_q8_0(const GemvParams& P, int mt, cudaStream_t st);                                      // gemv_ring.cu
+int ns_launch_gemv_ring_wide_q8_0(const GemvParams& P, const RingChoice& c, cudaStream_t st);                   // gemv_ring_wide.cu
 // NS_OK when every GEMV tile of an m-row launch of these weights has a kernel plan, else NS_E_UNSUPPORTED naming the ring (gemv.cu)
 int ns_gemv_planned(const ns_weight* const* ws, int nw, int mode, int m, bool norm);
 

@@ -5,6 +5,7 @@
 // uploaded verbatim and one kernel rewrites it N-major with K-contiguous nibbles and transposed scales.
 // Sources handled:
 //   * ggml rows of block_q4_0 (core/data_types.h:79-83: fp16 d + 16 bytes; byte j = elem j | elem j+16 << 4)
+//   * ggml rows of block_q8_0 (core/data_types.h:107-111: fp16 d + 32 int8 codes, element j in byte j)
 //   * canonical container  q int8 [K][N], scales f32 [K/g][N], zp int8 [K/g][N]   (what BTLAGemmPackB takes)
 //   * serialized BesTLA blob: QBuf nibbles in [N/NTile][KPad/PackRow][NTile][PackRow] order
 //     (bestla_prologue_b.h:490-510 reorderWeight + kernel_ref.h:40-58 padding_interleave + :155 compress_s8_s4),
@@ -44,6 +45,22 @@ __global__ void repack_q4_0_kernel(const uint8_t* __restrict__ rows, size_t nb01
   }
   *reinterpret_cast<uint4*>(q + (size_t)row * row_bytes + (size_t)b * 16) = make_uint4(w[0], w[1], w[2], w[3]);
   *reinterpret_cast<unsigned short*>(q + (size_t)row * row_bytes + sc_off + (size_t)b * 2) = h[0];
+}
+
+// ---- ggml Q8_0 rows -> NSB: one thread per block; the 32 codes keep their order, d goes to the scale array ------------
+__global__ void repack_q8_0_kernel(const uint8_t* __restrict__ rows, size_t nb01, int n, int nblocks,
+                                   uint8_t* __restrict__ q, size_t row_bytes, int sc_off) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (size_t)n * nblocks) return;
+  const int row = (int)(idx / nblocks), b = (int)(idx - (size_t)row * nblocks);
+  const unsigned short* src = reinterpret_cast<const unsigned short*>(rows + (size_t)row * nb01 + (size_t)b * 34);
+  uint32_t w[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) w[i] = (uint32_t)src[1 + 2 * i] | ((uint32_t)src[2 + 2 * i] << 16);
+  uint4* dst = reinterpret_cast<uint4*>(q + (size_t)row * row_bytes + (size_t)b * 32);
+  dst[0] = make_uint4(w[0], w[1], w[2], w[3]);
+  dst[1] = make_uint4(w[4], w[5], w[6], w[7]);
+  *reinterpret_cast<unsigned short*>(q + (size_t)row * row_bytes + sc_off + (size_t)b * 2) = src[0];
 }
 
 // ---- generic element accessors ---------------------------------------------------------------------------------------
@@ -146,7 +163,7 @@ __global__ void dequant_kernel(const uint8_t* __restrict__ rows, size_t pitch, i
   const float s = ns_scale_at(r + sc_off, stype, gi);
   const int z = asym ? (int)(signed char)r[zp_off + gi] : 0;
   float v;
-  if (wfmt == NS_W_S8) {
+  if (wfmt == NS_W_S8 || wfmt == NS_W_Q8_0) {  // Q8_0: fp32(d) * q, dequantize_row_q8_0 (quantize.h:780)
     v = (float)((int)(signed char)r[kk] - z) * s;
   } else {
     const uint32_t w = *reinterpret_cast<const uint32_t*>(r + (size_t)(kk >> 3) * 4);
@@ -204,6 +221,16 @@ int ns_launch_repack_q4_0(const void* rows_dev, size_t nb01, ns_weight* w, cudaS
   const int nblocks = w->k / 32;
   const size_t total = (size_t)w->n * nblocks;
   repack_q4_0_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const uint8_t*)rows_dev, nb01, w->n, nblocks,
+                                                                      w->rows, (size_t)w->pitch, w->sc_off);
+  NS_CUDA_TRY(cudaGetLastError());
+  ns_count_launch();
+  return NS_OK;
+}
+
+int ns_launch_repack_q8_0(const void* rows_dev, size_t nb01, ns_weight* w, cudaStream_t st) {
+  const int nblocks = w->k / 32;
+  const size_t total = (size_t)w->n * nblocks;
+  repack_q8_0_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const uint8_t*)rows_dev, nb01, w->n, nblocks,
                                                                       w->rows, (size_t)w->pitch, w->sc_off);
   NS_CUDA_TRY(cudaGetLastError());
   ns_count_launch();

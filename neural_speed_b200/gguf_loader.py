@@ -5,9 +5,10 @@ infos, aligned data) and maps llama tensors to `model.others[0..2]` / `layers[il
 Here the container is parsed with the `gguf` Python package (the format's own reader) and the tensors are handed over in the
 types the eval step consumes:
 
-  token_embd.weight   F32/F16/Q4_0 -> fp32 table (the reference's ne_get_rows dequantises the looked-up rows; same values)
+  token_embd.weight   F32/F16/Q4_0/Q8_0 -> fp32 table (the reference's ne_get_rows dequantises the looked-up rows; same values)
   *_norm.weight       F32
-  attn_q/k/v/output, ffn_gate/down/up, output.weight   Q4_0 rows (18-byte blocks) or Q6_K rows (210-byte blocks), untouched
+  attn_q/k/v/output, ffn_gate/down/up, output.weight   Q4_0 rows (18-byte blocks), Q8_0 rows (34-byte blocks) or Q6_K rows
+                      (210-byte blocks), untouched
 
 Host logic only (numpy); `parse()` is covered on CPU (tests/test_gguf_cpu.py).  `load_into_engine()` composes already-tested
 device entry points (Weight.from_q4_0_host / from_q6_K_host, Llama.set_*) but has not itself been run on a GPU in round 1.
@@ -18,7 +19,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-Q4_0_BLOCK, Q6_K_BLOCK = 18, 210
+Q4_0_BLOCK, Q8_0_BLOCK, Q6_K_BLOCK = 18, 34, 210
 
 
 def dequantize_q4_0(rows: np.ndarray, k: int) -> np.ndarray:
@@ -32,6 +33,16 @@ def dequantize_q4_0(rows: np.ndarray, k: int) -> np.ndarray:
     hi = (q >> 4).astype(np.int8) - 8
     vals = np.concatenate([lo, hi], axis=2).astype(np.float32) * d        # [n, nb, 32]
     return vals.reshape(n, k)
+
+
+def dequantize_q8_0(rows: np.ndarray, k: int) -> np.ndarray:
+    """block_q8_0 rows uint8 [N, K/32*34] -> fp32 [N, K]: fp32(d) * q, one fp32 product per element, element j in byte j of the
+    block's codes (dequantize_row_q8_0, vectors/cpu/quantize.h:780)."""
+    n = rows.shape[0]
+    b = np.ascontiguousarray(rows, np.uint8).reshape(n, k // 32, Q8_0_BLOCK)
+    d = b[:, :, :2].copy().view(np.float16).astype(np.float32)            # [n, nb, 1]
+    q = b[:, :, 2:].copy().view(np.int8).astype(np.float32)
+    return (q * d).reshape(n, k)
 
 
 @dataclass
@@ -77,6 +88,9 @@ def parse(path: str) -> GGUFLlama:
         if t.tensor_type == gguf.GGMLQuantizationType.Q4_0:
             k, n = int(t.shape[0]), int(t.shape[1])
             return dequantize_q4_0(np.array(t.data, np.uint8).reshape(n, k // 32 * Q4_0_BLOCK), k)
+        if t.tensor_type == gguf.GGMLQuantizationType.Q8_0:
+            k, n = int(t.shape[0]), int(t.shape[1])
+            return dequantize_q8_0(np.array(t.data, np.uint8).reshape(n, k // 32 * Q8_0_BLOCK), k)
         raise ValueError(f"{name}: unsupported type {t.tensor_type.name} for an fp32 tensor")
 
     def quant(name, n_expect, k_expect):
@@ -86,9 +100,11 @@ def parse(path: str) -> GGUFLlama:
             raise ValueError(f"{name}: shape {n}x{k}, expected {n_expect}x{k_expect}")
         if t.tensor_type == gguf.GGMLQuantizationType.Q4_0:
             return ("q4_0", np.array(t.data, np.uint8).reshape(n, k // 32 * Q4_0_BLOCK))
+        if t.tensor_type == gguf.GGMLQuantizationType.Q8_0:
+            return ("q8_0", np.array(t.data, np.uint8).reshape(n, k // 32 * Q8_0_BLOCK))
         if t.tensor_type == gguf.GGMLQuantizationType.Q6_K:
             return ("q6_K", np.array(t.data, np.uint8).reshape(n, k // 256 * Q6_K_BLOCK))
-        raise ValueError(f"{name}: weight type {t.tensor_type.name} not supported (Q4_0 / Q6_K)")
+        raise ValueError(f"{name}: weight type {t.tensor_type.name} not supported (Q4_0 / Q8_0 / Q6_K)")
 
     tok = f32("token_embd.weight")
     hp["n_vocab"] = int(tok.shape[0])
@@ -122,7 +138,11 @@ def load_into_engine(model: GGUFLlama, n_ctx: int | None = None, queue=None):
         typ, rows = tr
         if typ == "btla":  # a serialized BesTLA blob (NE files, neural_speed_b200/ne_loader.py)
             return Weight.from_blob(rows, queue)
-        return Weight.from_q6_K_host(rows, n, k, queue) if typ == "q6_K" else Weight.from_q4_0_host(rows, n, k, queue)
+        if typ == "q6_K":
+            return Weight.from_q6_K_host(rows, n, k, queue)
+        if typ == "q8_0":
+            return Weight.from_q8_0_host(rows, n, k, queue)
+        return Weight.from_q4_0_host(rows, n, k, queue)
 
     E, FF = hp["n_embd"], hp["n_ff"]
     kvd = E // hp["n_head"] * hp["n_head_kv"]
