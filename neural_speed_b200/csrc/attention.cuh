@@ -14,8 +14,11 @@ constexpr int kAttnMmaRows = 64, kAttnMmaKeys = 64;
 constexpr int kTileInts = 5;  // ints per entry of the ragged tile table
 
 struct AttnAttr {  // dynamic shared memory already granted to each kernel (function attributes are per device)
-  size_t generic = 0, rows = 0;
-  bool decode = false;
+  struct Grant {
+    const void* kern;
+    size_t smem;
+  } granted[16];  // 15 attention kernels can ask for more than 48 KB
+  int n = 0;
 };
 // {cos, sin} of the one-position back shift per rotary pair, fp16 (model_utils.cpp:165-192); passed by value
 struct ShiftTable {
