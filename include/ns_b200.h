@@ -340,12 +340,33 @@ enum ns_llama_tensor {
   NS_LT_OUT_NORM = 1, /* others[1]  [n_embd] f32          */
   NS_LT_OUTPUT = 2,   /* others[2]  n_vocab x n_embd weight (any ns_weight format, incl. Q6_K) */
   NS_LT_ATTN_NORM = 3, NS_LT_WQ = 4, NS_LT_WK = 5, NS_LT_WV = 6, NS_LT_WO = 7, /* layers[il].norm[0], attn[0..3] */
-  NS_LT_FFN_NORM = 8, NS_LT_W1 = 9, NS_LT_W2 = 10, NS_LT_W3 = 11               /* layers[il].norm[1], ffn[0..2]  */
+  NS_LT_FFN_NORM = 8, NS_LT_W1 = 9, NS_LT_W2 = 10, NS_LT_W3 = 11,              /* layers[il].norm[1], ffn[0..2]  */
+  NS_LT_BQ = 12, NS_LT_BK = 13, NS_LT_BV = 14  /* Qwen2 only: q / k / v biases, f32 [n_embd] / [kvd] / [kvd] (ns_llama_set_f32) */
 };
 NS_API ns_llama* ns_llama_create(const ns_llama_hparams* hp, void* queue);
 NS_API void ns_llama_free(ns_llama* ctx);
 NS_API int ns_llama_set_f32(ns_llama* ctx, int tensor, int layer, const float* host, size_t count);
 NS_API int ns_llama_set_weight(ns_llama* ctx, int tensor, int layer, const ns_weight* w);
+/* ---- architecture ----------------------------------------------------------------------------------------------------------
+ *   NS_LLAMA_ARCH_LLAMA  (default) the graph above
+ *   NS_LLAMA_ARCH_QWEN2  Qwen1.5 / Qwen2 / Qwen2.5 (models/qwen/qwen.cpp, version 2): Llama's graph with q / k / v biases
+ *                        (Q = W_q x + b_q, ...) and NeoX RoPE (ne_rope_inplace mode 2: pairs (i, i + hd/2)).
+ * The NeoX rotation runs as the mode-0 rotation on an interleaved head order: within each head, P maps dim i -> 2i and
+ * i + hd/2 -> 2i + 1 (i < hd/2), and rope_mode0(P x) == P rope_neox(x) bit for bit at rope_scale 1.  ns_llama_set_weight(WQ | WK)
+ * on a Qwen2 context therefore makes a context-owned device copy of the weight with its rows in P order per head (the caller's
+ * handle stays borrowed and unmodified; the copy is freed when the slot is set again and by ns_llama_free), and b_q / b_k are
+ * stored in P order.  q.k sums the same products, V is not permuted, so everything after attention is unchanged.  The K cache
+ * (ns_llama_kv_cache / ns_llama_kv_planes) holds each head's keys in P order.
+ * Allowed only before any matmul weight or bias is set (NS_E_INVALID otherwise).  NS_E_UNSUPPORTED for rope_scale != 1 (the
+ * reference's NeoX branch scales the angle twice) and with streaming on; ns_llama_set_streaming refuses n_keep >= 0 on a Qwen2
+ * context (the reference has no NeoX shift-RoPE-K).  Every eval entry point returns NS_E_INVALID until each layer has its three
+ * biases; NS_LT_BQ / BK / BV on a Llama context are NS_E_INVALID. */
+#define NS_LLAMA_ARCH_LLAMA 0
+#define NS_LLAMA_ARCH_QWEN2 1
+NS_API int ns_llama_set_arch(ns_llama* ctx, int arch);
+/* The weight a context runs for matmul tensor `tensor` of layer `layer` (for tests): the caller's handle, or on a Qwen2 context
+ * the P-order copy for NS_LT_WQ / NS_LT_WK; NULL when unset or for a tensor id that is no matmul weight. */
+NS_API const ns_weight* ns_llama_weight(const ns_llama* ctx, int tensor, int layer);
 /* evaluate n_tokens new tokens after n_past cached ones; logits_host (nullable) gets the n_vocab logits of the LAST token,
  * next_token (nullable) its greedy pick.  Synchronous (host buffers). */
 NS_API int ns_llama_eval(ns_llama* ctx, const int32_t* tokens, int n_tokens, int n_past, float* logits_host, int32_t* next_token);

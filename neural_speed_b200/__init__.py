@@ -69,7 +69,7 @@ EXPORTS = [
     "ns_llama_beam_search", "ns_llama_kv_copy", "ns_llama_kv_cache", "ns_llama_beam_candidates_workspace_bytes", "ns_llama_beam_candidates",
     "ns_beam_candidates_row_host", "ns_logf_host", "ns_beam_search_host",
     "ns_llama_set_kv_type", "ns_llama_kv_type", "ns_llama_kv_planes", "ns_llama_attention_q8_0", "ns_llama_attention_batch_q8_0",
-    "ns_llama_attention_ragged_q8_0",
+    "ns_llama_attention_ragged_q8_0", "ns_llama_set_arch", "ns_llama_weight",
     "ns_comm_handle_bytes", "ns_comm_create", "ns_comm_get_handle", "ns_comm_open_peers", "ns_comm_link_local", "ns_comm_all_reduce_f32",
     "ns_comm_status", "ns_comm_free",
 ]
@@ -193,6 +193,9 @@ def lib() -> C.CDLL:
     L.ns_llama_free.argtypes = [vp]
     L.ns_llama_set_f32.argtypes = [vp, i, i, vp, sz]
     L.ns_llama_set_weight.argtypes = [vp, i, i, vp]
+    L.ns_llama_set_arch.argtypes = [vp, i]
+    L.ns_llama_weight.restype = vp
+    L.ns_llama_weight.argtypes = [vp, i, i]
     L.ns_llama_eval.argtypes = [vp, vp, i, i, vp, vp]
     L.ns_llama_generate.argtypes = [vp, C.c_int32, i, i, vp]
     L.ns_llama_kv_bytes.restype = C.c_ulonglong
@@ -556,15 +559,26 @@ class Llama:
     sampler of Model.generate(do_sample=True) (model_post_sample_top_k_top_p_repeat), drawn on the device so generate() and
     generate_batch() keep feeding picks back without a host round trip."""
 
-    TOK_EMBD, OUT_NORM, OUTPUT, ATTN_NORM, WQ, WK, WV, WO, FFN_NORM, W1, W2, W3 = range(12)
+    TOK_EMBD, OUT_NORM, OUTPUT, ATTN_NORM, WQ, WK, WV, WO, FFN_NORM, W1, W2, W3, BQ, BK, BV = range(15)
+    ARCHS = {"llama": 0, "qwen2": 1}  # NS_LLAMA_ARCH_*
 
     def __init__(self, n_vocab, n_embd, n_head, n_head_kv, n_layer, n_ff, n_ctx, norm_eps=1e-6, rope_theta=10000.0, rope_scale=1.0,
-                 queue=None):
+                 queue=None, arch="llama"):
+        """arch "qwen2": q / k / v biases (set_f32 BQ / BK / BV) and NeoX RoPE (ns_llama_set_arch)"""
+        if arch not in self.ARCHS:
+            raise ValueError(f"arch {arch!r}: one of {sorted(self.ARCHS)}")
         self.hp = LlamaHParams(n_vocab, n_embd, n_head, n_head_kv, n_layer, n_ff, n_ctx, norm_eps, rope_theta, rope_scale)
         self.h = C.c_void_p(lib().ns_llama_create(C.byref(self.hp), queue))
         if not self.h:
             raise RuntimeError("ns_llama_create failed: " + last_error())
         self._keep = []
+        self.arch = arch
+        if arch != "llama":
+            try:
+                _check(lib().ns_llama_set_arch(self.h, self.ARCHS[arch]), "ns_llama_set_arch")
+            except Exception:
+                self.close()
+                raise
 
     def set_f32(self, tensor: int, layer: int, arr: np.ndarray):
         a = np.ascontiguousarray(arr, np.float32)

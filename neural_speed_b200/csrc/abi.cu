@@ -708,8 +708,12 @@ static int launch_set(int path, const ns_weight* const* w, int nw, int mode, con
   if (path == NS_PATH_IMMA) return ns_launch_gemm_imma(w, nw, mode, act, lda, dst, ldo, m, bias, bcast, residual, eltop, ws, st);
   if (path == NS_PATH_TC) {
     if (int rc = ns_launch_act_bf16(w[0], act, lda, m, ws, st)) return rc;
-    for (int i = 0; i < nw; ++i)
-      if (int rc = ns_launch_gemm_tc(w[i], ws, dst + (size_t)i * m * ldo, ldo, m, bias, bcast, residual, st)) return rc;
+    const float* b = bias;
+    for (int i = 0; i < nw; ++i) {
+      if (int rc = ns_launch_gemm_tc(w[i], ws, dst + (size_t)i * m * ldo, ldo, m, b, bcast, residual, st)) return rc;
+      // a QKV node's broadcast bias is [b_q | b_k | b_v]: each weight adds its own part
+      if (b && bcast && mode == NS_GEMV_CONCAT) b += w[i]->n;
+    }
     return NS_OK;
   }
   const int tile = path == NS_PATH_Q6K ? 4 : ns_gemv_tile_rows(w[0]);
@@ -770,18 +774,32 @@ extern "C" int ns_rmsnorm_mul_mat(const ns_weight* w, const float* act, int lda,
   return mul_mat_impl(w, act, lda, dst, ldo, m, nullptr, residual, 0, workspace, queue, norm_w, norm_eps);
 }
 
+int ns_mul_mat_bias(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* bias, void* workspace,
+                    cudaStream_t st, const float* norm_w, float norm_eps) {
+  return mul_mat_impl(w, act, lda, dst, ldo, m, bias, nullptr, bias ? NS_MM_BIAS_BCAST : 0, workspace, (void*)st, norm_w, norm_eps);
+}
+
+// A broadcast bias of a QKV node is read at bias[i * m * ldo + row] by the GEMV and IMMA epilogues (the output's offset in the
+// [3][m][ldo] layout): that is [b_q | b_k | b_v] for one row; the wgmma launches take one part each
+bool ns_qkv_bias_ok(int path, int m) { return m == 1 || path == NS_PATH_TC; }
+
 int ns_mul_qkv_norm(const ns_weight* wq, const ns_weight* wk, const ns_weight* wv, const float* act, int lda, float* dst, int ldo,
-                    int m, void* workspace, void* queue, const float* norm_w, float norm_eps) {
+                    int m, void* workspace, void* queue, const float* norm_w, float norm_eps, const float* bias) {
   if (int rc = ns_ensure_device()) return rc;
   if (!wq || !wk || !wv || !act || !dst || m <= 0) return NS_E_INVALID;
   const ns_weight* wl[3] = {wq, wk, wv};
   if (norm_w && !norm_foldable(wl, 3, m)) return norm_unsupported("ns_rmsnorm_mul_qkv");
   const int path = ns_route(NS_NODE_QKV, wl, m, norm_w ? NS_ROUTE_NORM : 0);
   if (path < 0) return path;
+  if (bias && (!ns_qkv_bias_ok(path, m) || ldo != wq->n || wk->n != wq->n || wv->n != wq->n)) {
+    ns_set_error("ns_mul_qkv: a bias needs one row or the wgmma path, and ldo == n (m=%d path=%d)", m, path);
+    return NS_E_UNSUPPORTED;
+  }
   cudaStream_t st = stream_of(queue);
   void* ws = pick_ws(workspace, st, path_workspace_bytes(path, m, wq->kpad));
   if (!ws) return NS_E_CUDA;
-  return launch_set(path, wl, 3, NS_GEMV_CONCAT, act, lda, dst, ldo, m, nullptr, 0, nullptr, NS_ELT_DEFAULT, norm_w, norm_eps, 0, ws, st);
+  return launch_set(path, wl, 3, NS_GEMV_CONCAT, act, lda, dst, ldo, m, bias, bias ? 1 : 0, nullptr, NS_ELT_DEFAULT, norm_w, norm_eps, 0,
+                    ws, st);
 }
 extern "C" int ns_mul_qkv(const ns_weight* wq, const ns_weight* wk, const ns_weight* wv, const float* act, int lda,
                           float* dst, int ldo, int m, void* workspace, void* queue) {

@@ -118,9 +118,16 @@ int ns_ffn_silu_residual(const ns_weight* w1, const ns_weight* w2, const ns_weig
 // abi.cu: plain matmul node of the decode engine (one_image: see GemvParams)
 int ns_mul_mat_engine(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* residual, void* workspace,
                       cudaStream_t st, const float* norm_w, float norm_eps);
-// abi.cu: fused QKV with the attention RMSNorm folded into the activation quantiser (norm_w may be NULL: plain ns_mul_qkv)
+// abi.cu: fused QKV with the attention RMSNorm folded into the activation quantiser (norm_w may be NULL: plain ns_mul_qkv).
+// bias (may be NULL): [b_q | b_k | b_v] broadcast over the rows; it needs m == 1 or the wgmma path (ns_qkv_bias_ok): the GEMV and
+// integer tensor-core epilogues index a broadcast bias by the output's offset in the [3][m][ldo] layout.
 int ns_mul_qkv_norm(const ns_weight* wq, const ns_weight* wk, const ns_weight* wv, const float* act, int lda, float* dst, int ldo,
-                    int m, void* workspace, void* queue, const float* norm_w, float norm_eps);
+                    int m, void* workspace, void* queue, const float* norm_w, float norm_eps, const float* bias = nullptr);
+bool ns_qkv_bias_ok(int path, int m);
+// abi.cu: dst = W * act + bias (broadcast over the rows; NULL: none), the RMSNorm folded in when norm_w is set (the eval step's
+// Q / K / V matmuls; with bias NULL exactly ns_mul_mat / ns_rmsnorm_mul_mat)
+int ns_mul_mat_bias(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* bias, void* workspace,
+                    cudaStream_t st, const float* norm_w, float norm_eps);
 
 // moe.cu: dst[i] = src[idx[i]] (gather) or dst[idx[i]] = src[i] (scatter), rows of `cols` floats
 int ns_launch_move_rows(bool gather, const float* src, int ld_src, const int* idx_dev, float* dst, int ld_dst, int rows, int cols,

@@ -1,4 +1,4 @@
-"""GGUF (llama architecture) -> tensors for the device eval step (SURVEY §8 f.3, first slice).
+"""GGUF (llama and qwen2 architectures) -> tensors for the device eval step (SURVEY §8 f.3, first slice).
 
 The reference reads GGUF in C++ (`models/model_utils/gguf.h`, `model_files.h:246-860`: header, key/value metadata, tensor
 infos, aligned data) and maps llama tensors to `model.others[0..2]` / `layers[il].norm/attn/ffn` (`models/llama/llama_utils.cpp`).
@@ -7,6 +7,7 @@ types the eval step consumes:
 
   token_embd.weight   F32/F16/Q4_0/Q8_0 -> fp32 table (the reference's ne_get_rows dequantises the looked-up rows; same values)
   *_norm.weight       F32
+  attn_q/k/v.bias     F32 (qwen2 only: Qwen1.5 / Qwen2 / Qwen2.5 files, models/qwen/qwen_utils.cpp:130-143)
   attn_q/k/v/output, ffn_gate/down/up, output.weight   Q4_0 rows (18-byte blocks), Q8_0 rows (34-byte blocks) or Q6_K rows
                       (210-byte blocks), untouched
 
@@ -52,6 +53,7 @@ class GGUFLlama:
     out_norm: np.ndarray                      # fp32 [n_embd]
     output: tuple                             # (type, rows uint8)
     layers: list = field(default_factory=list)  # dicts: attn_norm, ffn_norm (fp32) and wq, wk, wv, wo, w1, w2, w3 = (type, rows)
+    arch: str = "llama"                       # "qwen2": the layer dicts also hold bq, bk, bv (fp32)
 
 
 _LAYER_TENSORS = {"attn_q": "wq", "attn_k": "wk", "attn_v": "wv", "attn_output": "wo", "ffn_gate": "w1", "ffn_down": "w2", "ffn_up": "w3"}
@@ -69,14 +71,14 @@ def parse(path: str) -> GGUFLlama:
     import gguf
     r = gguf.GGUFReader(path)
     arch = bytes(r.get_field("general.architecture").parts[-1]).decode()
-    if arch != "llama":
-        raise ValueError(f"only the llama architecture is supported, file says {arch!r}")
-    hp = dict(n_embd=int(_field(r, "llama.embedding_length")), n_layer=int(_field(r, "llama.block_count")),
-              n_ff=int(_field(r, "llama.feed_forward_length")), n_head=int(_field(r, "llama.attention.head_count")),
-              n_ctx=int(_field(r, "llama.context_length", 2048)),
-              norm_eps=float(_field(r, "llama.attention.layer_norm_rms_epsilon", 1e-6)),  # reference default (model_types.h)
-              rope_theta=float(_field(r, "llama.rope.freq_base", 10000.0)), rope_scale=1.0)
-    hp["n_head_kv"] = int(_field(r, "llama.attention.head_count_kv", hp["n_head"]))
+    if arch not in ("llama", "qwen2"):
+        raise ValueError(f"only the llama and qwen2 architectures are supported, file says {arch!r}")
+    hp = dict(n_embd=int(_field(r, f"{arch}.embedding_length")), n_layer=int(_field(r, f"{arch}.block_count")),
+              n_ff=int(_field(r, f"{arch}.feed_forward_length")), n_head=int(_field(r, f"{arch}.attention.head_count")),
+              n_ctx=int(_field(r, f"{arch}.context_length", 2048)),
+              norm_eps=float(_field(r, f"{arch}.attention.layer_norm_rms_epsilon", 1e-6)),  # reference default (model_types.h)
+              rope_theta=float(_field(r, f"{arch}.rope.freq_base", 10000.0)), rope_scale=1.0)
+    hp["n_head_kv"] = int(_field(r, f"{arch}.attention.head_count_kv", hp["n_head"]))
     tensors = {t.name: t for t in r.tensors}
 
     def f32(name):
@@ -112,11 +114,17 @@ def parse(path: str) -> GGUFLlama:
     kvd = E // hp["n_head"] * hp["n_head_kv"]
     shapes = dict(wq=(E, E), wk=(kvd, E), wv=(kvd, E), wo=(E, E), w1=(FF, E), w2=(E, FF), w3=(FF, E))
     out_name = "output.weight" if "output.weight" in tensors else "token_embd.weight"  # tied embeddings
-    model = GGUFLlama(hp, tok, f32("output_norm.weight"), quant(out_name, hp["n_vocab"], E))
+    model = GGUFLlama(hp, tok, f32("output_norm.weight"), quant(out_name, hp["n_vocab"], E), arch=arch)
     for il in range(hp["n_layer"]):
         L = dict(attn_norm=f32(f"blk.{il}.attn_norm.weight"), ffn_norm=f32(f"blk.{il}.ffn_norm.weight"))
         for gname, ours in _LAYER_TENSORS.items():
             L[ours] = quant(f"blk.{il}.{gname}.weight", *shapes[ours])
+        if arch == "qwen2":
+            for gname, ours, n in (("attn_q", "bq", E), ("attn_k", "bk", kvd), ("attn_v", "bv", kvd)):
+                b = f32(f"blk.{il}.{gname}.bias").reshape(-1)
+                if b.size != n:
+                    raise ValueError(f"blk.{il}.{gname}.bias: {b.size} values, expected {n}")
+                L[ours] = b
         model.layers.append(L)
     return model
 
@@ -132,7 +140,7 @@ def load_into_engine(model: GGUFLlama, n_ctx: int | None = None, queue=None):
         # kernel keeps one score per position in shared memory (~54k positions at head size 128); ask explicitly for more
         hp["n_ctx"] = 32768
     eng = Llama(hp["n_vocab"], hp["n_embd"], hp["n_head"], hp["n_head_kv"], hp["n_layer"], hp["n_ff"], hp["n_ctx"],
-                hp["norm_eps"], hp["rope_theta"], hp["rope_scale"], queue)
+                hp["norm_eps"], hp["rope_theta"], hp["rope_scale"], queue, arch=model.arch)
 
     def weight(tr, n, k):
         typ, rows = tr
@@ -156,4 +164,7 @@ def load_into_engine(model: GGUFLlama, n_ctx: int | None = None, queue=None):
         eng.set_f32(Llama.FFN_NORM, il, L["ffn_norm"])
         for name, (tid, n, k) in ids.items():
             eng.set_weight(tid, il, weight(L[name], n, k))
+        if model.arch == "qwen2":
+            for name, tid in (("bq", Llama.BQ), ("bk", Llama.BK), ("bv", Llama.BV)):
+                eng.set_f32(tid, il, L[name])
     return eng
