@@ -287,6 +287,15 @@ NS_API int ns_gemv_ring_plan_q8_0(int k, int mode, int m, int fused, int norm, i
  * (one image for every node of a token); no bias, optional residual */
 NS_API int ns_mul_mat_engine_image(const ns_weight* w, const float* act, int lda, float* dst, int ldo, int m, const float* residual,
                                    void* workspace, void* queue);
+/* ns_ffn_silu as the eval step runs its prompt FFN nodes, for parity tests: dst = W2 (silu(W1 act) * (W3 act)) [+ residual].  On the
+ * wgmma GEMM path silu(gate) * up goes straight into the down projection's bf16 activation image (the same values the two-step
+ * ns_ffn_silu rounds from its fp32 product) and tmp [2][m][fmid] keeps only the gate and up outputs. */
+NS_API int ns_ffn_silu_engine_image(const ns_weight* w1, const ns_weight* w2, const ns_weight* w3, const float* act, int lda, float* tmp,
+                                    float* dst, int ldo, int m, const float* residual, void* workspace, void* queue);
+/* The wgmma GEMM's launch plan for an m x n output over kpad (k rounded up to 32) inputs, for tests: out[3] = {token tile T,
+ * k slices, k blocks of 64 per slice}.  Slices above 1 add fp32 partial tiles into a zeroed dst with atomics; residual_is_dst
+ * (a residual or bias aliasing dst) keeps one.  Uses the SM count of the current device.  NS_E_INVALID on bad arguments. */
+NS_API int ns_gemm_tc_plan(int m, int n, int kpad, int residual_is_dst, int* out);
 
 /* CUDA-graph capture of a sequence of calls on one queue (replaces the reference's per-token graph rebuild +
  * ne_graph_compute, models/llama/llama.cpp:136-143 / core/ne_layers.c:11915): begin, issue ns_* device calls with

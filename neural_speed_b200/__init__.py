@@ -55,7 +55,8 @@ EXPORTS = [
     "ns_mul_mat", "ns_mul_qkv", "ns_ffn_silu", "ns_ffn_gelu",
     "ns_mul_mat_id", "ns_ffn_id", "ns_mul_mat_id_q4_0_f32_host", "ns_moe_plan",
     "ns_rmsnorm_fusable", "ns_rmsnorm_mul_mat", "ns_rmsnorm_mul_qkv", "ns_rmsnorm_ffn_silu", "ns_mul_mat_q4_0_f32_host", "ns_mul_mat_q6_K_f32_host", "ns_mul_mat_q8_0_f32_host",
-    "ns_prepare_activation", "ns_matmul_prepared", "ns_gemv_ring_plan", "ns_gemv_ring_plan_q8_0", "ns_mul_mat_engine_image", "ns_graph_begin", "ns_graph_end", "ns_graph_launch", "ns_graph_free",
+    "ns_prepare_activation", "ns_matmul_prepared", "ns_gemv_ring_plan", "ns_gemv_ring_plan_q8_0", "ns_mul_mat_engine_image", "ns_ffn_silu_engine_image",
+    "ns_gemm_tc_plan", "ns_graph_begin", "ns_graph_end", "ns_graph_launch", "ns_graph_free",
     "ns_device_quantize_q4_0", "ns_device_quantize_act",
     "BTLAGemmPackBSize", "BTLAGemmQuantPackB", "BTLAGemmPackB", "BTLAGemmUnPackB", "ns_quantize_row_q4_0", "ns_split_weight_size", "ns_split_weight",
     "ns_llama_create", "ns_llama_free", "ns_llama_set_f32", "ns_llama_set_weight", "ns_llama_eval", "ns_llama_generate", "ns_llama_set_exact_prefill",
@@ -180,6 +181,8 @@ def lib() -> C.CDLL:
     L.ns_gemv_ring_plan.argtypes = [i] * 9 + [vp]
     L.ns_gemv_ring_plan_q8_0.argtypes = [i] * 5 + [vp]
     L.ns_mul_mat_engine_image.argtypes = [vp, vp, i, vp, i, i, vp, vp, vp]
+    L.ns_ffn_silu_engine_image.argtypes = [vp, vp, vp, vp, i, vp, vp, i, i, vp, vp, vp]
+    L.ns_gemm_tc_plan.argtypes = [i, i, i, i, vp]
     L.ns_graph_begin.argtypes = [vp]
     L.ns_graph_end.restype = vp
     L.ns_graph_end.argtypes = [vp]

@@ -855,6 +855,12 @@ int ns_ffn_silu_residual(const ns_weight* w1, const ns_weight* w2, const ns_weig
   return ffn_impl(w1, w2, w3, NS_ELT_DEFAULT, nullptr, nullptr, 0, act, lda, tmp, dst, ldo, m, workspace, (void*)st, residual, norm_w,
                   norm_eps, one_image);
 }
+extern "C" int ns_ffn_silu_engine_image(const ns_weight* w1, const ns_weight* w2, const ns_weight* w3, const float* act, int lda,
+                                        float* tmp, float* dst, int ldo, int m, const float* residual, void* workspace, void* queue) {
+  if (!w3) return NS_E_INVALID;
+  return ffn_impl(w1, w2, w3, NS_ELT_DEFAULT, nullptr, nullptr, 0, act, lda, tmp, dst, ldo, m, workspace, queue, residual, nullptr, 0.f,
+                  1);
+}
 // dst = residual + FFN_SiLU(rms_norm(act) * norm_w): llama.cpp:601-698 with the norm folded into the gate/up launch
 extern "C" int ns_rmsnorm_ffn_silu(const ns_weight* w1, const ns_weight* w2, const ns_weight* w3, const float* act, int lda,
                                    const float* norm_w, float norm_eps, float* tmp, float* dst, int ldo, int m, const float* residual,

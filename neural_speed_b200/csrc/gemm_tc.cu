@@ -245,8 +245,6 @@ __global__ void __launch_bounds__(kThreads, 1)
         const uint4 qv = pk[i];
         words[4 * i] = qv.x, words[4 * i + 1] = qv.y, words[4 * i + 2] = qv.z, words[4 * i + 3] = qv.w;
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_empty[sp]);  // packed bytes are in registers
       if (kb >= SD) mbar_wait(&d_empty[sd], ((kb / SD) - 1) & 1);
       unsigned char* drow_base = deq + sd * DEQ_STAGE + (r >> 3) * 1024 + swz * 128;
       if (!(P.dbg & 1))
@@ -285,7 +283,13 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
       fence_proxy_async();  // generic-proxy writes -> visible to the MMA
       __syncwarp();
-      if (lane == 0) mbar_arrive(&d_full[sd]);
+      // The packed slot is released only now that every lane has consumed its words: released right after the loads were
+      // issued, the producer's next TMA into the slot could land before a lane's LDS had read it, and int8 rows then took
+      // bytes of block kb + SP (tests/test_gpu_gemm_tc.py, exact tier)
+      if (lane == 0) {
+        mbar_arrive(&p_empty[sp]);
+        mbar_arrive(&d_full[sd]);
+      }
     }
   } else {
     // ============================ consumers: warpgroup g owns weight rows [64g, 64g + 64) of the tile ============================
@@ -379,8 +383,33 @@ __global__ void __launch_bounds__(256) act_to_bf16_v8_kernel(const float* __rest
   }
 }
 
+// One launch's token tile and k split.  Small M gives too few output tiles to fill the SMs, so the k blocks are cut into up to 16
+// slices of >= 8 blocks (512 k) each, one CTA per tile and slice, their partial tiles added with fp32 atomics.  A residual or bias
+// that aliases dst keeps one slice: dst is zeroed before a split launch.
+struct TcPlan {
+  int T, splits, kb_per_split;
+};
+TcPlan tc_plan(int m, int n, int kpad, bool dst_aliased) {
+  TcPlan p;
+  p.T = m <= 32 ? 32 : (m <= 64 ? 64 : 128);
+  const int total_kb = (kpad + BLOCK_K - 1) / BLOCK_K;
+  const int tiles = ((n + BLOCK_N - 1) / BLOCK_N) * ((m + p.T - 1) / p.T);
+  int splits = 1;
+  static const int env_splits = getenv("NS_TC_SPLITS") ? atoi(getenv("NS_TC_SPLITS")) : 0;  // tuning aid
+  if (3 * tiles < 2 * ns_num_sms() && !dst_aliased) {
+    splits = ns_num_sms() / tiles;  // floor: one CTA per SM is resident (416 threads, ~100-160 KB smem), a partial second wave doubles the time
+    if (splits > total_kb / 8) splits = total_kb / 8;  // keep >= 8 k blocks (512 k) per slice
+    if (splits > 16) splits = 16;
+    if (splits < 1) splits = 1;
+  }
+  if (env_splits > 0) splits = env_splits;
+  p.kb_per_split = (total_kb + splits - 1) / splits;
+  p.splits = (total_kb + p.kb_per_split - 1) / p.kb_per_split;
+  return p;
+}
+
 template <int T, bool W8>
-int launch_t(const CUtensorMap& mw, const CUtensorMap& ma, const GemmParams& P, cudaStream_t st) {
+int launch_t(const CUtensorMap& mw, const CUtensorMap& ma, const GemmParams& P, const TcPlan& plan, cudaStream_t st) {
   using L = Smem<T, W8>;
   auto kern = gemm_w4_tc_kernel<T, W8>;
   static bool attr_set = false;
@@ -388,29 +417,26 @@ int launch_t(const CUtensorMap& mw, const CUtensorMap& ma, const GemmParams& P, 
     NS_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::total));
     attr_set = true;
   }
-  dim3 grid((P.n + BLOCK_N - 1) / BLOCK_N, (P.m + T - 1) / T);
+  dim3 grid((P.n + BLOCK_N - 1) / BLOCK_N, (P.m + T - 1) / T, (unsigned)plan.splits);
   GemmParams Q = P;
-  const int total_kb = (P.kpad + BLOCK_K - 1) / BLOCK_K;
-  int splits = 1;
-  const int tiles = (int)(grid.x * grid.y);
-  static const int env_splits = getenv("NS_TC_SPLITS") ? atoi(getenv("NS_TC_SPLITS")) : 0;  // tuning aid
-  if (3 * tiles < 2 * ns_num_sms() && P.residual != P.dst && P.bias != P.dst) {
-    splits = ns_num_sms() / tiles;  // floor: one CTA per SM is resident (416 threads, ~100-160 KB smem), a partial second wave doubles the time
-    if (splits > total_kb / 8) splits = total_kb / 8;  // keep >= 8 k blocks (512 k) per slice
-    if (splits > 16) splits = 16;
-    if (splits < 1) splits = 1;
-  }
-  if (env_splits > 0) splits = env_splits;
-  Q.kb_per_split = (total_kb + splits - 1) / splits;
-  splits = (total_kb + Q.kb_per_split - 1) / Q.kb_per_split;
-  grid.z = (unsigned)splits;
-  if (splits > 1) NS_CUDA_TRY(cudaMemset2DAsync(P.dst, (size_t)P.ldo * 4, 0, (size_t)P.n * 4, (size_t)P.m, st));
+  Q.kb_per_split = plan.kb_per_split;
+  if (plan.splits > 1) NS_CUDA_TRY(cudaMemset2DAsync(P.dst, (size_t)P.ldo * 4, 0, (size_t)P.n * 4, (size_t)P.m, st));
   NS_CUDA_TRY(ns_launch_pdl(kern, grid, dim3(kThreads), (size_t)L::total, st, mw, ma, Q));
   ns_count_launch();
   return NS_OK;
 }
 
 }  // namespace
+
+extern "C" int ns_gemm_tc_plan(int m, int n, int kpad, int residual_is_dst, int* out) {
+  if (m < 1 || n < 1 || kpad < 32 || kpad % 32 || !out) {
+    ns_set_error("ns_gemm_tc_plan: invalid arguments (m=%d n=%d kpad=%d)", m, n, kpad);
+    return NS_E_INVALID;
+  }
+  const TcPlan p = tc_plan(m, n, kpad, residual_is_dst != 0);
+  out[0] = p.T, out[1] = p.splits, out[2] = p.kb_per_split;
+  return NS_OK;
+}
 
 size_t ns_gemm_tc_workspace_bytes(int m, int kpad) { return ns_round_up((size_t)m * kpad * 2, 256); }
 
@@ -532,7 +558,8 @@ int ns_launch_gemm_tc(const ns_weight* w, const void* ws, float* dst, int ldo, i
     return NS_E_UNSUPPORTED;
   }
   const __nv_bfloat16* abf = (const __nv_bfloat16*)ws;
-  const int T = m <= 32 ? 32 : (m <= 64 ? 64 : 128);
+  const TcPlan plan = tc_plan(m, w->n, w->kpad, residual == dst || bias == dst);
+  const int T = plan.T;
   const bool w8 = w->wfmt == NS_W_S8 || w->wfmt == NS_W_Q8_0;  // natural-order int8 codes (ggml Q8_0: zero point 0, fp16 d)
   CUtensorMap mw, ma;
   // packed nibbles: uint8 [n][q_bytes] with row pitch `pitch`; box = 32 bytes (64 k) x 128 rows, no swizzle
@@ -566,14 +593,14 @@ int ns_launch_gemm_tc(const ns_weight* w, const void* ws, float* dst, int ldo, i
   P.dbg = dbg;
   if (w8) {
     switch (T) {
-      case 32: return launch_t<32, true>(mw, ma, P, st);
-      case 64: return launch_t<64, true>(mw, ma, P, st);
-      default: return launch_t<128, true>(mw, ma, P, st);
+      case 32: return launch_t<32, true>(mw, ma, P, plan, st);
+      case 64: return launch_t<64, true>(mw, ma, P, plan, st);
+      default: return launch_t<128, true>(mw, ma, P, plan, st);
     }
   }
   switch (T) {
-    case 32: return launch_t<32, false>(mw, ma, P, st);
-    case 64: return launch_t<64, false>(mw, ma, P, st);
-    default: return launch_t<128, false>(mw, ma, P, st);
+    case 32: return launch_t<32, false>(mw, ma, P, plan, st);
+    case 64: return launch_t<64, false>(mw, ma, P, plan, st);
+    default: return launch_t<128, false>(mw, ma, P, plan, st);
   }
 }

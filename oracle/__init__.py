@@ -493,6 +493,78 @@ def gemv_bound_ratio(got, a_eff, w_eff):
     return float((np.abs(np.asarray(got, np.float64) - want) / unit).max())
 
 
+# 4-bit float codebooks by code (sign in bit 3 for the FP4 ones): FP4 "BNB" and FP4 E2M1 (kernel_ref.h:1209-1230, :1300-1321);
+# NF4 comes from liboracle (orc_nf4_unpack)
+_F4_BNB = [0.0, 5.208333333e-03, 0.66666667, 1.0, 0.33333333, 0.5, 0.16666667, 0.25]
+_F4_E2M1 = [0.0, 0.010416666666666666, 0.16666666666666666, 0.25, 0.3333333333333333, 0.5, 0.6666666666666666, 1.0]
+
+
+def f4_levels(kind):
+    """the 16 fp32 levels of codebook 'nf4', 'f4_bnb' or 'f4_e2m1', indexed by code"""
+    if kind == "nf4":
+        return np.array([lib().orc_nf4_unpack(c) for c in range(16)], np.float32)
+    half = np.array(_F4_BNB if kind == "f4_bnb" else _F4_E2M1, np.float32)
+    return np.concatenate([half, -half])
+
+
+def _bf16(x):
+    return bf16_bits_to_f32(f32_to_bf16_bits(np.asarray(x, np.float32)))
+
+
+def tc_operands(a, fmt, q=None, scales=None, zp=None, group=32, stype="f32", shuffle=None):
+    """The operands of the wgmma GEMM (gemm_w4_tc_kernel, DESIGN.md section 4): (a_eff [M,K], w_eff [K,N]), bf16 values in fp32.
+      a        fp32 [M,K] (None: a_eff is None); with an act-order shuffle (int [K]) image column k is a[:, shuffle[k]]
+      fmt      's4' / 's8': q = signed integer codes, zp [ceil(K/g),N] or None;  'nf4' / 'f4_bnb' / 'f4_e2m1': q = codebook
+               codes 0..15;  'q4_0': q = nibble - 8;  'q8_0': q = int8 codes (both: group 32, fp16 d)
+      scales   [ceil(K/g),N] as handed to the weight loader, stored as stype 'f32' / 'bf16' / 'f16' (round to nearest even)
+    a_eff = bf16_rn(a).  With s = bf16_rn(stored scale, widened to fp32):
+      integer codes  w_eff = bf16_rn(bf16(q - zp) * s)          (q - zp is exact in bf16: |q - zp| <= 255)
+      codebooks      w_eff = bf16_rn(bf16_rn(level[q]) * s)
+    Products of two bf16 values are exact in fp32, so each bf16_rn above is the kernel's single rounding of an HMUL2."""
+    a_eff = None
+    if a is not None:
+        a = np.asarray(a, np.float32)
+        a_eff = _bf16(a[:, np.asarray(shuffle)] if shuffle is not None else a)
+    qi = np.asarray(q, np.int32)
+    k = qi.shape[0]
+    if fmt in ("q4_0", "q8_0"):
+        group, stype, zp = 32, "f16", None
+    sc = np.asarray(scales, np.float32)
+    if stype == "bf16":
+        sc = _bf16(sc)
+    elif stype == "f16":
+        sc = sc.astype(np.float16).astype(np.float32)
+    s = _bf16(sc)[np.arange(k) // group]
+    if fmt in ("nf4", "f4_bnb", "f4_e2m1"):
+        base = _bf16(f4_levels(fmt)[qi])
+    else:
+        d = qi - (np.asarray(zp, np.int32)[np.arange(k) // group] if zp is not None else 0)
+        assert np.abs(d).max(initial=0) <= 255
+        base = d.astype(np.float32)
+    return a_eff, _bf16(base * s)
+
+
+def tc_grid(a_eff, w_eff):
+    """log2 of the finest product grid of two bf16 operand sets: min lsb(a) + min lsb(w), lsb(v) = floor(log2|v|) - 7 (the weight of
+    the last of a bf16 value's 8 significand bits).  Every product a * w is an integer multiple of 2^grid."""
+    def lsb(x):
+        x = np.abs(np.asarray(x, np.float64))
+        return int(np.floor(np.log2(x[x > 0].min()))) - 7
+    return lsb(a_eff) + lsb(w_eff)
+
+
+def tc_exact_budget(a_eff, w_eff, mag=None, extra=None):
+    """max over outputs of (sum_k |a_eff w_eff| [+ extra]) in units of 2^tc_grid.  Below 2^24 every partial sum of the products
+    (and of extra, when its terms lie on the grid), in any order and any split, is an integer multiple of the grid below 2^24
+    of it: an exact fp32 value, so an fp32 accumulation gives the fp64 sum bit for bit.  mag: gemv_stated's second output, if
+    already computed; extra: [M,N] magnitudes of the epilogue's addends (|bias| + |residual|)."""
+    if mag is None:
+        mag = gemv_stated(a_eff, w_eff)[1]
+    if extra is not None:
+        mag = mag + np.asarray(extra, np.float64)
+    return float(np.max(mag)) / 2.0 ** tc_grid(a_eff, w_eff)
+
+
 def imma_act(a, comp, g):
     """The activations of an integer block-sum matmul as the quantisers give them: (codes - zero point) int64 [M,K], scales fp32
     [M, K/ab] and the activation block ab.  comp: 'q8_0' (quantize_row_q8_0: blocks of 32, fp16 d), 'int8' (u8 with zero points

@@ -238,8 +238,9 @@ def parse(blob) -> dict:
                 red=rbuf, dq=dqbuf, shuffle=shbuf)
 
 
-def unpack(blob) -> np.ndarray:
-    """Dequantise a blob to fp32 [K,N] (unpackWeight semantics)."""
+def codes(blob) -> dict:
+    """The stored operands of a blob: q int32 [K,N] (signed integer codes, or the 0..15 codebook codes of a float blob), scale
+    fp32 [ceil(K/blk),N] as stored (bf16 / fp16 widened), zp int32 [..] or None, blk, prologue (2: float codebook)."""
     h = parse(blob)
     n, k, npad, kpad, nt, pr, blk = h["n"], h["k"], h["npad"], h["kpad"], h["ntile"], h["packrow"], h["blocksize"]
     raw = np.frombuffer(h["qbuf"], np.uint8)
@@ -261,13 +262,23 @@ def unpack(blob) -> np.ndarray:
         sc = bf16_bits_to_f32(np.frombuffer(h["scale"], np.uint16))
     else:
         sc = np.frombuffer(h["scale"], np.float16).astype(np.float32)
-    sc = sc.reshape(nk, h["cstep"])[:, :n]
-    gi = np.arange(k) // blk
-    if h["prologue"] == 2:
+    raw_nb = -(-k // blk)
+    sc = sc.reshape(nk, h["cstep"])[:raw_nb, :n]
+    zp = None
+    if h["zp"] is not None:
+        zp = np.frombuffer(h["zp"], np.int8).reshape(nk, h["cstep"])[:raw_nb, :n].astype(np.int32)
+    return dict(q=np.ascontiguousarray(t), scale=np.ascontiguousarray(sc), zp=zp, blk=blk, prologue=h["prologue"])
+
+
+def unpack(blob) -> np.ndarray:
+    """Dequantise a blob to fp32 [K,N] (unpackWeight semantics)."""
+    c = codes(blob)
+    t, sc, blk = c["q"], c["scale"], c["blk"]
+    gi = np.arange(t.shape[0]) // blk
+    if c["prologue"] == 2:
         from . import lib
         lut = np.array([lib().orc_nf4_unpack(c) for c in range(16)], np.float32)
         return (lut[t] * sc[gi]).astype(np.float32)
-    if h["zp"] is not None:
-        zp = np.frombuffer(h["zp"], np.int8).reshape(nk, h["cstep"])[:, :n].astype(np.int32)
-        t = t - zp[gi]
+    if c["zp"] is not None:
+        t = t - c["zp"][gi]
     return (t.astype(np.float32) * sc[gi]).astype(np.float32)
