@@ -360,20 +360,23 @@ NS_API int ns_llama_set_weight(ns_llama* ctx, int tensor, int layer, const ns_we
  *   NS_LLAMA_ARCH_LLAMA  (default) the graph above
  *   NS_LLAMA_ARCH_QWEN2  Qwen1.5 / Qwen2 / Qwen2.5 (models/qwen/qwen.cpp, version 2): Llama's graph with q / k / v biases
  *                        (Q = W_q x + b_q, ...) and NeoX RoPE (ne_rope_inplace mode 2: pairs (i, i + hd/2)).
+ *   NS_LLAMA_ARCH_PHI3   Phi-3 (models/phi/phi3.cpp): Llama's graph with NeoX RoPE and no biases.  Phi-3-mini's head size 96
+ *                        runs on the split decode and tensor-core prompt attention like 64 / 128 (fp16 KV cache only).
  * The NeoX rotation runs as the mode-0 rotation on an interleaved head order: within each head, P maps dim i -> 2i and
- * i + hd/2 -> 2i + 1 (i < hd/2), and rope_mode0(P x) == P rope_neox(x) bit for bit at rope_scale 1.  ns_llama_set_weight(WQ | WK)
- * on a Qwen2 context therefore makes a context-owned device copy of the weight with its rows in P order per head (the caller's
+ * i + hd/2 -> 2i + 1 (i < hd/2; at hd 96: i -> 2i, i + 48 -> 2i + 1), and rope_mode0(P x) == P rope_neox(x) bit for bit at
+ * rope_scale 1.  ns_llama_set_weight(WQ | WK) on a Qwen2 or Phi-3 context therefore makes a context-owned device copy of the weight with its rows in P order per head (the caller's
  * handle stays borrowed and unmodified; the copy is freed when the slot is set again and by ns_llama_free), and b_q / b_k are
  * stored in P order.  q.k sums the same products, V is not permuted, so everything after attention is unchanged.  The K cache
  * (ns_llama_kv_cache / ns_llama_kv_planes) holds each head's keys in P order.
  * Allowed only before any matmul weight or bias is set (NS_E_INVALID otherwise).  NS_E_UNSUPPORTED for rope_scale != 1 (the
  * reference's NeoX branch scales the angle twice) and with streaming on; ns_llama_set_streaming refuses n_keep >= 0 on a Qwen2
- * context (the reference has no NeoX shift-RoPE-K).  Every eval entry point returns NS_E_INVALID until each layer has its three
- * biases; NS_LT_BQ / BK / BV on a Llama context are NS_E_INVALID. */
+ * or Phi-3 context (the reference has no NeoX shift-RoPE-K).  On a Qwen2 context every eval entry point returns NS_E_INVALID
+ * until each layer has its three biases; NS_LT_BQ / BK / BV on a Llama or Phi-3 context are NS_E_INVALID. */
 #define NS_LLAMA_ARCH_LLAMA 0
 #define NS_LLAMA_ARCH_QWEN2 1
+#define NS_LLAMA_ARCH_PHI3 2
 NS_API int ns_llama_set_arch(ns_llama* ctx, int arch);
-/* The weight a context runs for matmul tensor `tensor` of layer `layer` (for tests): the caller's handle, or on a Qwen2 context
+/* The weight a context runs for matmul tensor `tensor` of layer `layer` (for tests): the caller's handle, or on a Qwen2 / Phi-3 context
  * the P-order copy for NS_LT_WQ / NS_LT_WK; NULL when unset or for a tensor id that is no matmul weight. */
 NS_API const ns_weight* ns_llama_weight(const ns_llama* ctx, int tensor, int layer);
 /* evaluate n_tokens new tokens after n_past cached ones; logits_host (nullable) gets the n_vocab logits of the LAST token,
@@ -409,7 +412,7 @@ NS_API int ns_llama_set_streaming(ns_llama* ctx, int n_keep);
  *
  * 1 <= n_seq <= 32 KV blocks (default 1).  Reallocates and zeroes the cache; every sequence restarts at n_past 0; drops the
  * captured graphs.  NS_E_UNSUPPORTED for n_seq > 1 with streaming on (llama.cpp:104 forbids the pair) or a head size other
- * than 64 / 128.  ns_llama_set_streaming returns NS_E_UNSUPPORTED for n_keep >= 0 while n_seq > 1.  ns_llama_eval and
+ * than 64 / 96 / 128.  ns_llama_set_streaming returns NS_E_UNSUPPORTED for n_keep >= 0 while n_seq > 1.  ns_llama_eval and
  * ns_llama_generate serve sequence 0. */
 NS_API int ns_llama_set_sequences(ns_llama* ctx, int n_seq);
 /* ns_llama_eval on KV block `seq` (prompts, exact-prefill mode and all argument rules as ns_llama_eval) */
@@ -419,7 +422,7 @@ NS_API int ns_llama_eval_seq(ns_llama* ctx, int seq, const int32_t* tokens, int 
  * next_tokens (nullable) [n] greedy picks; n_past[i] + 1 <= n_ctx.  One CUDA graph per n (captured on first use) serves any
  * set of sequences at any positions.  NS_E_INVALID (nothing launched) for n outside [1, n_seq], a sequence id outside
  * [0, n_seq) or given twice, n_past[i] < 0 or past the context, null pointers; NS_E_UNSUPPORTED with streaming on or a head
- * size other than 64 / 128. */
+ * size other than 64 / 96 / 128. */
 NS_API int ns_llama_decode_batch(ns_llama* ctx, int n, const int* seq, const int32_t* tokens, const int* n_past,
                                  float* logits_host, int32_t* next_tokens);
 /* greedy generation for n distinct sequences, each pick fed back on the device; out_tokens [n][n_new];
@@ -434,10 +437,10 @@ NS_API int ns_llama_generate_batch(ns_llama* ctx, int n, const int* seq, const i
  * Every matmul node is routed by ns_route at T rows, as a prompt of T tokens is (so a decode token in a pass of T > 32 rows takes
  * the bf16 wgmma GEMM for that step); the one-token segments' attention is ns_llama_decode_batch's, each longer segment's is
  * the tensor-core prompt attention (NS_ATTN_MMA) on its block, bit for bit -- also for 2 .. 7 tokens, where ns_llama_eval_seq
- * takes NS_ATTN_ROWS.  When every segment has one token the call is ns_llama_decode_batch (its captured graph); other passes
+ * takes NS_ATTN_ROWS at head sizes 64 / 128.  When every segment has one token the call is ns_llama_decode_batch (its captured graph); other passes
  * run eagerly.  NS_E_INVALID (nothing launched) for n outside [1, n_seq], a sequence id outside [0, n_seq) or given twice,
  * n_tokens[i] < 1, n_past[i] < 0 or n_past[i] + n_tokens[i] > n_ctx, T > 4096 rows (a fixed cap per call: chunk longer
- * prompts), null pointers; NS_E_UNSUPPORTED with streaming on, a head size other than 64 / 128, or exact-prefill mode with
+ * prompts), null pointers; NS_E_UNSUPPORTED with streaming on, a head size other than 64 / 96 / 128, or exact-prefill mode with
  * T > 32 (its integer block sums hold up to 32 rows). */
 NS_API int ns_llama_eval_batch(ns_llama* ctx, int n, const int* seq, const int* n_tokens, const int32_t* tokens,
                                const int* n_past, float* logits_host, int32_t* next_tokens);
@@ -576,7 +579,7 @@ typedef struct ns_llama_beams {
 /* prompts: n_tokens[r] >= 1 tokens each, back to back in `tokens`, with n_tokens[r] + max_new_tokens - 1 <= n_ctx (the last pick
  * is never evaluated).  out_tokens [n][max_new_tokens]: request r's response in out_tokens[r][0 .. out_len[r]); out_score [n]
  * (nullable): its length-penalised score.  NS_E_UNSUPPORTED while sampling or streaming is on, for a head size other than
- * 64 / 128, or in exact-prefill mode for prompts of more than 32 tokens in all (the prompt pass is ns_llama_eval_batch's); NS_E_INVALID for a field or length out of range or a null pointer.  A refused call launches nothing. */
+ * 64 / 96 / 128, or in exact-prefill mode for prompts of more than 32 tokens in all (the prompt pass is ns_llama_eval_batch's); NS_E_INVALID for a field or length out of range or a null pointer.  A refused call launches nothing. */
 NS_API int ns_llama_beam_search(ns_llama* ctx, int n, const int* n_tokens, const int32_t* tokens, const ns_llama_beams* cfg,
                                 int32_t* out_tokens, int* out_len, float* out_score);
 /* model_kv_cache_seq_cpy (model_utils.cpp:2058-2064) in one launch: positions [p0, p1) of KV block src[i] into block dst[i] for
@@ -631,10 +634,11 @@ NS_API int ns_llama_kv_planes(const ns_llama* ctx, void** k, void** kd, void** v
  * of q [m][n_head * hd] in place and of the m new rows k [m][n_head_kv * hd] at positions n_past .. n_past + m - 1, k and v appended
  * to the fp16 caches kc / vc [n_head_kv][n_ctx][hd], out [m][n_head * hd] = causal softmax(K q / sqrt(hd)) V (llama.cpp:286-302).
  * All pointers are device memory.  kernel: NS_ATTN_AUTO (what ns_llama_eval runs for this shape) or one kernel forced:
- *   NS_ATTN_SPLIT_DECODE  m = 1, hd 64 / 128: context split over 256-position ranges, per-range results merged
+ *   NS_ATTN_SPLIT_DECODE  m = 1, hd 64 / 96 / 128: context split over 256-position ranges, per-range results merged
  *   NS_ATTN_ROWS          hd 64 / 128: one CTA per (head, row); RoPE and the KV append fused in when m = 1
- *   NS_ATTN_MMA           hd 64 / 128: causal prompt attention on mma.sync tensor cores
+ *   NS_ATTN_MMA           hd 64 / 96 / 128: causal prompt attention on mma.sync tensor cores
  *   NS_ATTN_GENERIC       any even hd: one CTA per (head, row) after a separate RoPE + KV-append launch
+ * NS_ATTN_AUTO at hd 96 takes NS_ATTN_SPLIT_DECODE for m = 1 and NS_ATTN_MMA otherwise.
  * A forced kernel that cannot take the shape returns NS_E_UNSUPPORTED without launching anything.
  * ws: device workspace of ns_llama_attention_workspace_bytes(n_head, hd, n_ctx) bytes, zeroed once by the caller:
  *   int state[4] (the call writes n_past to state[1]) | unsigned tickets[n_head] (zero again after every call), padded to 16 bytes |
@@ -658,8 +662,8 @@ NS_API int ns_llama_attention_ring(float* q, const float* k, const float* v, voi
 /* One layer's batched decode attention on its own, for parity tests (as ns_llama_attention with NS_ATTN_SPLIT_DECODE, row by row):
  * q [n][n_head * hd] (rotated in registers only), k / v [n][n_head_kv * hd], caches [n_seq][n_head_kv][n_ctx][hd] fp16; row i
  * appends to block seq[i] at position n_past[i] and attends to positions 0 .. n_past[i] of that block; out [n][n_head * hd].
- * seq / n_past are host arrays of n entries (distinct ids in [0, n_seq), 0 <= n_past[i] < n_ctx, else NS_E_INVALID); hd 64 / 128
- * (else NS_E_UNSUPPORTED); nothing is launched on a refused call.  ws: ns_llama_attention_batch_workspace_bytes(n, n_head, hd,
+ * seq / n_past are host arrays of n entries (distinct ids in [0, n_seq), 0 <= n_past[i] < n_ctx, else NS_E_INVALID); hd 64 / 96 /
+ * 128 (else NS_E_UNSUPPORTED); nothing is launched on a refused call.  ws: ns_llama_attention_batch_workspace_bytes(n, n_head, hd,
  * n_ctx) bytes, zeroed once by the caller: int rows[n][4] (n_past in slot 1) | int seq[n], padded to 16 bytes | unsigned
  * tickets[n][n_head] (zero again after every call), padded to 16 bytes | float partials[n][n_head][ceil(n_ctx / 256)][hd + 2]. */
 NS_API size_t ns_llama_attention_batch_workspace_bytes(int n, int n_head, int hd, int n_ctx);
@@ -670,7 +674,7 @@ NS_API int ns_llama_attention_batch(float* q, const float* k, const float* v, vo
  * that segment's block): segment i is n_tokens[i] >= 1 rows of sequence seq[i] at positions n_past[i] .., the segments back to
  * back in the caller's order (T = sum n_tokens rows).  q [T][n_head * hd] is rotated in place, k / v [T][n_head_kv * hd] are
  * rotated / appended to the caches [n_seq][n_head_kv][n_ctx][hd] fp16, out [T][n_head * hd].  Argument rules of
- * ns_llama_eval_batch (NS_E_INVALID, nothing launched), hd 64 / 128 (else NS_E_UNSUPPORTED).  ws: device workspace of
+ * ns_llama_eval_batch (NS_E_INVALID, nothing launched), hd 64 / 96 / 128 (else NS_E_UNSUPPORTED).  ws: device workspace of
  * ns_llama_attention_ragged_workspace_bytes(n, T) bytes: int rows[T][2] | int tiles[T / 64 + n][5], written by the call. */
 NS_API size_t ns_llama_attention_ragged_workspace_bytes(int n, int n_rows);
 NS_API int ns_llama_attention_ragged(float* q, const float* k, const float* v, void* kc, void* vc, int n_seq, int n, const int* seq,

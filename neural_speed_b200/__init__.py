@@ -563,11 +563,11 @@ class Llama:
     generate_batch() keep feeding picks back without a host round trip."""
 
     TOK_EMBD, OUT_NORM, OUTPUT, ATTN_NORM, WQ, WK, WV, WO, FFN_NORM, W1, W2, W3, BQ, BK, BV = range(15)
-    ARCHS = {"llama": 0, "qwen2": 1}  # NS_LLAMA_ARCH_*
+    ARCHS = {"llama": 0, "qwen2": 1, "phi3": 2}  # NS_LLAMA_ARCH_*
 
     def __init__(self, n_vocab, n_embd, n_head, n_head_kv, n_layer, n_ff, n_ctx, norm_eps=1e-6, rope_theta=10000.0, rope_scale=1.0,
                  queue=None, arch="llama"):
-        """arch "qwen2": q / k / v biases (set_f32 BQ / BK / BV) and NeoX RoPE (ns_llama_set_arch)"""
+        """arch "qwen2": q / k / v biases (set_f32 BQ / BK / BV) and NeoX RoPE; "phi3": NeoX RoPE, no biases (ns_llama_set_arch)"""
         if arch not in self.ARCHS:
             raise ValueError(f"arch {arch!r}: one of {sorted(self.ARCHS)}")
         self.hp = LlamaHParams(n_vocab, n_embd, n_head, n_head_kv, n_layer, n_ff, n_ctx, norm_eps, rope_theta, rope_scale)

@@ -147,9 +147,9 @@ __global__ void __launch_bounds__(kAttnThreads) attn_kernel(const float* __restr
   }
 }
 
-// Decode-shaped attention for head sizes 64 / 128: kAW warps per (head, token); a warp streams whole K/V rows (one 4- or 8-byte
-// load per lane), four rows in flight; with FUSE (single new token) the kernel also applies RoPE to its q head and to the
-// new k row and appends k,v to the cache, so rope_kv_kernel is not launched.
+// Decode-shaped attention for head sizes 64 / 128 (attn_all_hd): kAW warps per (head, token); a warp streams whole K/V rows (one
+// 4- or 8-byte load per lane), four rows in flight; with FUSE (single new token) the kernel also applies RoPE to its q head and to
+// the new k row and appends k,v to the cache, so rope_kv_kernel is not launched.
 constexpr int kAW = 16;  // warps per CTA: the kernel is a chain of dependent cache-row loads, more warps = more rows in flight
 template <int HD, bool FUSE>
 __global__ void __launch_bounds__(kAW * 32) attn_fast_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ knew, int ldk,
@@ -316,12 +316,15 @@ __global__ void __launch_bounds__(kAW * 32) attn_fast_kernel(const float* __rest
 // grid (n_head, ceil(n_ctx / 256)); CTA (h, s) owns cached positions [256 s, 256 s + 256) of head h and returns at once when the
 // sequence has not reached its range (the position lives in device memory: one CUDA graph serves every position).  The rows of a
 // head are contiguous in the cache ([kv head][n_ctx][hd] fp16), so the CTA's whole K and V ranges arrive as TWO cp.async.bulk copies
-// (<= 64 KB each) on one mbarrier: a single global-memory latency per launch instead of a chain of dependent row loads -- the old
-// kernel spent 2-3 round trips per pass at 100-200 positions.  Scores, soft_max and P.V then run out of shared memory.
+// (<= 64 KB each; 48 KB at head size 96, whose rows of 192 B keep every range 16-byte aligned) on one mbarrier: a single
+// global-memory latency per launch instead of a chain of dependent row loads -- the old kernel spent 2-3 round trips per pass at
+// 100-200 positions.  Scores, soft_max and P.V then run out of shared memory.
 // One active range (<= 256 positions): exactly the reference arithmetic (global maximum, e = fp16(exp(fp16(s - max))),
 // p = fp16(e / sum), fp32 sums).  Several: every CTA leaves {max, sum e, sum e V} of its range, the last one to arrive (ticket per
 // head) merges them with exp(max_s - max) weights -- same values up to the fp16 rounding of p (measured: tests/test_gpu_attention.py).
 // Bound: latency at short contexts; HBM (2 x len x hd x 2 B per kv head) at long ones, spread over n_head x ceil(len / 256) CTAs.
+// Head sizes 64 / 96 / 128 (attn_fast_hd): a lane owns EPL = hd / 32 consecutive elements of a row; 96 (fp16, RING = false only)
+// reads its three with 2-byte loads.
 //
 // RING = true: the StreamingLLM ring of the reference's shift-RoPE-K mode (llama.cpp:102-107, 351-354, 430-470), grid
 // (n_head_kv, ranges).  One CTA per (kv head, range) serves every query head of its group from the one staged tile, so no two CTAs
@@ -530,9 +533,12 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
       const uint2 u = *reinterpret_cast<const uint2*>(base + (size_t)r * HD + lane * 4);
       const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
       dst[0] = a.x, dst[1] = a.y, dst[2] = b.x, dst[3] = b.y;
-    } else {
+    } else if (EPL == 2) {
       const float2 a = __half22float2(*reinterpret_cast<const __half2*>(base + (size_t)r * HD + lane * 2));
       dst[0] = a.x, dst[1] = a.y;
+    } else {  // HD 96: three halves per lane, 6 bytes apart -- not aligned for a wider load (two lanes share a bank at most)
+#pragma unroll
+      for (int e = 0; e < EPL; ++e) dst[e] = __half2float(base[(size_t)r * HD + lane * EPL + e]);
     }
   };
   // pass 1: scores of the range
@@ -657,7 +663,8 @@ __global__ void __launch_bounds__(kDW * 32) attn_decode_kernel(const float* __re
 //   pass B  S again, e = fp16(exp(fp16(s - max))), l += e, O += e V (e is an exact fp16 value: the products are exact), out = O / l
 // (difference to the reference: it rounds e / l to fp16 before the V product; here the division happens once, in fp32, after it).
 // CTA = 64 query rows of one head (4 warps x 16 rows); K / V tiles of 64 keys staged in shared memory with 16-byte padded rows
-// (conflict-free 32-bit B-fragment loads for K, ldmatrix.trans for V); every q-tile of a head re-reads that head's K / V through L2.
+// (conflict-free 32-bit B-fragment loads for K, ldmatrix.trans for V; at HD 96 a row of 208 B rotates the banks by 20 words, still
+// conflict-free); every q-tile of a head re-reads that head's K / V through L2.
 // Bound: tensor pipe / shared-memory bandwidth (K and V of one head are 0.5 MB at 2048 positions -- L2 resident).
 //
 // RAGGED: the query rows are segments of several sequences (ns_llama_eval_batch, llama.cpp:414-489 run per input), grid
@@ -676,15 +683,17 @@ __device__ __forceinline__ void mma_f16_16816(float (&c)[4], const uint32_t (&a)
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
+// At HD 96 ptxas, left to itself, caps the ragged form near 168 registers and spills; one CTA per SM as the floor gives it the
+// registers it needs (the 64 / 128 forms keep the default bound).
 template <int HD, bool RAGGED = false, int KV = NS_KV_F16>
-__global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__ q, int ldq, const kv_elem_t<KV>* __restrict__ kc,
-                                                       const kv_elem_t<KV>* __restrict__ vc, const int* __restrict__ state, float* __restrict__ out,
-                                                       int ldo, int n_head, int n_head_kv, int n_ctx, int m, float scale,
-                                                       const int* __restrict__ tiles, const __half* __restrict__ kd,
-                                                       const __half* __restrict__ vd) {
+__global__ void __launch_bounds__(128, HD == 96 ? 1 : 0)
+    attn_mma_kernel(const float* __restrict__ q, int ldq, const kv_elem_t<KV>* __restrict__ kc, const kv_elem_t<KV>* __restrict__ vc,
+                    const int* __restrict__ state, float* __restrict__ out, int ldo, int n_head, int n_head_kv, int n_ctx, int m,
+                    float scale, const int* __restrict__ tiles, const __half* __restrict__ kd, const __half* __restrict__ vd) {
   constexpr bool Q8 = KV == NS_KV_Q8_0;
   constexpr int LD = HD + 8;  // halves per shared-memory row: 16 bytes of padding rotate the banks by 4 words per row
-  constexpr int KS = HD / 16, NT = HD / 8;
+  constexpr int KS = HD / 16, NT = HD / 8;  // HD 96: 6 k-steps of Q K^T, 12 n-tiles (6 ldmatrix.x4) of P V
+  static_assert(kAttnMmaKeys * (HD / 8) % 128 == 0, "load_tile: whole 16-byte chunks per thread");
   __shared__ __align__(16) __half Ks[kAttnMmaKeys * LD];
   __shared__ __align__(16) __half Vs[kAttnMmaKeys * LD];
   pdl_launch_dependents();
@@ -860,11 +869,12 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(const float* __restrict__
 
 // ---- one layer's attention: RoPE of q and of the m new k rows at positions state[1] + t, KV append, causal attention ----------
 // q [m][n_head * hd] (rotated in place unless a fused kernel rotates it in registers), k / v [m][n_head_kv * hd], cache
-// [n_head_kv][n_ctx][hd] (kv_cache.cuh), out [m][n_head * hd].  NS_ATTN_AUTO picks what the eval step has always run:
+// [n_head_kv][n_ctx][hd] (kv_cache.cuh), out [m][n_head * hd].  NS_ATTN_AUTO picks:
 //   hd 64 / 128, one row    attn_decode_kernel (context split over 256-position ranges) while the context has <= 1024 ranges
 //                           and NS_ATTN_OLD_DECODE is unset, else attn_fast_kernel<FUSE>
 //   hd 64 / 128, >= 8 rows  rope_kv_kernel + attn_mma_kernel unless NS_ATTN_SCALAR is set
 //   hd 64 / 128, otherwise  rope_kv_kernel + attn_fast_kernel
+//   hd 96                   attn_decode_kernel for one row, rope_kv_kernel + attn_mma_kernel for more (fp16 cache only)
 //   any other (even) hd     rope_kv_kernel + attn_kernel
 // A Q8_0 cache takes the split decode attention for one row and rope_kv_kernel + attn_mma_kernel for more, at head sizes 64 / 128;
 // attn_fast_kernel and attn_kernel have no Q8_0 form.
@@ -876,9 +886,9 @@ extern int attn_ranges(int n_ctx) { return (n_ctx + kSplitKeys - 1) / kSplitKeys
 
 // the kernel `kind` resolves to for this shape and cache format, or NS_E_UNSUPPORTED when a forced kernel cannot take it
 static int attn_resolve(int kind, int hd, int m, int n_ctx, int kv) {
-  const bool fast = hd == 128 || hd == 64;
+  const bool all = attn_all_hd(hd), fast = attn_fast_hd(hd);
   const bool q8 = kv == NS_KV_Q8_0 && kind >= NS_ATTN_AUTO && kind <= NS_ATTN_GENERIC;
-  if (q8 && !fast) {
+  if (q8 && !all) {
     ns_set_error("ns_llama: the Q8_0 KV cache needs head size 64 or 128, got %d", hd);
     return NS_E_UNSUPPORTED;
   }
@@ -890,8 +900,8 @@ static int attn_resolve(int kind, int hd, int m, int n_ctx, int kv) {
       ns_set_error("ns_llama: NS_ATTN_OLD_DECODE / NS_ATTN_SCALAR select kernels without a Q8_0 KV form");
       return NS_E_UNSUPPORTED;
     }
-    if (q8) kind = m == 1 ? NS_ATTN_SPLIT_DECODE : NS_ATTN_MMA;
-    else if (!fast) kind = NS_ATTN_GENERIC;
+    if (!fast) kind = NS_ATTN_GENERIC;
+    else if (q8 || !all) kind = m == 1 ? NS_ATTN_SPLIT_DECODE : NS_ATTN_MMA;  // the two kernels with a Q8_0 form and a head size 96 form
     else if (m == 1) kind = attn_ranges(n_ctx) <= 1024 && !old_decode ? NS_ATTN_SPLIT_DECODE : NS_ATTN_ROWS;
     else kind = m >= 8 && !scalar_attn ? NS_ATTN_MMA : NS_ATTN_ROWS;
   }
@@ -899,16 +909,16 @@ static int attn_resolve(int kind, int hd, int m, int n_ctx, int kv) {
     ns_set_error("ns_llama: attention kernel %d has no Q8_0 KV form (NS_ATTN_SPLIT_DECODE / NS_ATTN_MMA read Q8_0)", kind);
     return NS_E_UNSUPPORTED;
   }
-  if (q8 && kind == NS_ATTN_SPLIT_DECODE && attn_ranges(n_ctx) > 1024) {
-    ns_set_error("ns_llama: n_ctx %d too large for the split decode attention over a Q8_0 KV cache", n_ctx);
+  if ((q8 || (fast && !all)) && kind == NS_ATTN_SPLIT_DECODE && attn_ranges(n_ctx) > 1024) {
+    ns_set_error("ns_llama: n_ctx %d too large for the split decode attention %s", n_ctx, q8 ? "over a Q8_0 KV cache" : "at head size 96");
     return NS_E_UNSUPPORTED;
   }
   if (kind < NS_ATTN_SPLIT_DECODE || kind > NS_ATTN_GENERIC) {
     ns_set_error("ns_llama: unknown attention kernel %d", kind);
     return NS_E_INVALID;
   }
-  if (kind != NS_ATTN_GENERIC && !fast) {
-    ns_set_error("ns_llama: attention kernel %d needs head size 64 or 128, got %d", kind, hd);
+  if (kind != NS_ATTN_GENERIC && !(kind == NS_ATTN_ROWS ? all : fast)) {
+    ns_set_error("ns_llama: attention kernel %d needs head size %s, got %d", kind, kind == NS_ATTN_ROWS ? "64 or 128" : "64, 96 or 128", hd);
     return NS_E_UNSUPPORTED;
   }
   if (kind == NS_ATTN_SPLIT_DECODE && m != 1) {
@@ -936,8 +946,9 @@ extern ShiftTable shift_table(int hd, float freq_base) {
   return t;
 }
 
-// Runs f(HD, KV) with the head size and the cache format as compile-time constants (std::integral_constant): HD 64 or 128, the
-// sizes attn_decode_kernel, attn_mma_kernel and attn_fast_kernel are instantiated at; `what` names the caller when hd is another.
+// Runs f(HD, KV) with the head size and the cache format as compile-time constants (std::integral_constant): HD 64 or 128 with
+// either cache format, the sizes every fast kernel is instantiated at, or 96 with an fp16 cache, where attn_decode_kernel and
+// attn_mma_kernel are (f tests attn_all_hd(HD) before it names another kernel); `what` names the caller for any other pair.
 template <class F>
 static int attn_dispatch(const char* what, int hd, int kv, F&& f) {
   using F16 = std::integral_constant<int, NS_KV_F16>;
@@ -945,7 +956,8 @@ static int attn_dispatch(const char* what, int hd, int kv, F&& f) {
   const auto at = [&](auto HD) { return kv == NS_KV_Q8_0 ? f(HD, Q8{}) : f(HD, F16{}); };
   if (hd == 128) return at(std::integral_constant<int, 128>{});
   if (hd == 64) return at(std::integral_constant<int, 64>{});
-  ns_set_error("ns_llama: %s needs head size 64 or 128, got %d", what, hd);
+  if (hd == 96 && kv == NS_KV_F16) return f(std::integral_constant<int, 96>{}, F16{});
+  ns_set_error("ns_llama: %s needs head size 64 or 128 (or 96 with an fp16 KV cache), got %d", what, hd);
   return NS_E_UNSUPPORTED;
 }
 
@@ -996,7 +1008,7 @@ static int launch_decode(const AttnShape& s, const float* q, const float* k, con
   constexpr size_t smem = attn_decode_smem<HD>();
   if (int rc = grant_smem(attr, attn_decode_kernel<HD, RING, BATCH, KV>, smem)) return rc;
   // the eager pass before a capture runs this form where a streaming context's graph runs the ring form
-  if constexpr (!RING && !BATCH && KV == NS_KV_F16)
+  if constexpr (!RING && !BATCH && KV == NS_KV_F16 && attn_all_hd(HD))
     if (int rc = grant_smem(attr, attn_decode_kernel<HD, true>, smem)) return rc;
   using T = kv_elem_t<KV>;
   const dim3 grid((unsigned)(RING ? s.n_head_kv : s.n_head), (unsigned)s.nsplit, (unsigned)n_rows);
@@ -1060,6 +1072,10 @@ extern int launch_attention(int kind, float* q, const float* k, const float* v, 
     ns_set_error("ns_llama: the streaming ring shifts an fp16 KV cache only");
     return NS_E_UNSUPPORTED;
   }
+  if (ring && !attn_all_hd(hd)) {
+    ns_set_error("ns_llama: the streaming ring needs head size 64 or 128, got %d", hd);
+    return NS_E_UNSUPPORTED;
+  }
   if (ring && m == 1) kind = NS_ATTN_SPLIT_DECODE;  // the only kernel that carries the shift
   kind = attn_resolve(kind, hd, m, n_ctx, kv.type);
   if (kind < 0) return kind;
@@ -1069,16 +1085,16 @@ extern int launch_attention(int kind, float* q, const float* k, const float* v, 
     return launch_generic(s, q, kv, state, out, m, attr, st);
   }
   return attn_dispatch("attention kernel", hd, kv.type, [&](auto HD, auto KV) {  // attn_resolve left NS_ATTN_SPLIT_DECODE / MMA for Q8_0
-    constexpr bool f16 = KV == NS_KV_F16;
+    constexpr bool f16 = KV == NS_KV_F16, rows = f16 && attn_all_hd(HD);  // rows: the ring and attn_fast_kernel exist
     if (kind == NS_ATTN_SPLIT_DECODE) {
-      if constexpr (f16)
+      if constexpr (rows)
         if (ring) return launch_decode<HD, true, false, KV>(s, q, k, v, kv, state, nullptr, out, part, tickets, 1, ring->n_keep, ring->tab, attr, st);
       return launch_decode<HD, false, false, KV>(s, q, k, v, kv, state, nullptr, out, part, tickets, 1, -1, ShiftTable{}, attr, st);
     }
-    if constexpr (f16)
+    if constexpr (rows)
       if (kind == NS_ATTN_ROWS && m == 1) return launch_fast<HD, true>(s, q, k, v, kv, state, out, 1, attr, st);
     if (int rc = launch_rope_kv<false, KV>(s, q, k, v, kv, state, nullptr, m, st)) return rc;
-    if constexpr (f16)
+    if constexpr (rows)
       if (kind == NS_ATTN_ROWS) return launch_fast<HD, false>(s, q, k, v, kv, state, out, m, attr, st);
     return launch_mma<HD, false, KV>(s, q, kv, state, nullptr, out, m, (m + kAttnMmaRows - 1) / kAttnMmaRows, st);
   });
@@ -1208,8 +1224,8 @@ static int attention_batch_entry(const char* who, float* q, const float* k, cons
     return NS_E_INVALID;
   }
   if (int rc = check_rows(who, n_seq, n, seq, n_past, 1, n_ctx)) return rc;
-  if (hd != 64 && hd != 128) {
-    ns_set_error("%s: head size %d (the batched decode attention takes 64 or 128)", who, hd);
+  if (!attn_fast_hd(hd)) {
+    ns_set_error("%s: head size %d (the batched decode attention takes 64, 96 or 128)", who, hd);
     return NS_E_UNSUPPORTED;
   }
   cudaStream_t st = ns_stream_of(queue);
@@ -1351,8 +1367,8 @@ static int attention_ragged_entry(const char* who, float* q, const float* k, con
   }
   int n_rows = 0;
   if (int rc = check_segments(who, n_seq, n_ctx, n, seq, n_tokens, n_past, &n_rows)) return rc;
-  if (hd != 64 && hd != 128) {
-    ns_set_error("%s: head size %d (the ragged prompt attention takes 64 or 128)", who, hd);
+  if (!attn_fast_hd(hd)) {
+    ns_set_error("%s: head size %d (the ragged prompt attention takes 64, 96 or 128)", who, hd);
     return NS_E_UNSUPPORTED;
   }
   std::vector<int> order(n), first, rows, tiles;

@@ -13,11 +13,17 @@ constexpr int kMaxBatchRows = 4096;  // rows of one pass over segments; the call
 constexpr int kAttnMmaRows = 64, kAttnMmaKeys = 64;
 constexpr int kTileInts = 5;  // ints per entry of the ragged tile table
 
+// Head sizes of the split decode and tensor-core prompt attention with an fp16 KV cache: one-row steps, prompts, the batched decode
+// and the ragged prompt attention, so every pass over several KV blocks and beam search.
+constexpr bool attn_fast_hd(int hd) { return hd == 64 || hd == 96 || hd == 128; }
+// Head sizes where attn_fast_kernel (NS_ATTN_ROWS), the streaming ring and the Q8_0 KV cache exist as well
+constexpr bool attn_all_hd(int hd) { return hd == 64 || hd == 128; }
+
 struct AttnAttr {  // dynamic shared memory already granted to each kernel (function attributes are per device)
   struct Grant {
     const void* kern;
     size_t smem;
-  } granted[16];  // 15 attention kernels can ask for more than 48 KB
+  } granted[17];  // 17 attention kernels can ask for more than 48 KB
   int n = 0;
 };
 // {cos, sin} of the one-position back shift per rotary pair, fp16 (model_utils.cpp:165-192); passed by value
@@ -43,7 +49,8 @@ int launch_attention(int kind, float* q, const float* k, const float* v, const K
 
 // Batched decode attention: one new token for each of n sequences, one launch (attn_decode_kernel<HD, false, true>).  rstate:
 // [n][4] row states (n_past in slot 1), seqs [n] KV block per row, caches from the layer's block 0 on, q / out
-// [n][n_head * hd], k / v [n][n_head_kv * hd], part [n][n_head][ranges][hd + 2], tickets [n][n_head].  hd 64 / 128 only.
+// [n][n_head * hd], k / v [n][n_head_kv * hd], part [n][n_head][ranges][hd + 2], tickets [n][n_head].  hd 64 / 96 / 128
+// (attn_fast_hd), 96 with an fp16 cache only.
 int launch_attention_batch(const float* q, const float* k, const float* v, const KvPtrs& kv, const int* rstate,
                            const int* seqs, float* out, float* part, unsigned* tickets, int n, int n_head, int n_head_kv, int hd,
                            int n_ctx, float rope_theta, float rope_scale, AttnAttr& attr, cudaStream_t st);

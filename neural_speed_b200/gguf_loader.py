@@ -1,4 +1,4 @@
-"""GGUF (llama and qwen2 architectures) -> tensors for the device eval step (SURVEY §8 f.3, first slice).
+"""GGUF (llama, qwen2 and phi3 architectures) -> tensors for the device eval step (SURVEY §8 f.3, first slice).
 
 The reference reads GGUF in C++ (`models/model_utils/gguf.h`, `model_files.h:246-860`: header, key/value metadata, tensor
 infos, aligned data) and maps llama tensors to `model.others[0..2]` / `layers[il].norm/attn/ffn` (`models/llama/llama_utils.cpp`).
@@ -10,6 +10,11 @@ types the eval step consumes:
   attn_q/k/v.bias     F32 (qwen2 only: Qwen1.5 / Qwen2 / Qwen2.5 files, models/qwen/qwen_utils.cpp:130-143)
   attn_q/k/v/output, ffn_gate/down/up, output.weight   Q4_0 rows (18-byte blocks), Q8_0 rows (34-byte blocks) or Q6_K rows
                       (210-byte blocks), untouched
+  phi3 files          attn_qkv.weight: the fused q / k / v rows, split by rows into wq [0, E), wk [E, E + kvd), wv [E + kvd,
+                      E + 2 kvd) (separate attn_q / k / v are accepted too); ffn_up.weight: 2 n_ff rows, gate first (phi3.cpp:327-329),
+                      split into w1 (gate) and w3 (up).  Rows of every supported type are self-contained, so a split is a row
+                      slice.  LongRoPE files (rope_factors_long / _short, the 128k variants) and partial rotary
+                      (rope.dimension_count != head size) are refused.
 
 Host logic only (numpy); `parse()` is covered on CPU (tests/test_gguf_cpu.py).  `load_into_engine()` composes already-tested
 device entry points (Weight.from_q4_0_host / from_q6_K_host, Llama.set_*) but has not itself been run on a GPU in round 1.
@@ -53,7 +58,7 @@ class GGUFLlama:
     out_norm: np.ndarray                      # fp32 [n_embd]
     output: tuple                             # (type, rows uint8)
     layers: list = field(default_factory=list)  # dicts: attn_norm, ffn_norm (fp32) and wq, wk, wv, wo, w1, w2, w3 = (type, rows)
-    arch: str = "llama"                       # "qwen2": the layer dicts also hold bq, bk, bv (fp32)
+    arch: str = "llama"                       # "qwen2": the layer dicts also hold bq, bk, bv (fp32); or "phi3"
 
 
 _LAYER_TENSORS = {"attn_q": "wq", "attn_k": "wk", "attn_v": "wv", "attn_output": "wo", "ffn_gate": "w1", "ffn_down": "w2", "ffn_up": "w3"}
@@ -71,8 +76,8 @@ def parse(path: str) -> GGUFLlama:
     import gguf
     r = gguf.GGUFReader(path)
     arch = bytes(r.get_field("general.architecture").parts[-1]).decode()
-    if arch not in ("llama", "qwen2"):
-        raise ValueError(f"only the llama and qwen2 architectures are supported, file says {arch!r}")
+    if arch not in ("llama", "qwen2", "phi3"):
+        raise ValueError(f"only the llama, qwen2 and phi3 architectures are supported, file says {arch!r}")
     hp = dict(n_embd=int(_field(r, f"{arch}.embedding_length")), n_layer=int(_field(r, f"{arch}.block_count")),
               n_ff=int(_field(r, f"{arch}.feed_forward_length")), n_head=int(_field(r, f"{arch}.attention.head_count")),
               n_ctx=int(_field(r, f"{arch}.context_length", 2048)),
@@ -80,6 +85,13 @@ def parse(path: str) -> GGUFLlama:
               rope_theta=float(_field(r, f"{arch}.rope.freq_base", 10000.0)), rope_scale=1.0)
     hp["n_head_kv"] = int(_field(r, f"{arch}.attention.head_count_kv", hp["n_head"]))
     tensors = {t.name: t for t in r.tensors}
+    if arch == "phi3":
+        hd = hp["n_embd"] // hp["n_head"]
+        n_rot = int(_field(r, "phi3.rope.dimension_count", hd))
+        if n_rot != hd:
+            raise ValueError(f"phi3: rope.dimension_count {n_rot} != head size {hd} (partial rotary is not supported)")
+        if any(n.startswith(("rope_factors_long", "rope_factors_short")) for n in tensors):
+            raise ValueError("phi3: rope_factors_long / rope_factors_short tensors (LongRoPE, the 128k models) are not supported")
 
     def f32(name):
         t = tensors[name]
@@ -108,6 +120,12 @@ def parse(path: str) -> GGUFLlama:
             return ("q6_K", np.array(t.data, np.uint8).reshape(n, k // 256 * Q6_K_BLOCK))
         raise ValueError(f"{name}: weight type {t.tensor_type.name} not supported (Q4_0 / Q8_0 / Q6_K)")
 
+    def split(name, parts, k):
+        """the fused rows of `name` sliced into consecutive row ranges of parts[i] rows each"""
+        typ, rows = quant(name, sum(parts), k)
+        bounds = np.cumsum([0] + list(parts))
+        return [(typ, np.ascontiguousarray(rows[a:b])) for a, b in zip(bounds[:-1], bounds[1:])]
+
     tok = f32("token_embd.weight")
     hp["n_vocab"] = int(tok.shape[0])
     E, FF = hp["n_embd"], hp["n_ff"]
@@ -117,8 +135,14 @@ def parse(path: str) -> GGUFLlama:
     model = GGUFLlama(hp, tok, f32("output_norm.weight"), quant(out_name, hp["n_vocab"], E), arch=arch)
     for il in range(hp["n_layer"]):
         L = dict(attn_norm=f32(f"blk.{il}.attn_norm.weight"), ffn_norm=f32(f"blk.{il}.ffn_norm.weight"))
+        pre = f"blk.{il}."
+        if arch == "phi3" and pre + "attn_qkv.weight" in tensors:
+            L["wq"], L["wk"], L["wv"] = split(pre + "attn_qkv.weight", (E, kvd, kvd), E)
+        if arch == "phi3":
+            L["w1"], L["w3"] = split(pre + "ffn_up.weight", (FF, FF), E)
         for gname, ours in _LAYER_TENSORS.items():
-            L[ours] = quant(f"blk.{il}.{gname}.weight", *shapes[ours])
+            if ours not in L:
+                L[ours] = quant(f"{pre}{gname}.weight", *shapes[ours])
         if arch == "qwen2":
             for gname, ours, n in (("attn_q", "bq", E), ("attn_k", "bk", kvd), ("attn_v", "bv", kvd)):
                 b = f32(f"blk.{il}.{gname}.bias").reshape(-1)
